@@ -14,13 +14,18 @@ period 3600 s) + Poisson training (rate 1) per ingress, default_policy/energy_aw
 120 simulated seconds (~17 k events per replica).
 
 JSON keys beyond the base contract:
-  roofline        algorithmic HBM bytes (SURVEY.md §8d: 96 + 76*D per event) / event-loop kernel time vs measured HBM peak
-                  (frac), the same over the whole step (frac_step), and where the DRAM-traffic figure comes from
+  roofline        algorithmic HBM bytes (SURVEY.md §8d: 96 + 76*D per event) / event-loop kernel time vs the HBM peak
+                  (frac), the same over the whole step (frac_step)
   cpu_baseline    the oracle (C restatement of the reference loop) on the box's host cores, bounded sample
   e2e             same metric through the drop-in MultiIngressPaperSimulator(...).run() — host spec in, kernels,
                   summaries + CSV rows back in host memory — timed on the host clock; cold first run reported beside it
   configs         every BASELINE.json config at its per-GPU replica count (one device-timed batch each, after the headline)
   strong_scaling  (N > 1) the headline workload with 65 536 replicas in TOTAL, split over the N GPUs
+
+--dump-outputs DIR writes what the last timed step computed, as a caller of the engine receives it: summary.npy (the
+[replicas, 88] float64 summary rows of rank 0; a fixed, seeded sample of rows, listed in summary_rows.npy, when they
+exceed 64 MB) and aggregate.npy (the all-reduced 16-double aggregate).  Inputs depend only on the arguments; the summary
+rows are then bit-identical from run to run, the aggregate's float sums (atomic adds) up to their last bits.
 """
 import argparse
 import json
@@ -40,12 +45,14 @@ from distributed_cluster_gpus_b200 import scenarios as SC, sharding, spec as S  
 
 METRIC = "simulated events/sec, 4-DC x 64-sim-GPU, 65536 replicas per GPU"
 UNIT = "events/s"
-HBM_FALLBACK_GBS = 6650.0  # /opt/skills/guides/B200_PROFILING.md fallback
+HBM_FALLBACK_GBS = 3350.0  # NVIDIA H100 SXM data sheet (HBM3, 3.35 TB/s at up to 700 W)
+DUMP_BYTES = 64 << 20      # --dump-outputs budget
 KERNELS_PER_STEP = 4       # dcsim_arrivals_kernel, dcsim_merge_kernel, dcsim_advance_kernel, dcsim_reduce_kernel
 
 # BASELINE.json configs (SURVEY.md §8d table): (label, scenario, how the replica count scales, count, GPUs the config is quoted on)
-#   "per_gpu": `count` replicas on every GPU (cfg2/cfg3: 65 536 on one B200; cfg5: 1 048 576 / 8 = 131 072 per GPU)
-#   "total"  : `count` replicas in the whole job, split over the GPUs (cfg4: 32 768 seeds per variant on 4 B200)
+#   "per_gpu": `count` replicas on every GPU (cfg2/cfg3: 65 536 on one H100; cfg5: 524 288 / 8 = 65 536 per GPU, the
+#              most whose ~0.87 MB per replica of event lists, FIFOs and state blocks fit 80 GB)
+#   "total"  : `count` replicas in the whole job, split over the GPUs (cfg4: 32 768 seeds per variant on 4 H100)
 CONFIG_TABLE = [
     ("cfg2", "cfg2_1x64_poisson_600s", "per_gpu", 65536, 1),
     ("cfg3_600s", "cfg3_4x64_sinusoid_600s", "per_gpu", 16384, 1),
@@ -55,7 +62,7 @@ CONFIG_TABLE = [
     ("cfg4/carbon_cost", "sweep_carbon_cost", "total", 32768, 4),
     ("cfg4/eco_route", "sweep_eco_route", "total", 32768, 4),
     ("cfg4/debug_n2", "sweep_debug_n2", "total", 32768, 4),
-    ("cfg5", "cfg5_8x256_sinusoid_60s", "per_gpu", 131072, 8),
+    ("cfg5", "cfg5_8x256_sinusoid_60s", "per_gpu", 65536, 8),
 ]
 
 
@@ -72,7 +79,7 @@ def config_dict(sc, args, world, extra=None):
                        f"per ingress, algo {sc['algo']}/{sc['policy']}, {sc['duration']:.0f} simulated s",
            "scenario": sc["name"], "replicas_per_gpu": args.replicas, "replicas_total": args.replicas * world,
            "sim_duration_s": sc["duration"], "parallelism": f"replica-sharded x{world} (no data-path collective)",
-           "l2": "working set (event lists + FIFO rings + state blocks, tens of GB) is far larger than the 126 MB L2; no flush needed"}
+           "l2": "working set (event lists + FIFO rings + state blocks, tens of GB) is far larger than the 50 MB L2; no flush needed"}
     cfg.update(extra or {})
     return cfg
 
@@ -83,21 +90,11 @@ def hbm_peak():
         with open(path) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return HBM_FALLBACK_GBS, "fallback (B200_PROFILING.md)"
-
-
-def measured_traffic():
-    """DRAM bytes per event-loop launch from the committed ncu capture of this workload (a constant read from
-    profiles/roofline_traffic.json — it is NOT measured in this run; the file says which capture it came from)."""
-    try:
-        with open(os.path.join(ROOT, "profiles", "roofline_traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return None
+        return HBM_FALLBACK_GBS, "fallback (H100 SXM data sheet)"
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
     FIELDS = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
               "clocks_event_reasons.sw_power_cap")
@@ -185,41 +182,6 @@ def usable_cpus():
     return max(1, int(n)), info
 
 
-def _py_worker(args):
-    sc, seed = args
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import ref_harness
-    return ref_harness.time_reference_as_shipped(sc, seed)
-
-
-def python_reference_leg(sc, cores):
-    """The reference's own Python loop, unmodified, timed here — only where its tree exists (/root/reference in the
-    build container, or baseline/_ref/); the GPU box has neither and the leg is skipped there."""
-    sys.path.insert(0, os.path.join(ROOT, "oracle"))
-    import ref_harness
-    root = next((p for p in (ref_harness.REFERENCE_ROOT, os.path.join(ROOT, "baseline", "_ref"))
-                 if os.path.isdir(os.path.join(p, "simcore"))), None)
-    if root is None:
-        return None
-    os.environ["DCSIM_REFERENCE_ROOT"] = root
-    ref_harness.REFERENCE_ROOT = root
-    import multiprocessing as mp
-    import oracle_lib
-    procs = max(1, min(cores, 16))
-    seeds = [4000 + i for i in range(procs)]
-    blob = SC.to_spec(sc).to_bytes()
-    events = sum(oracle_lib.run_batch(blob, 1, s, 0, oracle_lib.RNG_MT19937, 1)[1] for s in seeds)   # the stock runs' event counts
-    t0 = time.perf_counter()
-    with mp.get_context("spawn").Pool(procs) as pool:
-        walls = pool.map(_py_worker, [(sc, s) for s in seeds])
-    wall = time.perf_counter() - t0
-    return {"kind": "python", "value": events / max(walls), "unit": UNIT, "processes": procs,
-            "events_per_s_per_core": events / sum(walls), "reference_root": root,
-            "sample": f"{procs} unmodified reference runs side by side (one process each, own Mersenne Twister, CSV logs on "
-                      f"tmpfs): {events} events, slowest run() {max(walls):.2f} s (interpreter start-up and imports, "
-                      f"{wall - max(walls):.1f} s here, not counted)"}
-
-
 def cpu_sample(sc, threads, target_s, cap_replicas, seed):
     oracle_rate(sc, threads, threads)                        # load + page in
     ev, dt = oracle_rate(sc, threads, threads)               # calibration: one replica per thread
@@ -238,9 +200,6 @@ def cpu_baseline(sc, target_s=12.0):
            "sample": f"{n} replicas of the same workload ({ev} events) in {dt:.1f} s on {threads} threads "
                      "(= min(affinity, cgroup quota)); oracle/dcsim_oracle.c = C restatement of the reference's Python "
                      "loop (the Python original measured 7-20 k events/s/core on this scenario, tests/golden/*.json ref_wall_s)"}
-    py = python_reference_leg(sc, threads)
-    if py:
-        out["python_reference"] = py
     return out
 
 
@@ -264,9 +223,6 @@ def run_reference_arm(args, world, rank):
               "(= min(affinity, cgroup quota)), oracle port of the reference loop")
     cpu = {"value": value, "unit": UNIT, "cores": threads, "kind": "port", "sample": sample,
            "single_thread_events_per_s": ev1 / dt1, "events_per_s_per_core": value / threads, "host": host}
-    py = python_reference_leg(sc, threads)
-    if py:
-        cpu["python_reference"] = py
     line = {"impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus, "steps": args.steps,
             "warmup": args.warmup, "ms_per_step": 1000.0 * total / max(args.steps, 1), "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f64", "data": "synthetic",
@@ -330,6 +286,21 @@ def side_config(torch, dist, BatchedEngine, stream, world, rank, local_rank, sce
             "algorithmic_bytes_per_event": 96 + 76 * sc["n_dc"], "sim_duration_s": sc["duration"]}
 
 
+def dump_outputs(out_dir, summary, aggregate):
+    """summary rows (a fixed, seeded sample of rows beyond DUMP_BYTES) and the aggregate, float64, as DIR/<name>.npy."""
+    os.makedirs(out_dir, exist_ok=True)
+    rows_path = os.path.join(out_dir, "summary_rows.npy")
+    if os.path.exists(rows_path):                      # a previous sampled dump's index must not describe this one
+        os.remove(rows_path)
+    if summary.nbytes + aggregate.nbytes > DUMP_BYTES:
+        keep = (DUMP_BYTES - aggregate.nbytes) // (summary.shape[1] * 8 + 8)      # + 8 bytes per row for its index
+        rows = np.sort(np.random.default_rng(0).choice(len(summary), keep, replace=False))
+        summary = summary[rows]
+        np.save(rows_path, rows.astype(np.float64))
+    np.save(os.path.join(out_dir, "summary.npy"), np.ascontiguousarray(summary, dtype=np.float64))
+    np.save(os.path.join(out_dir, "aggregate.npy"), np.asarray(aggregate, dtype=np.float64))
+
+
 def run_b200(args, world, rank, local_rank):
     import torch
     import torch.distributed as dist
@@ -387,6 +358,8 @@ def run_b200(args, world, rank, local_rank):
     t1.record(stream)
     barrier()
     clocks = sampler.stop()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, eng.summary(), agg[args.warmup + args.steps - 1].cpu().numpy())
     elapsed_ms = torch.tensor([t0.elapsed_time(t1)], dtype=torch.float64, device="cuda")
     kernel_ms = [a.elapsed_time(b) for a, b in zip(k0, k1)]
     prepass_ms = sum(a.elapsed_time(b) for a, b in zip(p0, k0)) / args.steps
@@ -405,10 +378,7 @@ def run_b200(args, world, rank, local_rank):
     achieved = local_events_per_launch * b_alg / (kms / 1000.0) / 1e9
     step_ms = 1000.0 * elapsed_s / args.steps
     peak, peak_src = hbm_peak()
-    traffic = measured_traffic()
     roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                "traffic": traffic["dram_bytes_per_launch"] if traffic else None,
-                "traffic_source": ({k: traffic.get(k) for k in ("source", "captured", "build", "note")} if traffic else None),
                 "kernel": "dcsim_advance_kernel", "kernel_ms": kms, "arrivals_prepass_kernel_ms": prepass_ms,
                 "events_per_launch": local_events_per_launch,
                 "achieved_step": local_events_per_launch * b_alg / (step_ms / 1000.0) / 1e9,
@@ -416,7 +386,7 @@ def run_b200(args, world, rank, local_rank):
                 "algorithmic_bytes_per_event": b_alg, "peak_source": peak_src,
                 "note": "frac = algorithmic bytes / event-loop kernel time; frac_step = the same over the whole step (the 400 B "
                         "per event include the arrival / RNG work the pre-pass kernels do).  The path is warp-serial-latency "
-                        "bound, not HBM bound (SURVEY.md §8d): see DESIGN.md §4 for the issue-slot bound and profiles/ for ncu evidence",
+                        "bound, not HBM bound (SURVEY.md §8d): see DESIGN.md §4 for the issue-slot bound",
                 "events_per_s_per_resident_warp": local_events_per_launch / (kms / 1000.0) / max(1, info["resident_warps_per_sm"] * info["sm_count"])}
 
     if args.no_e2e:                                                            # tuning runs
@@ -528,7 +498,11 @@ def main():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true", help="tuning runs only: skip the end-to-end leg")
     ap.add_argument("--no-configs", action="store_true", help="skip the side records (other BASELINE configs, strong scaling)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's summary rows and aggregate as DIR/<name>.npy (float64, <= 64 MB)")
     args = ap.parse_args()
+    if args.steps < 1 or args.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))

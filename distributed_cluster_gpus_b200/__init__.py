@@ -1,4 +1,4 @@
-"""distributed_cluster_gpus_b200 — B200-native batched discrete-event engine.
+"""distributed_cluster_gpus_b200 — H100-native (sm_90a) batched discrete-event engine.
 
 Drop-in for ONE path of filrg/distributed_cluster_GPUs: the multi-DC event loop of
 simcore/simulator_paper_multi.py, run as tens of thousands of independent Monte-Carlo replicas per GPU.

@@ -44,7 +44,7 @@ def load():
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryMissing(
             f"{LIB_PATH} not found. Build it with `python -c 'import __graft_entry__ as g; g.build()'` "
-            "(nvcc, sm_100a). The batched engine has no CPU fallback.")
+            "(nvcc, sm_90a). The batched engine has no CPU fallback.")
     L = C.CDLL(LIB_PATH)
     vp, u64, u32, i32 = C.c_void_p, C.c_uint64, C.c_uint32, C.c_int
     L.dcsim_sizeof_spec.restype = C.c_size_t

@@ -18,19 +18,17 @@
 #define DCSIM_REPLICAS_PER_WARP (32 / DCSIM_LANES)
 #ifndef DCSIM_MIN_CTAS_PER_SM
 /* 32 lanes per replica: 8 CTAs x 4 warps = 32 warps/SM -> ptxas keeps the kernel within 64 registers.  With several
- * replicas per warp shared memory allows fewer warps anyway, so the register budget per thread is wider: 8 lanes run
- * best at 5 CTAs (96 registers, 80 replicas per SM) — 4 CTAs / 118 registers measured -13 %, 6 CTAs / 80 registers
- * (spills) -12 % (profiles/r02_ab_lane_group_occupancy.jsonl). */
+ * replicas per warp shared memory allows fewer warps anyway, so the register budget per thread is wider: 8 lanes at
+ * 5 CTAs (96 registers, 80 replicas per SM) — 4 CTAs leave too few replicas resident, 6 CTAs (80 registers) spill. */
 #define DCSIM_MIN_CTAS_PER_SM (DCSIM_LANES == 32 ? 8 : (DCSIM_LANES == 16 ? 6 : 5))
 #endif
 
 extern __shared__ __align__(16) char dcsim_smem[];
 
 /* CAP = the power-cap controller (algo = cap_greedy with power_cap > 0: SIM:207-338) is compiled in.  It is a
- * separate instantiation because merely inlining that cold code costs the common path 17 % (measured,
- * profiles/r01_variants_ab.md). */
+ * separate instantiation because merely inlining that cold code slows the common path (registers, code size). */
 /* MODE = where the replica's state block lives during the launch (a compile-time switch: a run-time select would turn
- * every state access into a generic load/store, measured -15 %):
+ * every state access into a generic load/store):
  *   DCSIM_MODE_STAGED  the whole block is staged in shared memory (small blocks: 4 DC x 64 is ~5 kB, 32 warps/SM);
  *   DCSIM_MODE_HEAD    only the head [0, L.rec_off) — header, event set, per-DC arrays, list window, seq ring —
  *                      is staged; the running-job records stay at the block's home in HBM/L2 and are touched once per

@@ -1,5 +1,5 @@
 /*
- * dcsim_b200.cu — sm_100a kernels and the C-ABI of include/dcsim_b200.h.
+ * dcsim_b200.cu — sm_90a kernels and the C-ABI of include/dcsim_b200.h.
  *
  * Kernels
  *   dcsim_arrivals_kernel     one thread per replica: the replica's arrival sequence (instants, routed DCs, size deviates).
@@ -11,7 +11,7 @@
  *   dcsim_reduce_kernel       [n_replicas][K] summaries -> DCSIM_AGG_K doubles (the only cross-GPU payload).
  *   dcsim_hist_reduce_kernel  per-replica job-latency histograms -> one [2][128] histogram (opt-in).
  *
- * Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false (see __graft_entry__.build()).
+ * Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see __graft_entry__.build()).
  * -fmad=false matters: the reference is CPython float arithmetic, one rounding per operation.
  */
 #include <cuda_runtime.h>
@@ -38,9 +38,11 @@ int dcsim_adv_min_ctas_g8(void);
  * otherwise run on one lane.  Per-thread scratch in shared memory, [slot][thread]: 2*MAX_ING stream clocks (f64),
  * 2*MAX_ING "latest arrival of the stream" indices (u32), DCSIM_TRNG_RING staged random words (u32). */
 #define DCSIM_ARRIVALS_THREADS 128
-/* 7 resident CTAs per SM (<= 73 registers, <= 32 kB of scratch each): 148 x 7 x 128 = 132 608 threads, so that a batch of
- * 131 072 replicas (BASELINE config 5 per GPU) is still ONE wave of this latency-bound kernel. */
-#define DCSIM_ARRIVALS_MIN_CTAS 7
+/* 5 resident CTAs per SM: 132 x 5 x 128 = 84 480 threads on an H100, so the largest per-GPU batch of the BASELINE configs
+ * (65 536 replicas) is ONE wave of this latency-bound kernel, and the register cap it implies (78 registers for the
+ * Philox path, 96 for MT19937 on sm_90a) leaves both paths without spills.  A tighter bound (7: 72 registers) spills
+ * and bought nothing measurable on the H100: the kernel's time was the same at 7, 5 and 4. */
+#define DCSIM_ARRIVALS_MIN_CTAS 5
 static size_t dcsim_arrivals_scratch_bytes(int n_ing) { /* per CTA: [slot][thread] arrays for 2 * n_ing streams */
   return (size_t)DCSIM_ARRIVALS_THREADS * ((size_t)(2 * n_ing) * (sizeof(double) + sizeof(uint32_t)) + DCSIM_TRNG_RING * sizeof(uint32_t));
 }
@@ -234,14 +236,13 @@ static cudaError_t size_launch(dcsim_t* h) {
   if ((e = cudaDeviceGetAttribute(&smem_sm, cudaDevAttrMaxSharedMemoryPerMultiprocessor, h->device)) != cudaSuccess) return e;
   /* Lanes per replica.  Four replicas per warp share everything warp-wide in an event (pop-min, DC sweep, the lane-0
    * handler's issue slots) and pay whenever the event set fits one round of 8 lanes: up to 5 DCs (n_dc finish slots +
-   * list + log + stale).  Measured with the event-level pop-min (profiles/r02_ab_s17_*): 4 DC x 64 +35 % over the
-   * 32-lane build, debug n=2 +34 %, joint_nf / carbon_cost (up to 64 running jobs per DC: a job_finish walks them 8
-   * at a time) +2..3 %; 8 DC x 256 (two slots per lane, all 8 lanes in the sweep) -10 %: it keeps the whole warp. */
+   * list + log + stale).  Above that (8 DC x 256: two slots per lane, all 8 lanes in the sweep) it keeps the whole
+   * warp. */
   int lanes = h->spec.n_dc <= 5 ? 8 : 32;
   if (lanes == 8) {
     /* ... unless four blocks per warp leave the SM with hardly more resident REPLICAS than one per warp would (very
-     * large heads: the power-cap controller's pools — cap_greedy 4 x 64: 12 vs 14 replicas per SM, and the 32-lane
-     * build is 1.6x faster there, profiles/r02_ab_s19_*; the bandit's tables: 52 vs 32, 8 lanes 18 % faster) */
+     * large heads: the power-cap controller's pools — cap_greedy 4 x 64: 12 vs 14 replicas per SM; the bandit's
+     * tables, 52 vs 32, stay on 8 lanes) */
     int w8 = 0, w32 = 0, unused = 0;
     const int bytes8 = 4 * h->L.rec_off, bytes32 = h->L.rec_off; /* head-staged: the smallest footprint of each */
     w8 = resident_warps_for(bytes8, smem_optin, smem_sm, min_ctas_for(8) * DCSIM_MAX_WARPS_PER_CTA, &unused);

@@ -1,5 +1,5 @@
 /*
- * dcsim_core.cuh — the device code of the B200 batched simulator (all kernels' bodies).
+ * dcsim_core.cuh — the device code of the H100 batched simulator (all kernels' bodies).
  *
  * The reference's multi-DC event loop (simcore/simulator_paper_multi.py:412-480 and the leaves it calls; citations
  * are relative to the reference tree) is split where its data dependencies split it:
@@ -35,7 +35,7 @@
  * counts rather than bit-for-bit.
  *
  * The file compiles two ways:
- *   - nvcc, sm_100a: DCSIM_LANES = 32, warp collectives are real (csrc/dcsim_b200.cu);
+ *   - nvcc, sm_90a: DCSIM_LANES = 32, warp collectives are real (csrc/dcsim_b200.cu);
  *   - g++ with -DDCSIM_HOST_EMU (tests/hostemu/, TEST-ONLY): DCSIM_LANES = 1, collectives are identities.
  *     It exists so the handler logic can be checked against the oracle where there is no GPU; it is not
  *     linked into, or reachable from, the product library.
@@ -217,8 +217,8 @@ DCSIM_DEV int dcsim_lat_bin(double lat) {
 /* Cold helpers are kept OUT OF LINE in the one-replica-per-warp build (by-value arguments only, so the context stays in
  * registers): inlining them costs the event loop registers and instruction-cache footprint on paths most launches never
  * take.  When a warp carries several replicas they are INLINED instead: a call made by one lane group while its
- * siblings are elsewhere in the loop is ruinous (the job-latency histogram's one-instruction helper measured +130 % on
- * the whole event loop as a call, < 1 % inlined: tools/hist_probe.py), and that build has registers to spare. */
+ * siblings are elsewhere in the loop is ruinous (tools/hist_probe.py times the job-latency histogram's one-instruction
+ * helper both ways), and that build has registers to spare. */
 #if defined(DCSIM_HOST_EMU)
 #define DCSIM_COLD static
 #elif DCSIM_LANES == 32
@@ -585,15 +585,14 @@ DCSIM_DEV double dcsim_mod_pos(double x, double y) {
 /* Thread-level Philox stream with a 32-word ring (element i at ring[i * stride]: [word][thread] in shared memory on
  * the GPU; the pointer is passed alongside the stream, not inside it, so that the accesses compile to LDS/STS).  The
  * ring is topped up ONCE per arrival, by all lanes of the warp at the same program point; refilling inside the
- * samplers instead makes 32 out-of-phase lanes drag the warp through the block function at almost every draw
- * (measured: 43 % of the pre-pass). */
+ * samplers instead makes 32 out-of-phase lanes drag the warp through the block function at almost every draw. */
 #define DCSIM_TRNG_RING 32u
 /* Word source = CPython's own Mersenne Twister instead of Philox (dcsim_set_rng(h, DCSIM_RNG_MT19937)): the replica
  * then IS the stock reference at random.seed(seed0 + r) (SIM:71).  State: 624 words in HBM, element i at
  * mt[i * mt_stride] ([word][replica], coalesced across the warp's replicas). */
 struct dcsim_mt_t { uint32_t* mt; uint64_t mt_stride; uint32_t mti; };
 /* The stream is a template over the word source so that the Philox instantiation carries no trace of the other one
- * (a run-time switch cost the pre-pass 3 %: different register allocation, more local-memory traffic). */
+ * (a run-time switch changes the register allocation and adds local-memory traffic). */
 template <bool MT> struct dcsim_trng_t { uint32_t k0, k1, pos, filled; };
 template <> struct dcsim_trng_t<true> { uint32_t k0, k1, pos, filled; dcsim_mt_t mt; };
 
@@ -656,8 +655,8 @@ DCSIM_DEV void dcsim_trng_block(dcsim_trng_t<MT>& g, uint32_t* ring, int stride)
 }
 template <bool MT>
 DCSIM_DEV void dcsim_trng_topup(dcsim_trng_t<MT>& g, uint32_t* ring, int stride) {
-  /* one block at a time: generating two with interleaved rounds (more ILP for a latency-bound kernel) measured 4 %
-     SLOWER — the longer live ranges cost more than the overlap gains (profiles/r02_variants_ab.md) */
+  /* one block at a time: generating two with interleaved rounds (more ILP for a latency-bound kernel) was SLOWER —
+     the longer live ranges cost more than the overlap gains */
   while (g.filled - g.pos <= DCSIM_TRNG_RING - 4u) dcsim_trng_block(g, ring, stride);
 }
 /* A sampler out-ran the ring (a long rejection run): one more block, out of line.  The Philox flavour takes the
@@ -741,7 +740,7 @@ DCSIM_DEV double dcsim_sin_phase_approx(double t, double inv_period, double two_
  * for the lane with the longest rejection run.  The accepted candidate's gap -log(1-U1)/max_rate is left to
  * dcsim_t_gap_finish(), which the arrival loop calls behind a warp-wide reconvergence point: written after the loop
  * in the same function, the compiler duplicated the log() into every loop exit and the lanes ran it one exit at a
- * time (ncu: 18 % of the kernel's instructions at a third of the lanes). */
+ * time. */
 /* What the draws of one inter-arrival gap leave to be done: gap = is_w ? v : -log(v) / rate. */
 struct dcsim_gap_draw_t { double v, rate; bool is_w; };
 template <bool MT>
@@ -1188,10 +1187,10 @@ DCSIM_DEV uint32_t* dcsim_list_seq_slot(dcsim_ctx_t& c, uint32_t m) {
  * job_finish, a start that becomes its DC's earliest finish, a log tick, the cap controller), whoever writes one raises
  * cand_dirty, and the reduction only runs when some replica of the warp is dirty (a clean one next to it recomputes what
  * it had).  In a saturated cluster most events are arrivals and transfers that queue: the 4 DC x 64 bench batch
- * re-reduces on a few percent of its events (event loop 126.8 -> 119.3 ms); a lightly loaded single DC is dirty on most
- * and pays for the bookkeeping (268 -> 279 ms) — profiles/r02_ab_s21_*.  What else was tried for (1), all slower: one
- * butterfly over the whole tuple (fewer dependent round trips, more instructions), every lane scanning the slots itself
- * (no shuffles at all: +20 %), probing chunks that switch the cache off when it misses (the switch costs what it saves).
+ * re-reduces on a few percent of its events; a lightly loaded single DC is dirty on most and pays for the bookkeeping.
+ * What else was tried for (1), all slower: one butterfly over the whole tuple (fewer dependent round trips, more
+ * instructions), every lane scanning the slots itself (no shuffles at all), probing chunks that switch the cache off
+ * when it misses (the switch costs what it saves).
  * With a warp per replica three REDUX.MIN are cheaper than the bookkeeping: no cache.
  *
  * The list's slot of the event set is never written: it stays +inf and takes part in (1) harmlessly.
@@ -1672,7 +1671,7 @@ DCSIM_DEV void dcsim_handle_finish(dcsim_ctx_t& c, int d) {
   double psum = 0.0;
   dcsim_warp_sync(); /* lane 0's reads of record k are done before anybody overwrites slot k */
   /* (issuing the pass's loads BEFORE lane 0's accounting, so that the two L2 round trips overlap, measured slower:
-     the loop then carries lane 0's code with every record field live — profiles/r02_variants_ab.md) */
+     the loop then carries lane 0's code with every record field live) */
   for (int base = 0; base < n1; base += DCSIM_LANES) {
     const int j = base + c.lane;
     const bool act = j < n1, moved = act && j >= k;
@@ -1991,7 +1990,7 @@ DCSIM_DEV void dcsim_replica_tail(dcsim_ctx_t& c) {
  *
  * Only the pop-min and these two syncs are event-level.  Making the HANDLERS event-level too (every replica of the
  * warp walks through job_finish, or through the list ring's refill, as soon as one of them has to — so that their
- * collectives also get the full mask) measured 10 % SLOWER (profiles/r02_ab_s16_*): handlers of different replicas
+ * collectives also get the full mask) was SLOWER: handlers of different replicas
  * are divergent paths of one warp, the scheduler interleaves them, and one replica's L2 round trip hides behind
  * another's arithmetic; a warp-wide sync inside a handler takes that away. */
 template <bool CAP, bool RECG>

@@ -144,7 +144,7 @@ class BatchedEngine:
         N.check(self._lib.dcsim_reduce_summary(self._h, C.c_void_p(device_ptr)), self._h)
 
     def enable_latency_histogram(self):
-        """Opt-in, before the first advance of a batch: job-latency histogram of the whole batch (~1 % of kernel time)."""
+        """Opt-in, before the first advance of a batch: job-latency histogram of the whole batch."""
         N.check(self._lib.dcsim_enable_latency_histogram(self._h), self._h)
 
     def latency_histogram(self) -> np.ndarray:
@@ -207,7 +207,7 @@ _COPY_POOL = None
 
 def _copy_rows(src: np.ndarray) -> np.ndarray:
     """A private copy of a large row-major array, row blocks on a few threads (numpy's copy loops release the GIL):
-    the 46 MB of summaries of a 65 536-replica batch take 9 ms on one thread, a third of that on four."""
+    a single-threaded copy of the 46 MB of summaries of a 65 536-replica batch is memory-latency bound."""
     global _COPY_POOL
     n = src.shape[0]
     if src.nbytes < (8 << 20):
@@ -264,8 +264,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
 
 def release_engine(eng, sp, device=0, cuda_stream=0):
     """Parks a finished engine for reuse (see acquire_engine); a previously parked batch engine is destroyed.  The
-    parked companion of LoggedReplica is a separate slot and is left alone (closing and re-creating it was 16 ms of
-    every run())."""
+    parked companion of LoggedReplica is a separate slot and is left alone (closing and re-creating it would cost
+    every run() its allocations)."""
     _drop_parked_batch_engine()
     _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream)
 
@@ -282,7 +282,7 @@ class LoggedReplica:
     that runs the same trajectory (same spec, same key) on its own stream WHILE the batch runs.
 
     Switching the recorders on inside the batch makes every replica carry the job log's fields in its running-job
-    records (60 instead of 40 bytes; fewer resident warps: +9 % on the 65 536-replica bench batch); a single warp
+    records (60 instead of 40 bytes: fewer resident warps); a single warp
     next to the batch's grid costs nothing — it is launched first, is resident before the grid fills the GPU, and
     finishes long before it.  Results are identical by construction (one replica = one deterministic trajectory)."""
 

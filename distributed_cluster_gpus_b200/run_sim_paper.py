@@ -21,7 +21,7 @@ ALGOS = ["default_policy", "cap_uniform", "cap_greedy", "joint_nf", "bandit", "c
 
 
 def parse_args(argv=None):
-    p = argparse.ArgumentParser(description="Geo GPU simulator (paper-style, multi-ingress) — B200 batched engine",
+    p = argparse.ArgumentParser(description="Geo GPU simulator (paper-style, multi-ingress) — H100 batched engine",
                                 formatter_class=argparse.ArgumentDefaultsHelpFormatter)
     p.add_argument("--duration", type=float, default=180.0, help="simulated seconds")
     p.add_argument("--policy", type=str, default="energy_aware", choices=["energy_aware", "perf_first"])

@@ -2,7 +2,7 @@
 
 Same constructor arguments, same ``run()``, same result carriers — the ``DataCenter`` objects are mutated in
 place and ``cluster_log.csv`` / ``job_log.csv`` are written with the reference's columns and number formats —
-but ``run()`` executes ``replicas`` independent trajectories on a B200 through the C-ABI of
+but ``run()`` executes ``replicas`` independent trajectories on an H100 through the C-ABI of
 include/dcsim_b200.h.  Replica ``r`` is the trajectory the reference would produce for ``rng_seed + r`` when its
 ``random`` module is backed by the Philox stream of oracle/philox_random.py.  Replica 0 fills the DataCenters and
 the CSVs; all replicas are available as ``self.summary`` ([replicas, spec.SUMMARY_K]).

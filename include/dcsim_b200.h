@@ -1,5 +1,5 @@
 /*
- * dcsim_b200.h — C-ABI of the B200-native batched discrete-event engine.
+ * dcsim_b200.h — C-ABI of the H100-native batched discrete-event engine.
  *
  * The reference (filrg/distributed_cluster_GPUs) has no FFI: its seam is the Python constructor
  * MultiIngressPaperSimulator(...) (simcore/simulator_paper_multi.py:31-55) followed by .run()

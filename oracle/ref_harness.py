@@ -1,4 +1,4 @@
-"""TEST INFRASTRUCTURE — not product code.  Runs ONLY where /root/reference is mounted.
+"""TEST INFRASTRUCTURE — not product code.  Runs ONLY where a reference checkout is named by $DCSIM_REFERENCE_ROOT.
 
 Drives the *unmodified* reference simulator (simcore/simulator_paper_multi.py) programmatically on
 the synthetic scenarios of SURVEY.md §8(d) and captures in-memory results (the CSVs round:
@@ -21,7 +21,7 @@ import sys
 import tempfile
 import time
 
-REFERENCE_ROOT = os.environ.get("DCSIM_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("DCSIM_REFERENCE_ROOT", "")
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 if _HERE not in sys.path:
@@ -46,8 +46,8 @@ def scenario(name, n_dc, gpus_per_dc, inf, trn, duration, freq_levels=None, algo
 
 def _import_reference():
     if not os.path.isdir(REFERENCE_ROOT):
-        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT}; goldens can only be regenerated "
-                           "in the build container")
+        raise RuntimeError(f"reference tree not found at {REFERENCE_ROOT!r}; set DCSIM_REFERENCE_ROOT to a checkout of "
+                           "the reference to regenerate the goldens")
     if REFERENCE_ROOT not in sys.path:
         sys.path.insert(0, REFERENCE_ROOT)
     from simcore.simulator_paper_multi import MultiIngressPaperSimulator
@@ -201,23 +201,3 @@ def run_reference(sc, seed, rng="philox", trace_events=0, log_dir=None):
     if trace_events:
         out["trace"] = st["trace"]
     return out
-
-
-def time_reference_as_shipped(sc, seed):
-    """Wall seconds of ONE reference run exactly as shipped — its own Mersenne Twister (SIM:71), CSV logging to a
-    tmpfs directory, no progress bar, nothing wrapped or re-bound.  The number of events that run processes is the
-    oracle's for the same seed in MT19937 mode (the oracle reproduces the stock run event for event), so the caller
-    divides.  Used by bench.py's optional `kind: "python"` leg, only where the reference tree is present."""
-    Sim, _, _, _ = _import_reference()
-    inputs = build_reference_inputs(sc)
-    logger = logging.getLogger("dcsim-ref-harness")
-    logger.addHandler(logging.NullHandler())
-    logger.propagate = False
-    logger.setLevel(logging.CRITICAL)
-    with tempfile.TemporaryDirectory(prefix="dcsim_ref_", dir="/dev/shm" if os.path.isdir("/dev/shm") else None) as log_dir:
-        sim = Sim(logger=logger, sim_duration=sc["duration"], log_interval=sc["log_interval"], log_path=log_dir,
-                  rng_seed=seed, algo=sc["algo"], power_cap=sc["power_cap"], show_progress=False,
-                  num_fixed_gpus=sc["num_fixed_gpus"], fixed_freq=sc["fixed_freq"], **inputs)
-        t0 = time.perf_counter()
-        sim.run()
-        return time.perf_counter() - t0

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Per-opcode breakdown of the executed warp-instructions of a profiled kernel (ncu --set full --import-source on).
 
-    python profiles/opcode_histogram.py gpurun_out/r1_prof_v8_advance.ncu-rep <events_in_the_profiled_launch>
+    python profiles/opcode_histogram.py advance.ncu-rep <events_in_the_profiled_launch>
 """
 import collections
 import csv

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Summarises an `ncu --set full --import-source on` report of dcsim_advance_kernel into a small markdown file.
 
-    python profiles/summarize_ncu.py gpurun_out/r1_prof_v2.ncu-rep <events_in_the_profiled_launch> > profiles/r01_ncu_v2.md
+    python profiles/summarize_ncu.py advance.ncu-rep <events_in_the_profiled_launch> > advance_ncu.md
 """
 import collections
 import csv

@@ -1,5 +1,5 @@
-"""Regenerates tests/golden/*.json by running the UNMODIFIED reference (only possible where /root/reference
-is mounted, i.e. in the build container).  Usage:  python tests/golden/make_golden.py [name-substring ...]
+"""Regenerates tests/golden/*.json by running the UNMODIFIED reference (only possible where
+$DCSIM_REFERENCE_ROOT names a reference checkout).  Usage:  python tests/golden/make_golden.py [name-substring ...]
 
 For every scenario of distributed_cluster_gpus_b200.scenarios.GOLDEN_SCENARIOS:
   * rng = "mt"     seed 123                 — the reference exactly as shipped (global Mersenne Twister);

@@ -1,6 +1,6 @@
-"""Golden files written by the reference's OWN command line, untouched: `python /root/reference/run_sim_paper.py
+"""Golden files written by the reference's OWN command line, untouched: `python $DCSIM_REFERENCE_ROOT/run_sim_paper.py
 <flags>` (its process-global Mersenne Twister, its default 8-DC scenario).  The product's CLI with the same flags
-plus `--rng mt19937` must write the same files.  Build-container only.   python tests/golden/make_golden_cli.py"""
+plus `--rng mt19937` must write the same files.  Needs a reference checkout.   python tests/golden/make_golden_cli.py"""
 import json
 import os
 import shutil
@@ -9,7 +9,7 @@ import sys
 import tempfile
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-REFERENCE_ROOT = os.environ.get("DCSIM_REFERENCE_ROOT", "/root/reference")
+REFERENCE_ROOT = os.environ.get("DCSIM_REFERENCE_ROOT", "")
 
 CASES = {
     "defaults_12s_seed7": ["--duration", "12", "--seed", "7"],
@@ -20,6 +20,9 @@ CASES = {
 }
 
 if __name__ == "__main__":
+    if not os.path.isfile(os.path.join(REFERENCE_ROOT, "run_sim_paper.py")):
+        raise SystemExit(f"reference tree not found at {REFERENCE_ROOT!r}; set DCSIM_REFERENCE_ROOT to a checkout of the "
+                         "reference to regenerate the CLI goldens")
     out = os.path.join(HERE, "cli")
     os.makedirs(out, exist_ok=True)
     for name, flags in CASES.items():

@@ -1,7 +1,7 @@
 """Regenerates tests/golden/fuzz_reference.json: RANDOM scenarios (generator of tools/fuzz_core.py, fixed seed) run
 through the UNMODIFIED reference — once with the Philox stream injected (oracle/ref_harness.py) and once exactly as
 shipped, on its own Mersenne Twister ("run_mt") — only possible where
-/root/reference is mounted.  The fixture pins the oracle (tests/test_oracle_vs_reference.py) and, through it, the
+$DCSIM_REFERENCE_ROOT names a reference checkout.  The fixture pins the oracle (tests/test_oracle_vs_reference.py) and, through it, the
 device path on parameter combinations nobody picked by hand.  Usage: python tests/golden/make_golden_fuzz.py [cases]
 """
 import json

@@ -259,9 +259,9 @@ def test_conditioning_probe_separates_chaotic_scenarios(oracle, hostemu):
 
 def test_round2_gpu_fuzz_flags_are_conditioning_not_logic(hostemu, oracle):
     """The two scenarios (of 7000) on which the final GPU build's event counts differ from the oracle's — both cap_greedy,
-    one replica of seven each (profiles/r02_fuzz_gpu_6000cases_f3.json): the host build of the same device source agrees
+    one replica of seven each (tests/golden/ill_conditioned_cap_greedy_cases_r2.json): the host build of the same device source agrees
     with the oracle on every count and every float, so the handler logic is the oracle's; every GPU build, round 1's
-    included, returns the same deviating answer (profiles/r02_fuzz_recheck_f3.jsonl) — libdevice vs glibc in the last
+    included, returned the same deviating answer (tools/fuzz_recheck.py) — libdevice vs glibc in the last
     bit, amplified by the controller's threshold decisions."""
     import json
     from conftest import GOLDEN_DIR

@@ -1,4 +1,4 @@
-"""Parity tests proper: the sm_100a kernel through the C-ABI against the oracle and the reference fixtures.
+"""Parity tests proper: the sm_90a kernel through the C-ABI against the oracle and the reference fixtures.
 
 Bar (BASELINE.json north_star): exact event / job / RNG-word counts; per-replica total energy and mean job
 latency within 1e-9 relative.  Every float of the summary is held to the same 1e-9.

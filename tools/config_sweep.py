@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Throughput of every BASELINE.json config on one GPU at its per-GPU replica count (not bench lines: context).
 
-    python tools/config_sweep.py > profiles/r01_config_sweep.json
+    python tools/config_sweep.py > config_sweep.json
 """
 import json
 import os

@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """Full-batch parity: EVERY replica of the bench workload (default 65 536 x cfg3, 120 s) from the CUDA kernel
-against the oracle run on all host cores.  Prints one JSON line; used to produce profiles/r01_full_parity.json.
+against the oracle run on all host cores.  Prints one JSON line.
 
     python tools/full_parity.py [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
 """

@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Differential fuzz on the GPU: the sm_100a kernels through the C-ABI against the C oracle on random scenarios
+"""Differential fuzz on the GPU: the sm_90a kernels through the C-ABI against the C oracle on random scenarios
 (the generator of tools/fuzz_core.py).  Counts must be exact, every float within 1e-9 relative (the parity bar);
 capacity overflows go through engine.run_to_completion's retry like in production.
 
-    python tools/fuzz_gpu.py --cases 300 --seed 7 > gpurun_out/fuzz_gpu.json
+    python tools/fuzz_gpu.py --cases 300 --seed 7 > fuzz_gpu.json
 """
 import argparse
 import json

@@ -2,7 +2,7 @@
 """Re-runs the cases a GPU fuzz flagged under several builds / launch shapes: is a mismatch a property of the SCENARIO
 (every build disagrees with the oracle on it, each in its own way: ill-conditioned) or of one build?
 
-    python tools/fuzz_recheck.py profiles/r02_fuzz_gpu_6000cases_f3_failed_cases.json label[:lib=path][:ENV=val] ...
+    python tools/fuzz_recheck.py failed_cases.json label[:lib=path][:ENV=val] ...
 """
 import json
 import os

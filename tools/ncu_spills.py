@@ -2,7 +2,7 @@
 """Where the local-memory traffic (register spills) of a kernel is: LDL/STL instructions of an ncu report with their
 executed counts, the source line each belongs to, and the hot SASS neighbourhood.
 
-    python tools/ncu_spills.py gpurun_out/x.ncu-rep <events>
+    python tools/ncu_spills.py x.ncu-rep <events>
 """
 import csv
 import io

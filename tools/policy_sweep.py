@@ -4,7 +4,7 @@ variant on the device path, N seeds each — with the cross-replica statistics a
 give (mean, 95 % CI, quantiles of total energy and mean job latency).  Under torchrun the seeds of every variant are
 sharded over the ranks and the 16-double aggregates are all-reduced.
 
-    python tools/policy_sweep.py --seeds 32768 > profiles/r01_policy_sweep.json
+    python tools/policy_sweep.py --seeds 32768 > policy_sweep.json
 """
 import argparse
 import json

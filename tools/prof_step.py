@@ -2,7 +2,7 @@
 """One scenario, a few batches: the command ncu wraps for launch lists and `--set full` captures.
 
     python tools/prof_step.py cfg3_4x64_sinusoid_120s 65536 [batches]
-Prints events per batch (the denominator of the per-event figures in profiles/)."""
+Prints events per batch (the denominator of per-event profiler figures)."""
 import json
 import os
 import sys
