@@ -21,6 +21,8 @@ EXPORTS = (
     "dcsim_summary_device_ptr", "dcsim_reduce_summary", "dcsim_enable_latency_histogram", "dcsim_fetch_latency_histogram", "dcsim_fetch_trace", "dcsim_fetch_job_log",
     "dcsim_fetch_cluster_log", "dcsim_launch_info", "dcsim_last_error", "dcsim_destroy", "dcsim_set_rng",
     "dcsim_recorder_counts", "dcsim_allreduce_summary", "dcsim_fetch_summary_host",
+    "dcsim_enable_cluster_ensemble", "dcsim_cluster_ensemble_capacity", "dcsim_fetch_cluster_ensemble",
+    "dcsim_ensemble_moments", "dcsim_ensemble_spread",
 )
 
 _lib = None
@@ -90,6 +92,17 @@ def load():
     if hasattr(L, "dcsim_recorder_counts"):
         L.dcsim_recorder_counts.restype = i32
         L.dcsim_recorder_counts.argtypes = [vp, C.POINTER(u32 * 3)]
+    if hasattr(L, "dcsim_enable_cluster_ensemble"):
+        L.dcsim_enable_cluster_ensemble.restype = i32
+        L.dcsim_enable_cluster_ensemble.argtypes = [vp, u32]
+        L.dcsim_cluster_ensemble_capacity.restype = i32
+        L.dcsim_cluster_ensemble_capacity.argtypes = [vp, C.POINTER(u32)]
+        L.dcsim_fetch_cluster_ensemble.restype = i32
+        L.dcsim_fetch_cluster_ensemble.argtypes = [vp, vp, C.c_size_t]
+        L.dcsim_ensemble_moments.restype = i32
+        L.dcsim_ensemble_moments.argtypes = [vp, vp]
+        L.dcsim_ensemble_spread.restype = i32
+        L.dcsim_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

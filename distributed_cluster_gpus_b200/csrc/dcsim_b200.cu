@@ -10,6 +10,7 @@
  *                             over <CAP, MODE> (power-cap controller compiled in / what is staged) and picked per handle.
  *   dcsim_reduce_kernel       [n_replicas][K] summaries -> DCSIM_AGG_K doubles (the only cross-GPU payload).
  *   dcsim_hist_reduce_kernel  per-replica job-latency histograms -> one [2][128] histogram (opt-in).
+ *   dcsim_ens_*_kernel        the cluster-log ensemble (opt-in) -> per-column moments, then spread + histograms.
  *
  * Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see __graft_entry__.build()).
  * -fmad=false matters: the reference is CPython float arithmetic, one rounding per operation.
@@ -103,6 +104,107 @@ __global__ void dcsim_reduce_kernel(const double* __restrict__ summary, uint64_t
   }
 }
 
+/* ---- cluster-log ensemble reductions --------------------------------------------------------------------------
+ * Column = (tick, field, dc): n_replicas contiguous doubles.  One CTA per column: thread t takes replicas t, t + 256, ...
+ * in order, then a fixed shuffle tree and the warps' partials in warp order — the float sums depend on the replica
+ * count only, so they are bit-identical from run to run (no float atomics). */
+#define DCSIM_ENS_THREADS 256
+
+/* Ticks each replica recorded (its DCSIM_S_EV_LOG) into nlog[0, n), their maximum into nlog[n] (the capacity check). */
+__global__ void dcsim_ens_counts_kernel(const double* __restrict__ summary, uint64_t n, uint32_t* __restrict__ nlog) {
+  uint32_t m = 0u;
+  for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t k = (uint32_t)summary[r * DCSIM_SUMMARY_K + DCSIM_S_EV_LOG];
+    nlog[r] = k;
+    m = k > m ? k : m;
+  }
+  m = __reduce_max_sync(0xffffffffu, m);
+  if ((threadIdx.x & 31u) == 0u && m) atomicMax(nlog + n, m);
+}
+
+__device__ __forceinline__ double dcsim_ens_min(double a, double b) { return b < a ? b : a; }
+__device__ __forceinline__ double dcsim_ens_max(double a, double b) { return b > a ? b : a; }
+
+/* Pass 1: out = [4][n_cols] {n, sum, min, max} over the replicas that recorded the column's tick. */
+__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_moments_kernel(const double* __restrict__ ens, const uint32_t* __restrict__ nlog,
+                                                                              uint64_t n, uint64_t n_cols, uint32_t cols_per_tick,
+                                                                              double* __restrict__ out) {
+  __shared__ double s_sum[DCSIM_ENS_THREADS / 32], s_lo[DCSIM_ENS_THREADS / 32], s_hi[DCSIM_ENS_THREADS / 32];
+  __shared__ uint32_t s_cnt[DCSIM_ENS_THREADS / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (uint64_t col = blockIdx.x; col < n_cols; col += gridDim.x) {
+    const uint32_t tick = (uint32_t)(col / cols_per_tick);
+    const double* x = ens + col * n;
+    double sum = 0.0, lo = DCSIM_INF, hi = -DCSIM_INF;
+    uint32_t cnt = 0u;
+    for (uint64_t r = threadIdx.x; r < n; r += DCSIM_ENS_THREADS) {
+      if (tick < nlog[r]) { const double v = x[r]; sum += v; lo = dcsim_ens_min(lo, v); hi = dcsim_ens_max(hi, v); ++cnt; }
+    }
+    for (int o = 16; o > 0; o >>= 1) {
+      sum += __shfl_xor_sync(0xffffffffu, sum, o);
+      lo = dcsim_ens_min(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+      hi = dcsim_ens_max(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+      cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+    }
+    if (lane == 0) { s_sum[w] = sum; s_lo[w] = lo; s_hi[w] = hi; s_cnt[w] = cnt; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int k = 1; k < DCSIM_ENS_THREADS / 32; ++k) {
+        sum += s_sum[k]; lo = dcsim_ens_min(lo, s_lo[k]); hi = dcsim_ens_max(hi, s_hi[k]); cnt += s_cnt[k];
+      }
+      out[col] = (double)cnt; out[n_cols + col] = sum; out[2 * n_cols + col] = lo; out[3 * n_cols + col] = hi;
+    }
+    __syncthreads();
+  }
+}
+
+/* Pass 2: m2[col] = sum (x - mean)^2 and hist[col][DCSIM_ENS_BINS] over [lo, hi] (bin rule: include/dcsim_b200.h). */
+__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_spread_kernel(const double* __restrict__ ens, const uint32_t* __restrict__ nlog,
+                                                                             uint64_t n, uint64_t n_cols, uint32_t cols_per_tick, int n_dc,
+                                                                             const double* __restrict__ mean, const double* __restrict__ lo_in,
+                                                                             const double* __restrict__ hi_in, double* __restrict__ m2_out,
+                                                                             unsigned long long* __restrict__ hist_out) {
+  __shared__ uint32_t bins[DCSIM_ENS_BINS];
+  __shared__ double s_m2[DCSIM_ENS_THREADS / 32];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (uint64_t col = blockIdx.x; col < n_cols; col += gridDim.x) {
+    for (int b = threadIdx.x; b < DCSIM_ENS_BINS; b += DCSIM_ENS_THREADS) bins[b] = 0u;
+    __syncthreads();
+    const uint32_t tick = (uint32_t)(col / cols_per_tick);
+    const int field = (int)((col / (uint64_t)n_dc) % DCSIM_ENS_FIELDS);
+    const bool integral = field >= DCSIM_ENS_BUSY && field <= DCSIM_ENS_Q_TRAIN;
+    const double mu = mean[col], lo = lo_in[col], hi = hi_in[col];
+    double width = 0.0; /* 0: everything in bin 0 */
+    if (hi > lo) {
+      if (integral) { const double span = hi - lo + 1.0; width = span <= (double)DCSIM_ENS_BINS ? 1.0 : ceil(span / (double)DCSIM_ENS_BINS); }
+      else width = (hi - lo) / (double)DCSIM_ENS_BINS;
+    }
+    const double* x = ens + col * n;
+    double m2 = 0.0;
+    for (uint64_t r = threadIdx.x; r < n; r += DCSIM_ENS_THREADS) {
+      if (tick < nlog[r]) {
+        const double v = x[r], dv = v - mu;
+        m2 += dv * dv;
+        int b = 0;
+        if (width > 0.0) {
+          const double f = floor((v - lo) / width);
+          b = f >= (double)(DCSIM_ENS_BINS - 1) ? DCSIM_ENS_BINS - 1 : (f > 0.0 ? (int)f : 0);
+        }
+        atomicAdd(&bins[b], 1u);
+      }
+    }
+    for (int o = 16; o > 0; o >>= 1) m2 += __shfl_xor_sync(0xffffffffu, m2, o);
+    if (lane == 0) s_m2[w] = m2;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      for (int k = 1; k < DCSIM_ENS_THREADS / 32; ++k) m2 += s_m2[k];
+      m2_out[col] = m2;
+    }
+    for (int b = threadIdx.x; b < DCSIM_ENS_BINS; b += DCSIM_ENS_THREADS) hist_out[col * DCSIM_ENS_BINS + b] = bins[b];
+    __syncthreads();
+  }
+}
+
 /* ================================================================================================
  * C-ABI
  * ============================================================================================== */
@@ -143,6 +245,9 @@ struct dcsim {
   double max_transfer;
   uint32_t* d_hist;
   uint32_t* d_mt; /* [624][n_replicas] Mersenne Twister states, rng_kind == DCSIM_RNG_MT19937 only */
+  double* d_ens;       /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble (opt-in) */
+  uint32_t* d_ens_nlog; /* [n_replicas] ticks each replica recorded, + 1 word: the largest DCSIM_S_EV_LOG */
+  uint32_t ens_cap;
   int rng_kind;
   uint32_t cap_arr;
   unsigned long long events_seen;
@@ -150,6 +255,10 @@ struct dcsim {
 };
 
 static thread_local char g_create_err[512] = "";
+
+static size_t ens_bytes(const dcsim_t* h, uint32_t ticks) {
+  return (size_t)ticks * DCSIM_ENS_FIELDS * (size_t)h->spec.n_dc * (size_t)h->n_replicas * sizeof(double);
+}
 
 static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", long long b = 0) {
   char* dst = h ? h->err : g_create_err;
@@ -384,6 +493,7 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
   CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, (size_t)h->n_replicas * (size_t)h->L.total_bytes, h->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->stream));
   if (h->d_hist) CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t), h->stream));
+  if (h->d_ens) CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, ens_bytes(h, h->ens_cap), h->stream)); /* NaN: not recorded */
   h->seed0 = base_seed + first_replica_id;
   h->arrivals_ready = 0;
   h->launches = 0; /* a reset batch is "fresh": recorders may be re-targeted before its first advance */
@@ -456,6 +566,7 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->max_transfer = h->max_transfer;
   P->lat_hist = h->d_hist;
   P->mt_state = h->d_mt;
+  P->ens = h->d_ens; P->ens_cap = h->ens_cap;
 }
 
 int dcsim_prepare(dcsim_t* h) {
@@ -628,6 +739,98 @@ int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
+int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks) {
+  if (!h) return DCSIM_E_INVALID;
+  const uint32_t ticks = max_ticks ? max_ticks : dcsim_ens_ticks(&h->spec);
+  if (h->d_ens && h->ens_cap == ticks) return DCSIM_OK;
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_cluster_ensemble must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (h->d_ens) { cudaFree(h->d_ens); h->d_ens = NULL; h->ens_cap = 0; }
+  if (!h->d_ens_nlog) CUDA_TRY(h, cudaMalloc(&h->d_ens_nlog, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  const size_t bytes = ens_bytes(h, ticks);
+  const cudaError_t e = cudaMalloc(&h->d_ens, bytes ? bytes : sizeof(double));
+  if (e != cudaSuccess) {
+    h->d_ens = NULL;
+    if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
+    cudaGetLastError();
+    return set_err(h, DCSIM_E_NOMEM, "enable_cluster_ensemble: %s%lld bytes of device memory do not fit (run fewer replicas)", "",
+                   (long long)bytes);
+  }
+  h->ens_cap = ticks;
+  CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, bytes, h->stream)); /* NaN: not recorded */
+  return DCSIM_OK;
+}
+
+int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out) {
+  if (!h || !ticks_out) return DCSIM_E_INVALID;
+  *ticks_out = h->d_ens ? h->ens_cap : 0u;
+  return DCSIM_OK;
+}
+
+/* Every replica's recorded tick count into d_ens_nlog; fails when one of them went past the capacity (synchronises). */
+static int ens_counts(dcsim_t* h) {
+  if (!h->d_ens) return set_err(h, DCSIM_E_STATE, "cluster ensemble not enabled (dcsim_enable_cluster_ensemble)%s%lld");
+  if (!h->launches) return set_err(h, DCSIM_E_STATE, "cluster ensemble read before the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_ens_nlog + h->n_replicas, 0, sizeof(uint32_t), h->stream));
+  int blocks = (int)((h->n_replicas + 255) / 256);
+  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, h->d_ens_nlog);
+  CUDA_TRY(h, cudaGetLastError());
+  uint32_t most = 0u;
+  CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (most > h->ens_cap) {
+    snprintf(h->err, sizeof(h->err), "cluster ensemble overflow: a replica recorded %u log ticks, capacity %u", most, h->ens_cap);
+    return DCSIM_E_STATE;
+  }
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  const int rc = ens_counts(h);
+  if (rc != DCSIM_OK) return rc;
+  const size_t tick_bytes = ens_bytes(h, 1);
+  size_t ticks = out_bytes / tick_bytes;
+  if (ticks > h->ens_cap) ticks = h->ens_cap;
+  if (ticks) {
+    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_ens, ticks * tick_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  }
+  return DCSIM_OK;
+}
+
+static int ens_grid(const dcsim_t* h, uint64_t n_cols) { return (int)(n_cols < (1ull << 20) ? (n_cols ? n_cols : 1ull) : (1ull << 20)); }
+
+int dcsim_ensemble_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = ens_counts(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
+  const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
+  if (!n_cols) return DCSIM_OK;
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(h->d_ens, h->d_ens_nlog, h->n_replicas, n_cols,
+                                                                                     cols_per_tick, dev_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
+                          uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = ens_counts(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
+  const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
+  if (!n_cols) return DCSIM_OK;
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(h->d_ens, h->d_ens_nlog, h->n_replicas, n_cols,
+                                                                                    cols_per_tick, h->spec.n_dc, dev_mean, dev_lo, dev_hi,
+                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
 int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {
   if (!h || !out3) return DCSIM_E_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
@@ -696,6 +899,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_hist); cudaFree(h->d_agg); cudaFree(h->d_hist_out);
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
   cudaFree(h->d_mt);
+  cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
   cudaFree(h->d_arr_t); cudaFree(h->d_arr_raw); cudaFree(h->d_arr_meta); cudaFree(h->d_arr_pred); cudaFree(h->d_arr_tx);
   cudaFree(h->d_arr_fin); cudaFree(h->d_ml_t); cudaFree(h->d_ml_aux); cudaFree(h->d_ml_meta); cudaFree(h->d_arr_hdr);
   if (h->own_stream) cudaStreamDestroy(h->own_stream);

@@ -468,8 +468,9 @@ struct dcsim_kparams_t {
   uint32_t* lat_hist;   /* [n_replicas][2][DCSIM_LAT_BINS] job-latency histograms, or NULL */
   uint32_t* mt_state;   /* [624][n_replicas] Mersenne Twister states (rng = MT19937 only), else NULL */
   uint32_t cap_arr;
-  uint32_t _pad33;
-  double end_eps;       /* end_time + 1e-9, the _schedule cut-off (SIM:161) */
+  uint32_t ens_cap;     /* ticks the cluster-log ensemble holds */
+  double* ens;          /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble, or NULL */
+  double end_eps;      /* end_time + 1e-9, the _schedule cut-off (SIM:161) */
   double max_transfer;  /* largest finite transfer_s[ingress][dc][jtype] of the scenario */
 };
 
@@ -1873,6 +1874,46 @@ DCSIM_DEV void dcsim_control_cap_greedy(dcsim_ctx_t& c) {
   }
 }
 
+/* Log ticks a replica processes: the SIM:157 / :949 chain t += log_interval from 0 against the loop's t > end_time
+ * cut-off (SIM:427).  The log event is always pending until then, so the count does not depend on the random stream.
+ * Host code: the default capacity of the cluster-log ensemble. */
+static inline uint32_t dcsim_ens_ticks(const dcsim_spec_t* sp) {
+  uint32_t n = 0u;
+  for (double t = 0.0 + sp->log_interval; !(t > sp->end_time) && n < 0xffffffffu; t = t + sp->log_interval) ++n;
+  return n;
+}
+
+/* Cluster-log ensemble (opt-in: P->ens): DC d's values at log tick `tick` of replica r, each computed the way
+ * write_csv_logs (simulator_paper_multi.py) derives its CSV column from the cluster record (SIM:944-948).  One scattered
+ * 8-byte store per field; the layout [tick][field][dc][replica] is for the reductions, which read it coalesced. */
+DCSIM_COLD void dcsim_ens_record(const dcsim_kparams_t* P, char* blk, char* rec, uint32_t r, uint32_t tick, int d, double now,
+                                 double acc) {
+  const dcsim_layout_t& L = P->L;
+  const struct { char* blk; } v = {blk};
+  const int n = DCI(v, DI_NRUN)[d], busy = DCI(v, DI_BUSY)[d];
+  const uint32_t* meta = dcsim_at<uint32_t>(rec, L.rn_meta) + d * L.cap_run;
+  int run_inf = 0;
+  for (int i = 0; i < n; ++i) run_inf += ((meta[i] >> 16) & 1u) ? 0 : 1;
+  const int total = P->spec.dc[d].total_gpus;
+  const double ub = DCF(v, DF_UTIL_BEGIN)[d];
+  double elapsed = now - (ub != 0.0 ? ub : now); /* max(1e-9, now - (util_begin_ts or now)) */
+  elapsed = elapsed > 1e-9 ? elapsed : 1e-9;
+  const double util_avg = total ? DCF(v, DF_UTIL_TIME)[d] / ((double)total * elapsed) : 0.0;
+  const uint64_t fs = (uint64_t)P->spec.n_dc * P->n_replicas; /* field stride */
+  double* o = P->ens + ((uint64_t)tick * DCSIM_ENS_FIELDS * (uint64_t)P->spec.n_dc + (uint64_t)d) * P->n_replicas + r;
+  o[DCSIM_ENS_FREQ * fs] = DCF(v, DF_CUR_FREQ)[d];
+  o[DCSIM_ENS_BUSY * fs] = (double)busy;
+  o[DCSIM_ENS_RUN_TOTAL * fs] = (double)n;
+  o[DCSIM_ENS_RUN_INF * fs] = (double)run_inf;
+  o[DCSIM_ENS_RUN_TRAIN * fs] = (double)(n - run_inf);
+  o[DCSIM_ENS_Q_INF * fs] = (double)DCI(v, DI_QN_INF)[d];
+  o[DCSIM_ENS_Q_TRAIN * fs] = (double)DCI(v, DI_QN_TRN)[d];
+  o[DCSIM_ENS_UTIL_AVG * fs] = util_avg;
+  o[DCSIM_ENS_ACC_JOB_UNIT * fs] = acc;
+  o[DCSIM_ENS_POWER_W * fs] = DCF(v, DF_POWER)[d];
+  o[DCSIM_ENS_ENERGY_J * fs] = DCF(v, DF_ENERGY)[d];
+}
+
 /* SIM:929-949 + the :221-225 heuristic of _control.  DC-parallel: one DC per lane.
  * Entered with all prior writes visible; leaves with its own writes visible (trailing sync). */
 template <bool CAP>
@@ -1881,6 +1922,8 @@ DCSIM_DEV void dcsim_handle_log(dcsim_ctx_t& c) {
   const dcsim_layout_t& L = c.P->L;
   const double interval = sp.log_interval;
   const bool rec = c.is_logged && c.P->rec.cluster != nullptr;
+  const bool ens = c.P->ens != nullptr;
+  if (ens) dcsim_warp_sync(); /* lane 0's ev_log bump (dcsim_event_body) is visible to the lanes that read it below */
   if constexpr (CAP) { /* SIM:464: _control() precedes _handle_log() */
     if (c.lane == 0) dcsim_control_cap_greedy(c);
     dcsim_warp_sync();
@@ -1898,6 +1941,10 @@ DCSIM_DEV void dcsim_handle_log(dcsim_ctx_t& c) {
     double acc = DCF(c, DF_ACC_UNIT)[d];
     for (int i = 0; i < n; ++i) acc += tpt[i] * interval; /* SIM:941-942, running jobs in dict order */
     DCF(c, DF_ACC_UNIT)[d] = acc;
+    if (ens) {
+      const uint32_t tick = c.H->ev_log - 1u; /* bumped before the handler: right across chunked launches too */
+      if (tick < c.P->ens_cap) dcsim_ens_record(c.P, c.blk, c.rec, c.r, tick, d, c.now, acc);
+    }
     if (rec) { /* cluster_log.csv row, SIM:944-948; the rows of one tick are DC-ordered */
       const uint32_t r = c.P->rec.counts[2] + (uint32_t)d;
       if (r < c.P->rec.cluster_cap) {

@@ -19,6 +19,8 @@ assert CLUSTER_DTYPE.itemsize == C.sizeof(S.ClusterRec)
 
 
 LAT_BINS = 128
+ENS_FIELDS = 11     # DCSIM_ENS_FIELDS (names: ensemble.FIELDS)
+ENS_BINS = 1024     # DCSIM_ENS_BINS
 
 
 def latency_bin_edges() -> np.ndarray:
@@ -47,10 +49,13 @@ RNG_KINDS = {"philox": 0, "mt19937": 1}
 
 
 class RecorderOverflow(RuntimeError):
-    """A recorder (0 trace, 1 job log, 2 cluster log) saw more rows than its capacity; `.needed` says how many."""
+    """A recorder (0 trace, 1 job log, 2 cluster log, 3 cluster-log ensemble) saw more rows (ensemble: log ticks) than its
+    capacity; `.needed` says how many."""
 
     def __init__(self, which, needed, capacity):
-        super().__init__(f"{('trace', 'job log', 'cluster log')[which]} needs {needed} rows, capacity {capacity}")
+        unit = "ticks" if which == 3 else "rows"
+        super().__init__(f"{('trace', 'job log', 'cluster log', 'cluster ensemble')[which]} needs {needed} {unit}, "
+                         f"capacity {capacity}")
         self.which, self.needed, self.capacity = which, needed, capacity
 
 
@@ -66,6 +71,7 @@ class BatchedEngine:
         self._lib = N.load()
         self._h = C.c_void_p()
         self.n_replicas = int(n_replicas)
+        self.device = int(device)
         self.spec = spec
         blob = spec.to_bytes()
         self._blob = C.create_string_buffer(blob, len(blob))
@@ -74,6 +80,7 @@ class BatchedEngine:
         if cuda_stream:
             self.set_stream(cuda_stream)
         self._trace_cap = self._jobs_cap = self._cluster_cap = 0
+        self._ens_cap = 0
 
     # -- configuration ---------------------------------------------------------------------------
     def set_stream(self, cuda_stream: int):
@@ -152,6 +159,46 @@ class BatchedEngine:
         out = np.zeros((2, LAT_BINS), dtype=np.uint64)
         N.check(self._lib.dcsim_fetch_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
+
+    # -- cluster-log ensemble (ensemble.py turns it into per-tick statistics) --------------------------------------
+    def enable_cluster_ensemble(self, max_ticks=None):
+        """Opt-in, before the first advance of a batch (stays on across reset): every replica records the values of its
+        cluster_log.csv rows at every log tick (ensemble.FIELDS).  ``max_ticks=None``: the exact tick count of the spec."""
+        N.check(self._lib.dcsim_enable_cluster_ensemble(self._h, int(max_ticks or 0)), self._h)
+        cap = C.c_uint32(0)
+        N.check(self._lib.dcsim_cluster_ensemble_capacity(self._h, C.byref(cap)), self._h)
+        self._ens_cap = int(cap.value)
+
+    @property
+    def cluster_ensemble_capacity(self) -> int:
+        """Log ticks the recorder holds (0: not enabled)."""
+        return self._ens_cap
+
+    def _ens_check(self, rc):
+        """A replica recorded more ticks than the capacity: RecorderOverflow (never a truncated ensemble)."""
+        if rc == N.E_STATE and self._ens_cap and b"overflow" in (self._lib.dcsim_last_error(self._h) or b""):
+            needed = int(self.summary()[:, S.S_EV_LOG].max())
+            raise RecorderOverflow(3, needed, self._ens_cap)
+        N.check(rc, self._h)
+
+    def cluster_ensemble_rows(self) -> np.ndarray:
+        """[ticks, FIELDS, n_dc, n_replicas] float64, ticks = the most any replica recorded; NaN where a replica did not
+        reach a tick.  Raises RecorderOverflow if a replica went past the capacity.  For tests and small batches."""
+        if not self._ens_cap:
+            raise RuntimeError("cluster ensemble not enabled (enable_cluster_ensemble)")
+        ticks = min(int(self.summary()[:, S.S_EV_LOG].max()), self._ens_cap)
+        out = np.empty((ticks, ENS_FIELDS, self.spec.n_dc, self.n_replicas), dtype=np.float64)
+        self._ens_check(self._lib.dcsim_fetch_cluster_ensemble(self._h, C.c_void_p(out.ctypes.data), out.nbytes))
+        return out
+
+    def ensemble_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][capacity * FIELDS * n_dc] float64 {n, sum, min, max} at ``device_ptr``."""
+        self._ens_check(self._lib.dcsim_ensemble_moments(self._h, C.c_void_p(device_ptr)))
+
+    def ensemble_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        self._ens_check(self._lib.dcsim_ensemble_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                        C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)))
 
     # -- recorders -------------------------------------------------------------------------------
     def recorder_counts(self):
@@ -239,8 +286,9 @@ _CACHED = {"key": None, "engine": None}
 _CACHED_LOGGED = {"key": None, "engine": None}   # the one-replica companion engine of LoggedReplica
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream):
-    return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""))
+def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False):
+    return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
+            bool(cluster_ensemble))
 
 
 def _drop_parked_batch_engine():
@@ -249,8 +297,10 @@ def _drop_parked_batch_engine():
     _CACHED["engine"], _CACHED["key"] = None, None
 
 
-def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0):
-    key = _cache_key(sp, n_replicas, device, cuda_stream)
+def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False):
+    """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on (a parked engine is only reused by a
+    caller that asks for the same)."""
+    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -259,7 +309,14 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
         eng.set_rng("philox")
         return eng
     _drop_parked_batch_engine()   # (tens of GB: gone before the new batch allocates; the one-replica companion stays)
-    return BatchedEngine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream)
+    eng = BatchedEngine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream)
+    if cluster_ensemble:
+        try:
+            eng.enable_cluster_ensemble()
+        except BaseException:
+            eng.close()
+            raise
+    return eng
 
 
 def release_engine(eng, sp, device=0, cuda_stream=0):
@@ -267,7 +324,7 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     parked companion of LoggedReplica is a separate slot and is left alone (closing and re-creating it would cost
     every run() its allocations)."""
     _drop_parked_batch_engine()
-    _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream)
+    _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0)
 
 
 def free_cached_engine():
@@ -315,15 +372,16 @@ class LoggedReplica:
 
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
-                      max_retries=3, configure=None, while_running=None):
+                      max_retries=3, configure=None, while_running=None, cluster_ensemble=False):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
-    kernels of the first attempt were launched and before the host waits for them (host work that can overlap)."""
+    kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
+    ``cluster_ensemble``: every attempt runs with the cluster-log ensemble recorder on."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
-        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream)
+        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

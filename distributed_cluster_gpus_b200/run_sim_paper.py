@@ -58,6 +58,9 @@ def parse_args(argv=None):
     p.add_argument("--gpus-per-dc", type=int, default=None, help="override total_gpus of every kept DC")
     p.add_argument("--freq-levels", type=str, default=None, help="comma-separated DVFS levels, e.g. 0.5,0.8,1.0")
     p.add_argument("--summary-json", type=str, default=None, help="write per-batch statistics to this file")
+    p.add_argument("--ensemble-csv", type=str, default=None, metavar="PATH",
+                   help="write per-tick statistics of every DC's cluster-log columns over all replicas (mean, std, min, "
+                        "p05/p25/p50/p75/p95, max; long format) to this file")
     p.add_argument("--gpus", type=int, default=1,
                    help="shard the replicas over this many GPUs of the node (one process per GPU; the only collective is "
                         "the all-reduce of the end-of-run statistics over NCCL).  Under torchrun the world size wins.")
@@ -90,7 +93,8 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         upgr_warmup=args.upgr_warmup, upgr_buffer=args.upgr_buffer, num_fixed_gpus=args.num_fixed_gpus,
         fixed_freq=args.fixed_freq, logger=get_logger(log_dir=out_dir),
         replicas=args.replicas if replicas is None else replicas, first_replica_id=first_replica_id,
-        device=args.device if device is None else device, write_logs=write_logs, rng=args.rng)
+        device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
+        cluster_ensemble=args.ensemble_csv is not None)
     return sim
 
 
@@ -115,10 +119,16 @@ def main(argv=None):
         return _main_sharded(args, world, rank)
     sim = build_simulator(args)
     sim.run()
+    _write_ensemble(args, sim)
     stats = batch_statistics(sim.summary)
     _add_latency_quantiles(stats, sim.latency_histogram)
     _report(args, stats)
     return sim
+
+
+def _write_ensemble(args, sim):
+    if args.ensemble_csv:
+        sim.cluster_ensemble.to_csv(args.ensemble_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_latency_quantiles(stats, hist):
@@ -155,8 +165,12 @@ def _main_sharded(args, world, rank):
         else:
             dist.init_process_group(backend)
     first, count = sharding.shard(args.replicas, rank, world)
+    if args.ensemble_csv and count == 0:
+        raise SystemExit("--ensemble-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
-    sim.run()
+    sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
+    if rank == 0:
+        _write_ensemble(args, sim)
     summ = sim.summary if count > 0 else sim.summary[:0]
     agg = torch.from_numpy(sharding.aggregate_rows(summ)).to(dev)
     hist = torch.from_numpy(sim.latency_histogram.astype(np.int64) if count > 0 else np.zeros((2, 128), np.int64)).to(dev)

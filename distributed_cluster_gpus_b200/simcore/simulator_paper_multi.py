@@ -59,7 +59,7 @@ class MultiIngressPaperSimulator:
                  num_fixed_gpus=1, fixed_freq=None,
                  # --- batched-engine additions (keyword only in spirit; defaults reproduce one trajectory) ---
                  replicas: int = 1, device: int = 0, first_replica_id: int = 0, write_logs: bool = True,
-                 cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox"):
+                 cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -93,6 +93,10 @@ class MultiIngressPaperSimulator:
         self.summary: Optional[np.ndarray] = None
         self.latency_histogram: Optional[np.ndarray] = None
         self.launch_info: Optional[dict] = None
+        # cluster_ensemble=True: after run(), per-tick statistics of every DC's cluster-log columns over all replicas (of
+        # all ranks when torch.distributed runs: every rank's run() takes part in the all-reduces), ensemble.EnsembleResult
+        self._want_ensemble = bool(cluster_ensemble)
+        self.cluster_ensemble = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -142,7 +146,8 @@ class MultiIngressPaperSimulator:
 
         try:
             eng, summ = run_to_completion(self._flatten, self.replicas, self.rng_seed, self.first_replica_id, self.device,
-                                          self.cuda_stream, configure=configure, while_running=while_running)
+                                          self.cuda_stream, configure=configure, while_running=while_running,
+                                          cluster_ensemble=self._want_ensemble)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -151,6 +156,9 @@ class MultiIngressPaperSimulator:
             self.summary = summ
             self.latency_histogram = eng.latency_histogram()     # [2, 128] job-latency counts of the whole batch
             self.launch_info = eng.launch_info()
+            if self._want_ensemble:
+                from ..ensemble import cluster_ensemble
+                self.cluster_ensemble = cluster_ensemble(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

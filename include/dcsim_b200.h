@@ -293,6 +293,49 @@ int dcsim_allreduce_summary(dcsim_t* h, void* nccl_comm, double* out);
 int dcsim_enable_latency_histogram(dcsim_t* h);
 int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
+/* Cluster-log ensemble: at every log tick, for EVERY replica, the values the replica's cluster_log.csv row of each DC
+ * would hold (simulator_paper_multi.py write_csv_logs), unrounded.  Device layout [tick][field][dc][replica] doubles,
+ * replica fastest (the reductions read it coalesced).  Tick k is the k-th processed log event (instant: the chain
+ * t += log_interval from 0, the same in every replica).  A replica writes ticks < capacity and keeps counting past that
+ * (its true count is DCSIM_S_EV_LOG of its summary row); a fetch or reduction that finds a replica past the capacity
+ * fails with DCSIM_E_STATE instead of truncating. */
+enum {
+  DCSIM_ENS_FREQ = 0,        /* current_freq, after the control_lower_idle rewrite (:221-225) */
+  DCSIM_ENS_BUSY = 1,        /* busy GPUs */
+  DCSIM_ENS_RUN_TOTAL = 2,   /* running jobs */
+  DCSIM_ENS_RUN_INF = 3,
+  DCSIM_ENS_RUN_TRAIN = 4,   /* run_total - run_inf */
+  DCSIM_ENS_Q_INF = 5,
+  DCSIM_ENS_Q_TRAIN = 6,
+  DCSIM_ENS_UTIL_AVG = 7,    /* util_gpu_time / (total * max(1e-9, now - (util_begin or now))), 0 when total == 0 */
+  DCSIM_ENS_ACC_JOB_UNIT = 8,
+  DCSIM_ENS_POWER_W = 9,
+  DCSIM_ENS_ENERGY_J = 10,   /* unrounded (the CSV shows energy_kJ) */
+  DCSIM_ENS_FIELDS = 11
+};
+#define DCSIM_ENS_BINS 1024
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, like the latency histogram).  max_ticks = 0:
+ * the exact number of log ticks of the spec (the t += log_interval chain replayed against the loop's t > end_time
+ * cut-off).  DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the buffer does not fit. */
+int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks);
+/* Tick capacity of the recorder (0 = not enabled). */
+int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out);
+/* Copies the first min(capacity, out_bytes / row bytes) ticks of the raw values, [tick][field][dc][replica] doubles,
+ * to host memory (synchronises).  Ticks a replica did not reach read as NaN.  For tests and small batches. */
+int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes);
+/* Pass 1, per column (tick, field, dc) over the replicas that recorded the tick: dev_out = [4][capacity * FIELDS * n_dc]
+ * doubles {n, sum, min, max} (an empty column: 0, 0, +inf, -inf).  The caller all-reduces rows 0-1 (sum), 2 (min), 3
+ * (max).  Fixed summation order (a function of the replica count only): bit-identical run to run.  Synchronises once to
+ * check the capacity. */
+int dcsim_ensemble_moments(dcsim_t* h, double* dev_out);
+/* Pass 2, given the global per-column mean, lo (min) and hi (max): dev_m2_out[column] = sum (x - mean)^2 (fixed order)
+ * and dev_hist_out[column][DCSIM_ENS_BINS] counts over [lo, hi].  Integer fields (busy, run_*, q_*) use unit bins
+ * centred on the integers lo, lo+1, ... when hi - lo + 1 <= DCSIM_ENS_BINS, else integer width ceil((hi - lo + 1) / BINS);
+ * the others width (hi - lo) / BINS, bin = min(BINS - 1, floor((x - lo) / width)) (all in bin 0 when hi == lo).  The
+ * caller all-reduces both (sum). */
+int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
+                          uint64_t* dev_hist_out);
+
 /* Word source of the replicas' random streams (before the first advance of a batch; stays across dcsim_reset).
  *   DCSIM_RNG_PHILOX   (default) Philox4x32-10, key = base_seed + replica id: counter-based, no state.
  *   DCSIM_RNG_MT19937  CPython's own Mersenne Twister seeded like random.seed(base_seed + replica id)
