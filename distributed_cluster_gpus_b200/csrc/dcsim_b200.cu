@@ -36,27 +36,36 @@ int dcsim_adv_min_ctas_g8(void);
 
 /* Arrival pre-pass: one THREAD per replica draws that replica's whole arrival sequence in the reference's draw order;
  * consecutive threads = consecutive replicas, so all 32 lanes of a warp run the samplers that the event loop would
- * otherwise run on one lane.  Per-thread scratch in shared memory, [slot][thread]: 2*MAX_ING stream clocks (f64),
- * 2*MAX_ING "latest arrival of the stream" indices (u32), DCSIM_TRNG_RING staged random words (u32). */
+ * otherwise run on one lane.  Per-thread scratch in shared memory, [slot][thread]: 2*n_ing stream clocks (f64),
+ * 2*n_ing "latest arrival of the stream" indices (u32), DCSIM_TRNG_RING staged random words (u32), DCSIM_ARR_STAGE
+ * staged arrivals (2 x f64 + 2 x u32). */
 #define DCSIM_ARRIVALS_THREADS 128
 /* 5 resident CTAs per SM: 132 x 5 x 128 = 84 480 threads on an H100, so the largest per-GPU batch of the BASELINE configs
- * (65 536 replicas) is ONE wave of this latency-bound kernel, and the register cap it implies (78 registers for the
- * Philox path, 96 for MT19937 on sm_90a) leaves both paths without spills.  A tighter bound (7: 72 registers) spills
- * and bought nothing measurable on the H100: the kernel's time was the same at 7, 5 and 4. */
+ * (65 536 replicas) is ONE wave of this kernel, and the register cap it implies leaves both paths without spills (88
+ * registers for the Philox path, 90 for MT19937 on sm_90a).  Shared memory allows the 5 CTAs up to 4 ingresses (40 KB per
+ * CTA); at 8 ingresses a CTA takes 52 KB and 4 fit, 67 584 threads: still one wave of 65 536.  A tighter bound
+ * (7: 72 registers) spills and bought nothing measurable on the H100: the kernel's time was the same at 7, 5 and 4
+ * (measured before the output staging, when the kernel's time went to its scattered stores, DESIGN.md §4.0). */
 #define DCSIM_ARRIVALS_MIN_CTAS 5
-static size_t dcsim_arrivals_scratch_bytes(int n_ing) { /* per CTA: [slot][thread] arrays for 2 * n_ing streams */
-  return (size_t)DCSIM_ARRIVALS_THREADS * ((size_t)(2 * n_ing) * (sizeof(double) + sizeof(uint32_t)) + DCSIM_TRNG_RING * sizeof(uint32_t));
+static size_t dcsim_arrivals_scratch_bytes(int n_ing) { /* per CTA: [slot][thread] arrays for 2 * n_ing streams, ring, stage */
+  return (size_t)DCSIM_ARRIVALS_THREADS * ((size_t)(2 * n_ing) * (sizeof(double) + sizeof(uint32_t)) + DCSIM_TRNG_RING * sizeof(uint32_t) +
+                                           DCSIM_ARR_STAGE * (2 * sizeof(double) + 2 * sizeof(uint32_t)));
 }
 extern __shared__ __align__(16) double dcsim_arr_scratch[];
 template <bool MT>
 __global__ void __launch_bounds__(DCSIM_ARRIVALS_THREADS, DCSIM_ARRIVALS_MIN_CTAS) dcsim_arrivals_kernel(const __grid_constant__ dcsim_kparams_t P) {
   const uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (r >= P.n_replicas) return;
+  if (r - (threadIdx.x & 31u) >= P.n_replicas) return; /* whole warps only: the output flush needs every lane of a warp */
   const int n_streams = 2 * P.spec.n_ing;
   double* clocks = dcsim_arr_scratch + threadIdx.x;                                             /* [stream][thread] */
   uint32_t* last = reinterpret_cast<uint32_t*>(dcsim_arr_scratch + n_streams * blockDim.x) + threadIdx.x; /* [stream][thread] */
   uint32_t* ring = last + n_streams * blockDim.x;                                               /* [word][thread] */
-  dcsim_generate_arrivals<MT>(&P, r, clocks, last, ring, (int)blockDim.x);
+  dcsim_arr_stage_t st;                                                                          /* [slot][thread] */
+  st.t = reinterpret_cast<double*>(ring - threadIdx.x + DCSIM_TRNG_RING * blockDim.x) + threadIdx.x; /* 8-byte aligned: blockDim.x is even */
+  st.raw = st.t + DCSIM_ARR_STAGE * blockDim.x;
+  st.meta = reinterpret_cast<uint32_t*>(st.raw - threadIdx.x + DCSIM_ARR_STAGE * blockDim.x) + threadIdx.x;
+  st.pred = st.meta + DCSIM_ARR_STAGE * blockDim.x;
+  dcsim_generate_arrivals<MT>(&P, r, clocks, last, ring, (int)blockDim.x, st);
 }
 
 /* List merge: one WARP per replica (lane-parallel over the replica's arrivals), a sliding window of them in shared memory. */
@@ -577,9 +586,14 @@ int dcsim_prepare(dcsim_t* h) {
   dcsim_kparams_t P;
   fill_kparams(h, &P, 0);
   const int nb = (int)((h->n_replicas + DCSIM_ARRIVALS_THREADS - 1) / DCSIM_ARRIVALS_THREADS);
-  const size_t scratch = dcsim_arrivals_scratch_bytes(h->spec.n_ing);
-  if (h->rng_kind == DCSIM_RNG_MT19937) dcsim_arrivals_kernel<true><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
-  else dcsim_arrivals_kernel<false><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
+  const size_t scratch = dcsim_arrivals_scratch_bytes(h->spec.n_ing); /* 52 KB at 8 ingresses: above the 48 KB default */
+  if (h->rng_kind == DCSIM_RNG_MT19937) {
+    CUDA_TRY(h, cudaFuncSetAttribute(dcsim_arrivals_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scratch));
+    dcsim_arrivals_kernel<true><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
+  } else {
+    CUDA_TRY(h, cudaFuncSetAttribute(dcsim_arrivals_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scratch));
+    dcsim_arrivals_kernel<false><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
+  }
   CUDA_TRY(h, cudaGetLastError());
   const int wpb = DCSIM_MERGE_THREADS / 32;
   dcsim_merge_kernel<<<(int)((h->n_replicas + wpb - 1) / wpb), DCSIM_MERGE_THREADS, 0, h->stream>>>(P);

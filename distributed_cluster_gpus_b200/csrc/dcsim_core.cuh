@@ -846,23 +846,59 @@ static inline double dcsim_test_quantize(double t) {
  * every later one was pushed while its predecessor — list entry `last` — was being processed (SIM:591-592). */
 DCSIM_DEV uint32_t dcsim_stream_rank(uint32_t last, int q) { return last == DCSIM_NO_PRED ? (uint32_t)q : 16u + last; }
 
+/* Output staging of the GPU pre-pass.  Written straight to the replica-major arrays, every arrival would be four warp
+ * stores with each lane in its own replica's row (cap_arr apart): 32 partly written sectors per store, spread over the
+ * whole multi-GB output.  Instead each thread stages DCSIM_ARR_STAGE arrivals in shared memory and the warp flushes them
+ * together, DCSIM_ARR_STAGE lanes per replica, so that every store writes contiguous runs of a few replicas' rows.  The
+ * arrival loop is warp-uniform and an alive replica adds exactly one arrival per iteration, so the alive lanes of a warp
+ * fill their stages in step; a replica that has ended keeps its last few arrivals until the warp's next flush. */
+#define DCSIM_ARR_STAGE 4u /* a power of two dividing 32 */
+struct dcsim_arr_stage_t { double* t; double* raw; uint32_t* meta; uint32_t* pred; }; /* [slot][thread] in shared memory */
+#ifndef DCSIM_HOST_EMU
+/* Writes arrivals [flushed, count) of the warp's replicas from their stages.  Called by all 32 lanes together: a lane
+ * writes other lanes' arrivals, so every lane of the warp must be there, including those without a replica. */
+DCSIM_DEV void dcsim_arr_flush(const dcsim_kparams_t* P, const dcsim_arr_stage_t& st, int stride, uint64_t r, uint32_t flushed,
+                               uint32_t count) {
+  const uint32_t lane = threadIdx.x & 31u, e = lane & (DCSIM_ARR_STAGE - 1u);
+  const uint32_t n_mine = count - flushed;
+#pragma unroll
+  for (uint32_t j0 = 0u; j0 < 32u; j0 += 32u / DCSIM_ARR_STAGE) {
+    const uint32_t j = j0 + lane / DCSIM_ARR_STAGE; /* the lane whose arrivals this one writes */
+    const uint32_t nj = __shfl_sync(0xffffffffu, n_mine, (int)j), fj = __shfl_sync(0xffffffffu, flushed, (int)j);
+    if (e < nj) {
+      const uint32_t k = fj + e;
+      const int src = (int)(k & (DCSIM_ARR_STAGE - 1u)) * stride + (int)j - (int)lane; /* stage slot of arrival k, thread j */
+      const uint64_t o = (r - lane + j) * (uint64_t)P->cap_arr + k;
+      P->arr_t[o] = st.t[src];
+      P->arr_raw[o] = st.raw[src];
+      P->arr_meta[o] = st.meta[src];
+      P->arr_pred[o] = st.pred[src];
+    }
+  }
+}
+#endif
+
 /* One replica's arrival list.  Per-thread scratch, element s of each array at [s * stride] ([slot][thread] in shared
  * memory): `next_t` the 2*n_ing stream clocks, `last_idx` the list index of each stream's latest arrival, `ring` the
- * DCSIM_TRNG_RING staged words of the stream. */
+ * DCSIM_TRNG_RING staged words of the stream, `st` (GPU only) the DCSIM_ARR_STAGE arrivals not yet written out; the
+ * host build writes every arrival where it belongs at once.  r >= n_replicas (lanes of the grid's ragged last warp):
+ * no replica, the lane only takes part in the warp's collectives. */
 template <bool MT>
-DCSIM_DEV void dcsim_generate_arrivals(const dcsim_kparams_t* P, uint64_t r, double* next_t, uint32_t* last_idx, uint32_t* ring, int stride) {
+DCSIM_DEV void dcsim_generate_arrivals(const dcsim_kparams_t* P, uint64_t r, double* next_t, uint32_t* last_idx, uint32_t* ring, int stride,
+                                       dcsim_arr_stage_t st = dcsim_arr_stage_t()) {
   const dcsim_spec_t& sp = P->spec;
   const int n_streams = 2 * sp.n_ing;
+  const bool ghost = r >= P->n_replicas;
   dcsim_trng_t<MT> g;
   const uint64_t key = P->seed0 + r;
   g.k0 = (uint32_t)key; g.k1 = (uint32_t)(key >> 32); g.pos = 0u; g.filled = 0u;
-  if constexpr (MT) { g.mt.mt = P->mt_state + r; g.mt.mt_stride = P->n_replicas; dcsim_mt_seed(g.mt, key); }
+  if constexpr (MT) { g.mt.mt = P->mt_state + r; g.mt.mt_stride = P->n_replicas; if (!ghost) dcsim_mt_seed(g.mt, key); }
   uint32_t status = 0u, first_mask = 0u, count = 0u;
   const double end_eps = P->end_eps;
   dcsim_squeeze_t sq[2];
   sq[0] = dcsim_squeeze_setup(sp.arr[0], sp.two_pi);
   sq[1] = dcsim_squeeze_setup(sp.arr[1], sp.two_pi);
-  for (int s = 0; s < n_streams; ++s) { /* SIM:154-156 */
+  for (int s = 0; !ghost && s < n_streams; ++s) { /* SIM:154-156 */
     dcsim_trng_topup(g, ring, stride);
     const double t = dcsim_test_quantize(0.0 + dcsim_t_gap(g, ring, stride, sp, (s & 1) ? sq[1] : sq[0], s & 1, 0.0, &status));
     const bool ok = !(t == DCSIM_INF) && !(t > end_eps);
@@ -870,15 +906,19 @@ DCSIM_DEV void dcsim_generate_arrivals(const dcsim_kparams_t* P, uint64_t r, dou
     last_idx[s * stride] = DCSIM_NO_PRED;
     if (ok) first_mask |= 1u << s;
   }
+#ifdef DCSIM_HOST_EMU
   double* out_t = P->arr_t + r * (uint64_t)P->cap_arr;
   double* out_raw = P->arr_raw + r * (uint64_t)P->cap_arr;
   uint32_t* out_meta = P->arr_meta + r * (uint64_t)P->cap_arr;
   uint32_t* out_pred = P->arr_pred + r * (uint64_t)P->cap_arr;
+#else
+  uint32_t flushed = 0u; /* arrivals [0, flushed) are in HBM, [flushed, count) in the stage */
+#endif
   const int k_bits = dcsim_bit_length((uint32_t)sp.n_dc);
   /* The loop is WARP-uniform: a replica that has ended (end_time, an overflow) stays in it, switched off, until the
    * warp's last one has — so that the lanes can be made to reconverge (a full-mask __syncwarp) between the divergent
    * part of an arrival (rejection loops of different lengths) and the part all of them share (the log of the gap). */
-  bool alive = true;
+  bool alive = !ghost;
   for (;;) {
     int s = -1;
     double t = DCSIM_INF;
@@ -935,19 +975,31 @@ DCSIM_DEV void dcsim_generate_arrivals(const dcsim_kparams_t* P, uint64_t r, dou
       next_t[s * stride] = has_next ? tn : DCSIM_INF;
       if (count >= P->cap_arr) { status |= DCSIM_ST_ARRIVALS_OVERFLOW; alive = false; }
       else {
-        out_t[count] = t;
-        out_raw[count] = raw;
-        out_meta[count] = (uint32_t)s | ((uint32_t)dc_sel << 4) | (has_next ? 0x80u : 0u) | raw_is_size;
-        out_pred[count] = last_idx[s * stride];
+        const uint32_t meta = (uint32_t)s | ((uint32_t)dc_sel << 4) | (has_next ? 0x80u : 0u) | raw_is_size;
+#ifdef DCSIM_HOST_EMU
+        out_t[count] = t; out_raw[count] = raw; out_meta[count] = meta; out_pred[count] = last_idx[s * stride];
+#else
+        const int slot = (int)(count & (DCSIM_ARR_STAGE - 1u)) * stride;
+        st.t[slot] = t; st.raw[slot] = raw; st.meta[slot] = meta; st.pred[slot] = last_idx[s * stride];
+#endif
         last_idx[s * stride] = count;
         ++count;
       }
     }
+#ifndef DCSIM_HOST_EMU
+    if (dcsim_event_any_full(count - flushed == DCSIM_ARR_STAGE)) { /* the alive lanes' stages are full */
+      dcsim_arr_flush(P, st, stride, r, flushed, count);
+      flushed = count;
+    }
+#endif
   }
+#ifndef DCSIM_HOST_EMU
+  dcsim_arr_flush(P, st, stride, r, flushed, count);
+#endif
   dcsim_arrhdr_t h;
   h.count = count; h.first_mask = first_mask; h.rng_words = g.pos; h.status = status;
   h.ml_count = 0u; h.max_ahead = 0u; h._pad[0] = h._pad[1] = 0u;
-  P->arr_hdr[r] = h;
+  if (!ghost) P->arr_hdr[r] = h;
 }
 
 /* ================================================================================================
