@@ -23,6 +23,8 @@ EXPORTS = (
     "dcsim_recorder_counts", "dcsim_allreduce_summary", "dcsim_fetch_summary_host",
     "dcsim_enable_cluster_ensemble", "dcsim_cluster_ensemble_capacity", "dcsim_fetch_cluster_ensemble",
     "dcsim_ensemble_moments", "dcsim_ensemble_spread",
+    "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_job_ensemble_moments",
+    "dcsim_job_ensemble_spread", "dcsim_fetch_dc_latency_histogram",
 )
 
 _lib = None
@@ -103,6 +105,19 @@ def load():
         L.dcsim_ensemble_moments.argtypes = [vp, vp]
         L.dcsim_ensemble_spread.restype = i32
         L.dcsim_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "dcsim_enable_job_ensemble"):
+        L.dcsim_enable_job_ensemble.restype = i32
+        L.dcsim_enable_job_ensemble.argtypes = [vp, C.c_double]
+        L.dcsim_job_ensemble_windows.restype = i32
+        L.dcsim_job_ensemble_windows.argtypes = [vp, C.POINTER(u32)]
+        L.dcsim_fetch_job_ensemble.restype = i32
+        L.dcsim_fetch_job_ensemble.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
+        L.dcsim_job_ensemble_moments.restype = i32
+        L.dcsim_job_ensemble_moments.argtypes = [vp, vp]
+        L.dcsim_job_ensemble_spread.restype = i32
+        L.dcsim_job_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.dcsim_fetch_dc_latency_histogram.restype = i32
+        L.dcsim_fetch_dc_latency_histogram.argtypes = [vp, vp, C.c_size_t]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

@@ -9,8 +9,10 @@
  *                             event loop of dcsim_core.cuh, stages it back, writes the summary row.  Instantiated
  *                             over <CAP, MODE> (power-cap controller compiled in / what is staged) and picked per handle.
  *   dcsim_reduce_kernel       [n_replicas][K] summaries -> DCSIM_AGG_K doubles (the only cross-GPU payload).
- *   dcsim_hist_reduce_kernel  per-replica job-latency histograms -> one [2][128] histogram (opt-in).
- *   dcsim_ens_*_kernel        the cluster-log ensemble (opt-in) -> per-column moments, then spread + histograms.
+ *   dcsim_hist_reduce_kernel  per-replica job-latency histograms -> one [2][128] histogram (opt-in); the same for the
+ *                             per-DC [n_dc][2][128] histograms of the job-log ensemble.
+ *   dcsim_ens_*_kernel        the cluster-log and job-log ensembles (opt-in) -> per-column moments, then spread +
+ *                             histograms.
  *
  * Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see __graft_entry__.build()).
  * -fmad=false matters: the reference is CPython float arithmetic, one rounding per operation.
@@ -18,6 +20,7 @@
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 
+#include <float.h>
 #include <new>
 #include <stdio.h>
 #include <stdlib.h>
@@ -77,11 +80,16 @@ __global__ void __launch_bounds__(DCSIM_MERGE_THREADS) dcsim_merge_kernel(const 
   dcsim_merge_arrivals(&P, r, (int)(threadIdx.x & 31u), &rings[threadIdx.x >> 5]);
 }
 
-/* Sums the per-replica latency histograms: thread b of every block owns bin b (coalesced 1 KB rows). */
-__global__ void dcsim_hist_reduce_kernel(const uint32_t* __restrict__ hist, uint64_t n, unsigned long long* __restrict__ out) {
-  unsigned long long acc = 0ull;
-  for (uint64_t r = blockIdx.x; r < n; r += gridDim.x) acc += hist[r * (2 * DCSIM_LAT_BINS) + threadIdx.x];
-  if (acc) atomicAdd(out + threadIdx.x, acc);
+/* Sums per-replica histogram rows of `row_len` counts: thread t of every block owns bins t, t + blockDim.x, ...
+ * (coalesced rows).  `status` (or NULL): the replicas whose word is not 0 are left out. */
+__global__ void dcsim_hist_reduce_kernel(const uint32_t* __restrict__ hist, uint64_t n, uint32_t row_len,
+                                         const uint32_t* __restrict__ status, unsigned long long* __restrict__ out) {
+  for (uint32_t b = threadIdx.x; b < row_len; b += blockDim.x) {
+    unsigned long long acc = 0ull;
+    for (uint64_t r = blockIdx.x; r < n; r += gridDim.x)
+      if (!status || status[r] == 0u) acc += hist[r * row_len + b];
+    if (acc) atomicAdd(out + b, acc);
+  }
 }
 
 /* Aggregates the summaries; every block reduces a slice, then one atomicAdd per component. */
@@ -113,41 +121,101 @@ __global__ void dcsim_reduce_kernel(const double* __restrict__ summary, uint64_t
   }
 }
 
-/* ---- cluster-log ensemble reductions --------------------------------------------------------------------------
- * Column = (tick, field, dc): n_replicas contiguous doubles.  One CTA per column: thread t takes replicas t, t + 256, ...
- * in order, then a fixed shuffle tree and the warps' partials in warp order — the float sums depend on the replica
- * count only, so they are bit-identical from run to run (no float atomics). */
+/* ---- ensemble reductions (cluster log, job log) ---------------------------------------------------------------
+ * A column is one value per replica.  One CTA per column: thread t takes replicas t, t + 256, ... in order, then a
+ * fixed shuffle tree and the warps' partials in warp order — the float sums depend on the replica count only, so they
+ * are bit-identical from run to run (no float atomics).  A column source (Src) says where a column's values are, which
+ * replicas count, and whether the column is an integer field:
+ *   Src::at(col) -> a view whose get(r, v) loads replica r's value into v, false when r does not count;
+ *   Src::integral(col). */
 #define DCSIM_ENS_THREADS 256
 
-/* Ticks each replica recorded (its DCSIM_S_EV_LOG) into nlog[0, n), their maximum into nlog[n] (the capacity check). */
-__global__ void dcsim_ens_counts_kernel(const double* __restrict__ summary, uint64_t n, uint32_t* __restrict__ nlog) {
+/* Column `field` of every replica's summary row (as u32) into out[0, n), the maximum into out[n]: the ticks each replica
+ * recorded (DCSIM_S_EV_LOG, the maximum is the capacity check) or its status bits (DCSIM_S_STATUS). */
+__global__ void dcsim_ens_counts_kernel(const double* __restrict__ summary, uint64_t n, int field, uint32_t* __restrict__ out) {
   uint32_t m = 0u;
   for (uint64_t r = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; r < n; r += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t k = (uint32_t)summary[r * DCSIM_SUMMARY_K + DCSIM_S_EV_LOG];
-    nlog[r] = k;
+    const uint32_t k = (uint32_t)summary[r * DCSIM_SUMMARY_K + field];
+    out[r] = k;
     m = k > m ? k : m;
   }
   m = __reduce_max_sync(0xffffffffu, m);
-  if ((threadIdx.x & 31u) == 0u && m) atomicMax(nlog + n, m);
+  if ((threadIdx.x & 31u) == 0u && m) atomicMax(out + n, m);
 }
+
+/* Cluster-log ensemble: column (tick, field, dc) = n_replicas contiguous doubles, counted by the replicas that recorded
+ * the tick (tick < nlog[r]). */
+struct dcsim_ens_cluster_src {
+  const double* ens;
+  const uint32_t* nlog;
+  uint64_t n;
+  uint32_t cols_per_tick;
+  int n_dc;
+  struct view {
+    const double* x;
+    const uint32_t* nlog;
+    uint32_t tick;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (!(tick < nlog[r])) return false;
+      v = x[r];
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const { return view{ens + col * n, nlog, (uint32_t)(col / cols_per_tick)}; }
+  __device__ __forceinline__ bool integral(uint64_t col) const {
+    const int field = (int)((col / (uint64_t)n_dc) % DCSIM_ENS_FIELDS);
+    return field >= DCSIM_ENS_BUSY && field <= DCSIM_ENS_Q_TRAIN;
+  }
+};
+
+/* Job-log ensemble: column (row, field, dc, jtype), `cells` = n_dc * 2 per field.  JOBS and LAT_SUM are stored
+ * ([row][DCSIM_JENS_STORED][cell][replica]); MEAN_LATENCY = LAT_SUM / JOBS over the replicas with a job in the cell.
+ * Only replicas with status 0 count. */
+struct dcsim_ens_job_src {
+  const double* jens;
+  const uint32_t* status;
+  uint64_t n;
+  uint32_t cells;
+  struct view {
+    const double* jobs;
+    const double* lat;
+    const uint32_t* status;
+    int field;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (status[r] != 0u) return false;
+      if (field == DCSIM_JENS_JOBS) { v = jobs[r]; return true; }
+      if (field == DCSIM_JENS_LAT_SUM) { v = lat[r]; return true; }
+      const double k = jobs[r];
+      if (!(k > 0.0)) return false;
+      v = lat[r] / k;
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const {
+    const uint64_t row = col / ((uint64_t)DCSIM_JENS_FIELDS * cells), cell = col % cells;
+    const double* jobs = jens + (row * DCSIM_JENS_STORED * cells + cell) * n;
+    return view{jobs, jobs + (uint64_t)cells * n, status, (int)((col / cells) % DCSIM_JENS_FIELDS)};
+  }
+  __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JENS_FIELDS == DCSIM_JENS_JOBS; }
+};
 
 __device__ __forceinline__ double dcsim_ens_min(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double dcsim_ens_max(double a, double b) { return b > a ? b : a; }
 
-/* Pass 1: out = [4][n_cols] {n, sum, min, max} over the replicas that recorded the column's tick. */
-__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_moments_kernel(const double* __restrict__ ens, const uint32_t* __restrict__ nlog,
-                                                                              uint64_t n, uint64_t n_cols, uint32_t cols_per_tick,
+/* Pass 1: out = [4][n_cols] {n, sum, min, max} over the replicas that count in the column. */
+template <class Src>
+__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_moments_kernel(const Src src, uint64_t n, uint64_t n_cols,
                                                                               double* __restrict__ out) {
   __shared__ double s_sum[DCSIM_ENS_THREADS / 32], s_lo[DCSIM_ENS_THREADS / 32], s_hi[DCSIM_ENS_THREADS / 32];
   __shared__ uint32_t s_cnt[DCSIM_ENS_THREADS / 32];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   for (uint64_t col = blockIdx.x; col < n_cols; col += gridDim.x) {
-    const uint32_t tick = (uint32_t)(col / cols_per_tick);
-    const double* x = ens + col * n;
+    const typename Src::view x = src.at(col);
     double sum = 0.0, lo = DCSIM_INF, hi = -DCSIM_INF;
     uint32_t cnt = 0u;
     for (uint64_t r = threadIdx.x; r < n; r += DCSIM_ENS_THREADS) {
-      if (tick < nlog[r]) { const double v = x[r]; sum += v; lo = dcsim_ens_min(lo, v); hi = dcsim_ens_max(hi, v); ++cnt; }
+      double v;
+      if (x.get(r, v)) { sum += v; lo = dcsim_ens_min(lo, v); hi = dcsim_ens_max(hi, v); ++cnt; }
     }
     for (int o = 16; o > 0; o >>= 1) {
       sum += __shfl_xor_sync(0xffffffffu, sum, o);
@@ -168,8 +236,8 @@ __global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_moments_kernel(co
 }
 
 /* Pass 2: m2[col] = sum (x - mean)^2 and hist[col][DCSIM_ENS_BINS] over [lo, hi] (bin rule: include/dcsim_b200.h). */
-__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_spread_kernel(const double* __restrict__ ens, const uint32_t* __restrict__ nlog,
-                                                                             uint64_t n, uint64_t n_cols, uint32_t cols_per_tick, int n_dc,
+template <class Src>
+__global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_spread_kernel(const Src src, uint64_t n, uint64_t n_cols,
                                                                              const double* __restrict__ mean, const double* __restrict__ lo_in,
                                                                              const double* __restrict__ hi_in, double* __restrict__ m2_out,
                                                                              unsigned long long* __restrict__ hist_out) {
@@ -179,20 +247,19 @@ __global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_spread_kernel(con
   for (uint64_t col = blockIdx.x; col < n_cols; col += gridDim.x) {
     for (int b = threadIdx.x; b < DCSIM_ENS_BINS; b += DCSIM_ENS_THREADS) bins[b] = 0u;
     __syncthreads();
-    const uint32_t tick = (uint32_t)(col / cols_per_tick);
-    const int field = (int)((col / (uint64_t)n_dc) % DCSIM_ENS_FIELDS);
-    const bool integral = field >= DCSIM_ENS_BUSY && field <= DCSIM_ENS_Q_TRAIN;
+    const bool integral = src.integral(col);
     const double mu = mean[col], lo = lo_in[col], hi = hi_in[col];
     double width = 0.0; /* 0: everything in bin 0 */
     if (hi > lo) {
       if (integral) { const double span = hi - lo + 1.0; width = span <= (double)DCSIM_ENS_BINS ? 1.0 : ceil(span / (double)DCSIM_ENS_BINS); }
       else width = (hi - lo) / (double)DCSIM_ENS_BINS;
     }
-    const double* x = ens + col * n;
+    const typename Src::view x = src.at(col);
     double m2 = 0.0;
     for (uint64_t r = threadIdx.x; r < n; r += DCSIM_ENS_THREADS) {
-      if (tick < nlog[r]) {
-        const double v = x[r], dv = v - mu;
+      double v;
+      if (x.get(r, v)) {
+        const double dv = v - mu;
         m2 += dv * dv;
         int b = 0;
         if (width > 0.0) {
@@ -257,6 +324,12 @@ struct dcsim {
   double* d_ens;       /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble (opt-in) */
   uint32_t* d_ens_nlog; /* [n_replicas] ticks each replica recorded, + 1 word: the largest DCSIM_S_EV_LOG */
   uint32_t ens_cap;
+  double* d_jens;          /* [jens_windows + 1][DCSIM_JENS_STORED][n_dc][2][n_replicas] job-log ensemble (opt-in) */
+  uint32_t* d_jens_hist;   /* [n_replicas][n_dc][2][DCSIM_LAT_BINS] its per-DC latency histograms */
+  uint32_t* d_jens_status; /* [n_replicas] status words (+ 1 word: their maximum), refreshed by every reduction */
+  unsigned long long* d_jens_hist_out; /* [n_dc][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_latency_histogram */
+  double jens_bin;
+  uint64_t jens_windows;
   int rng_kind;
   uint32_t cap_arr;
   unsigned long long events_seen;
@@ -267,6 +340,13 @@ static thread_local char g_create_err[512] = "";
 
 static size_t ens_bytes(const dcsim_t* h, uint32_t ticks) {
   return (size_t)ticks * DCSIM_ENS_FIELDS * (size_t)h->spec.n_dc * (size_t)h->n_replicas * sizeof(double);
+}
+
+static size_t jens_row_bytes(const dcsim_t* h) { /* one row (window) of the job-log ensemble */
+  return (size_t)DCSIM_JENS_STORED * (size_t)h->spec.n_dc * 2 * (size_t)h->n_replicas * sizeof(double);
+}
+static size_t jens_hist_bytes(const dcsim_t* h) {
+  return (size_t)h->n_replicas * (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(uint32_t);
 }
 
 static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", long long b = 0) {
@@ -503,6 +583,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
   CUDA_TRY(h, cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->stream));
   if (h->d_hist) CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t), h->stream));
   if (h->d_ens) CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, ens_bytes(h, h->ens_cap), h->stream)); /* NaN: not recorded */
+  if (h->d_jens) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, (h->jens_windows + 1) * jens_row_bytes(h), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->stream));
+  }
   h->seed0 = base_seed + first_replica_id;
   h->arrivals_ready = 0;
   h->launches = 0; /* a reset batch is "fresh": recorders may be re-targeted before its first advance */
@@ -576,6 +660,8 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->lat_hist = h->d_hist;
   P->mt_state = h->d_mt;
   P->ens = h->d_ens; P->ens_cap = h->ens_cap;
+  P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
+  P->finish_rec = (P->lat_hist || P->jens) ? 1u : 0u;
 }
 
 int dcsim_prepare(dcsim_t* h) {
@@ -744,7 +830,7 @@ int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   if (e == cudaSuccess) {
     int blocks = 8 * h->sm_count;
     if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
-    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->stream>>>(h->d_hist, h->n_replicas, d_out);
+    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->stream>>>(h->d_hist, h->n_replicas, 2 * DCSIM_LAT_BINS, NULL, d_out);
     e = cudaGetLastError();
   }
   if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, need, cudaMemcpyDeviceToHost, h->stream);
@@ -789,7 +875,7 @@ static int ens_counts(dcsim_t* h) {
   CUDA_TRY(h, cudaMemsetAsync(h->d_ens_nlog + h->n_replicas, 0, sizeof(uint32_t), h->stream));
   int blocks = (int)((h->n_replicas + 255) / 256);
   if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, h->d_ens_nlog);
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_EV_LOG, h->d_ens_nlog);
   CUDA_TRY(h, cudaGetLastError());
   uint32_t most = 0u;
   CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->stream));
@@ -824,8 +910,8 @@ int dcsim_ensemble_moments(dcsim_t* h, double* dev_out) {
   const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
   const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
   if (!n_cols) return DCSIM_OK;
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(h->d_ens, h->d_ens_nlog, h->n_replicas, n_cols,
-                                                                                     cols_per_tick, dev_out);
+  const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_out);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
 }
@@ -838,10 +924,119 @@ int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_
   const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
   const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
   if (!n_cols) return DCSIM_OK;
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(h->d_ens, h->d_ens_nlog, h->n_replicas, n_cols,
-                                                                                    cols_per_tick, h->spec.n_dc, dev_mean, dev_lo, dev_hi,
+  const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
                                                                                     dev_m2_out, (unsigned long long*)dev_hist_out);
   CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!(bin_s >= 0.0 && bin_s <= DBL_MAX)) return set_err(h, DCSIM_E_INVALID, "enable_job_ensemble: bin_s must be finite and >= 0%s%lld");
+  const double bin = bin_s > 0.0 ? bin_s : h->spec.log_interval;
+  if (h->d_jens && h->jens_bin == bin) return DCSIM_OK;
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_ensemble must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  cudaFree(h->d_jens); cudaFree(h->d_jens_hist);
+  h->d_jens = NULL; h->d_jens_hist = NULL; h->jens_windows = 0; h->jens_bin = 0.0;
+  const uint64_t windows = dcsim_jens_windows(h->spec.end_time, bin);
+  const double need = ((double)windows + 1.0) * (double)jens_row_bytes(h) + (double)jens_hist_bytes(h);
+  const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
+  if (windows >= 0xffffffffull || need >= 9.0e18)
+    return set_err(h, DCSIM_E_NOMEM, "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)", "", need_ll);
+  if (!h->d_jens_status) CUDA_TRY(h, cudaMalloc(&h->d_jens_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  if (!h->d_jens_hist_out) CUDA_TRY(h, cudaMalloc(&h->d_jens_hist_out, (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
+  const size_t rows_bytes = (windows + 1) * jens_row_bytes(h);
+  cudaError_t e = cudaMalloc(&h->d_jens, rows_bytes);
+  if (e == cudaSuccess) e = cudaMalloc(&h->d_jens_hist, jens_hist_bytes(h));
+  if (e != cudaSuccess) {
+    cudaFree(h->d_jens); cudaFree(h->d_jens_hist);
+    h->d_jens = NULL; h->d_jens_hist = NULL;
+    if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
+    cudaGetLastError();
+    return set_err(h, DCSIM_E_NOMEM, "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)", "", need_ll);
+  }
+  h->jens_bin = bin; h->jens_windows = windows;
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, rows_bytes, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out) {
+  if (!h || !windows_out) return DCSIM_E_INVALID;
+  *windows_out = h->d_jens ? (uint32_t)h->jens_windows : 0u;
+  return DCSIM_OK;
+}
+
+/* Every replica's status word into d_jens_status (on the stream: the reductions that read it follow it there). */
+static int jens_status(dcsim_t* h) {
+  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "job ensemble not enabled (dcsim_enable_job_ensemble)%s%lld");
+  if (!h->launches) return set_err(h, DCSIM_E_STATE, "job ensemble read before the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_status + h->n_replicas, 0, sizeof(uint32_t), h->stream));
+  int blocks = (int)((h->n_replicas + 255) / 256);
+  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_jens_status);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "job ensemble not enabled (dcsim_enable_job_ensemble)%s%lld");
+  if (!h->launches) return set_err(h, DCSIM_E_STATE, "job ensemble read before the first advance%s%lld");
+  const size_t need_rows = (h->jens_windows + 1) * jens_row_bytes(h), need_hist = jens_hist_bytes(h);
+  if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
+    return set_err(h, DCSIM_E_INVALID, "fetch_job_ensemble: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jens, need_rows, cudaMemcpyDeviceToHost, h->stream));
+  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jens_hist, need_hist, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = jens_status(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
+  const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
+  const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                              double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = jens_status(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
+  const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
+  const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
+                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  const uint32_t row_len = 2u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
+  const size_t need = (size_t)row_len * sizeof(uint64_t);
+  if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_latency_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
+  const int rc = jens_status(h);
+  if (rc != DCSIM_OK) return rc;
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist_out, 0, need, h->stream));
+  int blocks = 8 * h->sm_count;
+  if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
+  dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->stream>>>(h->d_jens_hist, h->n_replicas, row_len, h->d_jens_status,
+                                                                         h->d_jens_hist_out);
+  CUDA_TRY(h, cudaGetLastError());
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_jens_hist_out, need, cudaMemcpyDeviceToHost, h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
   return DCSIM_OK;
 }
 
@@ -914,6 +1109,7 @@ void dcsim_destroy(dcsim_t* h) {
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
   cudaFree(h->d_mt);
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
+  cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_status); cudaFree(h->d_jens_hist_out);
   cudaFree(h->d_arr_t); cudaFree(h->d_arr_raw); cudaFree(h->d_arr_meta); cudaFree(h->d_arr_pred); cudaFree(h->d_arr_tx);
   cudaFree(h->d_arr_fin); cudaFree(h->d_ml_t); cudaFree(h->d_ml_aux); cudaFree(h->d_ml_meta); cudaFree(h->d_arr_hdr);
   if (h->own_stream) cudaStreamDestroy(h->own_stream);

@@ -447,7 +447,7 @@ struct dcsim_kparams_t {
   uint64_t seed0;       /* Philox key of local replica 0 (base_seed + first_replica_id) */
   uint64_t max_events;  /* per replica per launch; 0 = run to the end */
   uint32_t budget32;    /* the same as one 32-bit compare: 0 (unlimited) and anything >= 2^32 become 0xffffffff (host-computed) */
-  uint32_t _pad32;
+  uint32_t finish_rec;  /* lat_hist or jens is set: the finish handler's one test for both opt-in recorders */
   char* state;          /* [n_replicas][L.total_bytes] */
   char* queues;         /* [n_replicas][L.queue_bytes] */
   double* summary;      /* [n_replicas][DCSIM_SUMMARY_K] */
@@ -472,6 +472,10 @@ struct dcsim_kparams_t {
   double* ens;          /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble, or NULL */
   double end_eps;      /* end_time + 1e-9, the _schedule cut-off (SIM:161) */
   double max_transfer;  /* largest finite transfer_s[ingress][dc][jtype] of the scenario */
+  double* jens;         /* [jens_windows + 1][DCSIM_JENS_STORED][n_dc][2][n_replicas] job-log ensemble, or NULL */
+  uint32_t* jens_hist;  /* [n_replicas][n_dc][2][DCSIM_LAT_BINS] per-DC job-latency histograms (with jens) */
+  double jens_bin;      /* finish-window width [s] */
+  uint64_t jens_windows; /* W */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -1630,6 +1634,38 @@ DCSIM_DEV void dcsim_handle_list(dcsim_ctx_t& c) {
   }
 } /* (the event's closing sync follows in dcsim_event_body) */
 
+/* Finish windows of the job-log ensemble: W = max(1, ceil(end_time / bin_s)) (the f64 expression ensemble.py repeats).
+ * Host code; more than 2^32 - 2 windows read as 0xffffffff (the caller refuses them). */
+static inline uint64_t dcsim_jens_windows(double end_time, double bin_s) {
+  const double w = ceil(end_time / bin_s);
+  return w >= 1.0 ? (w < 4294967295.0 ? (uint64_t)w : 0xffffffffull) : 1ull;
+}
+
+/* Job-log ensemble (opt-in: P->jens): a job of DC d and type jt that finished at `now` after `lat` seconds goes into
+ * replica r's cells of window min(floor(now / bin_s), W - 1) and of row W (the whole run), and into its per-DC latency
+ * histogram.  Fire-and-forget REDs as in dcsim_hist_add: nothing waits for them.  Each cell has one writer (lane 0 of
+ * the replica's group) and same-address relaxed atomics of one thread stay in program order, so every sum is the
+ * sequential sum in finish order. */
+DCSIM_COLD void dcsim_jens_add(const dcsim_kparams_t* P, uint32_t r, int d, int jt, double now, double lat) {
+  const uint64_t n = P->n_replicas, W = P->jens_windows;
+  const uint64_t fs = 2ull * (uint64_t)P->spec.n_dc * n; /* field stride */
+  const double f = floor(now / P->jens_bin);
+  const uint64_t k = f >= (double)(W - 1u) ? W - 1u : (uint64_t)f;
+  double* win = P->jens + k * (DCSIM_JENS_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  double* all = P->jens + W * (DCSIM_JENS_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  uint32_t* cell = P->jens_hist + ((uint64_t)r * (uint64_t)P->spec.n_dc + (uint64_t)d) * (2 * DCSIM_LAT_BINS) +
+                   (uint32_t)(jt * DCSIM_LAT_BINS + dcsim_lat_bin(lat));
+#ifdef DCSIM_HOST_EMU
+  win[DCSIM_JENS_JOBS * fs] += 1.0; win[DCSIM_JENS_LAT_SUM * fs] += lat;
+  all[DCSIM_JENS_JOBS * fs] += 1.0; all[DCSIM_JENS_LAT_SUM * fs] += lat;
+  *cell += 1u;
+#else
+  atomicAdd(win + DCSIM_JENS_JOBS * fs, 1.0); atomicAdd(win + DCSIM_JENS_LAT_SUM * fs, lat);
+  atomicAdd(all + DCSIM_JENS_JOBS * fs, 1.0); atomicAdd(all + DCSIM_JENS_LAT_SUM * fs, lat);
+  atomicAdd(cell, 1u);
+#endif
+}
+
 /* SIM:701-927 minus RL/elastic branches (lane 0 part, after the record was read and before it is erased). */
 DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const dcsim_spec_t& sp = c.P->spec;
@@ -1645,7 +1681,14 @@ DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const double lat = now - dcsim_at<double>(c.rec, L.rn_start)[i]; /* SIM:820 */
   H->lat_sum += lat;
   if (jt == DCSIM_JT_INFERENCE) { H->lat_sum_inf += lat; H->n_fin_inf++; } else { H->lat_sum_trn += lat; H->n_fin_trn++; }
-  if (c.P->lat_hist) dcsim_hist_add(c.P->lat_hist, (uint64_t)c.r, jt, lat);
+#ifdef DCSIM_HOST_EMU
+  if (c.P->lat_hist || c.P->jens) { /* (the host builds set the pointers only) */
+#else
+  if (__builtin_expect(c.P->finish_rec != 0u, 0)) { /* opt-in recorders: off, they cost this one test */
+#endif
+    if (c.P->lat_hist) dcsim_hist_add(c.P->lat_hist, (uint64_t)c.r, jt, lat);
+    if (c.P->jens) dcsim_jens_add(c.P, c.r, d, jt, now, lat);
+  }
   if (L.lean == 0) { /* the readers of a finished job's size / f / jid: job_log.csv and the bandit's reward */
     const double f_used = dcsim_at<double>(c.rec, L.rn_f)[i];
     if (c.is_logged && c.P->rec.jobs)

@@ -21,6 +21,7 @@ assert CLUSTER_DTYPE.itemsize == C.sizeof(S.ClusterRec)
 LAT_BINS = 128
 ENS_FIELDS = 11     # DCSIM_ENS_FIELDS (names: ensemble.FIELDS)
 ENS_BINS = 1024     # DCSIM_ENS_BINS
+JENS_STORED = 2     # DCSIM_JENS_STORED: jobs, lat_sum per (window, dc, jtype) and replica
 
 
 def latency_bin_edges() -> np.ndarray:
@@ -81,6 +82,7 @@ class BatchedEngine:
             self.set_stream(cuda_stream)
         self._trace_cap = self._jobs_cap = self._cluster_cap = 0
         self._ens_cap = 0
+        self._jens_windows, self._jens_bin = 0, None
 
     # -- configuration ---------------------------------------------------------------------------
     def set_stream(self, cuda_stream: int):
@@ -200,6 +202,53 @@ class BatchedEngine:
         self._ens_check(self._lib.dcsim_ensemble_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
                                                         C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)))
 
+    # -- job-log ensemble (ensemble.job_ensemble turns it into per-window statistics) --------------------------------
+    def enable_job_ensemble(self, bin_s=None):
+        """Opt-in, before the first advance of a batch (stays on across reset): every replica sums its finished jobs and
+        their latencies per finish window of ``bin_s`` seconds (None / 0: log_interval), DC and job type, plus a per-DC
+        job-latency histogram."""
+        N.check(self._lib.dcsim_enable_job_ensemble(self._h, float(bin_s or 0.0)), self._h)
+        w = C.c_uint32(0)
+        N.check(self._lib.dcsim_job_ensemble_windows(self._h, C.byref(w)), self._h)
+        self._jens_windows = int(w.value)
+        self._jens_bin = float(bin_s) if bin_s else float(self.spec.log_interval)
+
+    @property
+    def job_ensemble_windows(self) -> int:
+        """W, the finish windows (0: not enabled); the recorder's rows are W + 1, the last one the whole run."""
+        return self._jens_windows
+
+    @property
+    def job_ensemble_bin(self):
+        """The window width [s] (None: not enabled)."""
+        return self._jens_bin if self._jens_windows else None
+
+    def job_ensemble_rows(self):
+        """(rows [W + 1, JENS_STORED, n_dc, 2, n_replicas] float64 {jobs, lat_sum}, hist [n_dc, 2, LAT_BINS, n_replicas]
+        uint32): every replica's raw recorder.  For tests and small batches."""
+        if not self._jens_windows:
+            raise RuntimeError("job ensemble not enabled (enable_job_ensemble)")
+        rows = np.empty((self._jens_windows + 1, JENS_STORED, self.spec.n_dc, 2, self.n_replicas), dtype=np.float64)
+        hist = np.empty((self.n_replicas, self.spec.n_dc, 2, LAT_BINS), dtype=np.uint32)
+        N.check(self._lib.dcsim_fetch_job_ensemble(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
+                                                   C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
+
+    def job_ensemble_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][(W + 1) * 3 * n_dc * 2] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_job_ensemble_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def job_ensemble_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_job_ensemble_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                    C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
+    def dc_latency_histogram(self) -> np.ndarray:
+        """[n_dc, 2, LAT_BINS] uint64: job-latency counts per DC and job type over the replicas with status 0."""
+        out = np.zeros((self.spec.n_dc, 2, LAT_BINS), dtype=np.uint64)
+        N.check(self._lib.dcsim_fetch_dc_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
+        return out
+
     # -- recorders -------------------------------------------------------------------------------
     def recorder_counts(self):
         """(trace, job_log, cluster_log) rows the recorders WOULD have written: more than a recorder's capacity means
@@ -286,9 +335,14 @@ _CACHED = {"key": None, "engine": None}
 _CACHED_LOGGED = {"key": None, "engine": None}   # the one-replica companion engine of LoggedReplica
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False):
+def _job_bin(sp, job_ensemble, job_ensemble_bin):
+    """The job-log ensemble's resolved window width, None when it is off."""
+    return float(job_ensemble_bin or sp.log_interval) if job_ensemble else None
+
+
+def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None):
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            bool(cluster_ensemble))
+            bool(cluster_ensemble), job_bin)
 
 
 def _drop_parked_batch_engine():
@@ -297,10 +351,13 @@ def _drop_parked_batch_engine():
     _CACHED["engine"], _CACHED["key"] = None, None
 
 
-def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False):
-    """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on (a parked engine is only reused by a
-    caller that asks for the same)."""
-    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble)
+def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
+                   job_ensemble=False, job_ensemble_bin=None):
+    """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
+    ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval).  A parked engine is only reused
+    by a caller that asks for the same recorders."""
+    job_bin = _job_bin(sp, job_ensemble, job_ensemble_bin)
+    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -310,12 +367,14 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
         return eng
     _drop_parked_batch_engine()   # (tens of GB: gone before the new batch allocates; the one-replica companion stays)
     eng = BatchedEngine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream)
-    if cluster_ensemble:
-        try:
+    try:
+        if cluster_ensemble:
             eng.enable_cluster_ensemble()
-        except BaseException:
-            eng.close()
-            raise
+        if job_bin is not None:
+            eng.enable_job_ensemble(job_bin)
+    except BaseException:
+        eng.close()
+        raise
     return eng
 
 
@@ -324,7 +383,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     parked companion of LoggedReplica is a separate slot and is left alone (closing and re-creating it would cost
     every run() its allocations)."""
     _drop_parked_batch_engine()
-    _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0)
+    _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
+                                                        eng.job_ensemble_bin)
 
 
 def free_cached_engine():
@@ -372,16 +432,19 @@ class LoggedReplica:
 
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
-                      max_retries=3, configure=None, while_running=None, cluster_ensemble=False):
+                      max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
+                      job_ensemble_bin=None):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
     kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
-    ``cluster_ensemble``: every attempt runs with the cluster-log ensemble recorder on."""
+    ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
+    window width, None = log_interval)."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
-        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble)
+        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
+                             job_ensemble, job_ensemble_bin)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

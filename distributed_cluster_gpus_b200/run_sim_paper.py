@@ -61,6 +61,11 @@ def parse_args(argv=None):
     p.add_argument("--ensemble-csv", type=str, default=None, metavar="PATH",
                    help="write per-tick statistics of every DC's cluster-log columns over all replicas (mean, std, min, "
                         "p05/p25/p50/p75/p95, max; long format) to this file")
+    p.add_argument("--job-ensemble-csv", type=str, default=None, metavar="PATH",
+                   help="write, per finish window and for the whole run, statistics of every DC's job counts and mean "
+                        "latencies per job type over all replicas (long format), and per-DC latency quantiles, to this file")
+    p.add_argument("--job-ensemble-bin", type=float, default=None, metavar="SECONDS",
+                   help="finish-window width of --job-ensemble-csv (default: --log-interval)")
     p.add_argument("--gpus", type=int, default=1,
                    help="shard the replicas over this many GPUs of the node (one process per GPU; the only collective is "
                         "the all-reduce of the end-of-run statistics over NCCL).  Under torchrun the world size wins.")
@@ -94,7 +99,8 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         fixed_freq=args.fixed_freq, logger=get_logger(log_dir=out_dir),
         replicas=args.replicas if replicas is None else replicas, first_replica_id=first_replica_id,
         device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
-        cluster_ensemble=args.ensemble_csv is not None)
+        cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
+        job_ensemble_bin=args.job_ensemble_bin)
     return sim
 
 
@@ -129,6 +135,8 @@ def main(argv=None):
 def _write_ensemble(args, sim):
     if args.ensemble_csv:
         sim.cluster_ensemble.to_csv(args.ensemble_csv, [dc.name for dc in sim.dcs.values()])
+    if args.job_ensemble_csv:
+        sim.job_ensemble.to_csv(args.job_ensemble_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_latency_quantiles(stats, hist):
@@ -167,6 +175,8 @@ def _main_sharded(args, world, rank):
     first, count = sharding.shard(args.replicas, rank, world)
     if args.ensemble_csv and count == 0:
         raise SystemExit("--ensemble-csv needs at least one replica per rank")
+    if args.job_ensemble_csv and count == 0:
+        raise SystemExit("--job-ensemble-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:

@@ -59,7 +59,8 @@ class MultiIngressPaperSimulator:
                  num_fixed_gpus=1, fixed_freq=None,
                  # --- batched-engine additions (keyword only in spirit; defaults reproduce one trajectory) ---
                  replicas: int = 1, device: int = 0, first_replica_id: int = 0, write_logs: bool = True,
-                 cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False):
+                 cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
+                 job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -97,6 +98,11 @@ class MultiIngressPaperSimulator:
         # all ranks when torch.distributed runs: every rank's run() takes part in the all-reduces), ensemble.EnsembleResult
         self._want_ensemble = bool(cluster_ensemble)
         self.cluster_ensemble = None
+        # job_ensemble=True: after run(), per finish window of job_ensemble_bin seconds (None: log_interval) and for the
+        # whole run, statistics of every DC's job counts and mean latencies over all replicas (all ranks, as above),
+        # ensemble.JobEnsembleResult
+        self._want_job_ensemble, self._job_ensemble_bin = bool(job_ensemble), job_ensemble_bin
+        self.job_ensemble = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -147,7 +153,8 @@ class MultiIngressPaperSimulator:
         try:
             eng, summ = run_to_completion(self._flatten, self.replicas, self.rng_seed, self.first_replica_id, self.device,
                                           self.cuda_stream, configure=configure, while_running=while_running,
-                                          cluster_ensemble=self._want_ensemble)
+                                          cluster_ensemble=self._want_ensemble, job_ensemble=self._want_job_ensemble,
+                                          job_ensemble_bin=self._job_ensemble_bin)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -159,6 +166,9 @@ class MultiIngressPaperSimulator:
             if self._want_ensemble:
                 from ..ensemble import cluster_ensemble
                 self.cluster_ensemble = cluster_ensemble(eng)
+            if self._want_job_ensemble:
+                from ..ensemble import job_ensemble
+                self.job_ensemble = job_ensemble(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

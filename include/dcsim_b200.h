@@ -336,6 +336,42 @@ int dcsim_ensemble_moments(dcsim_t* h, double* dev_out);
 int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
                           uint64_t* dev_hist_out);
 
+/* Job-log ensemble: for EVERY replica, what its job_log.csv rows (simulator_paper_multi.py:820) add up to per finish
+ * window, DC and job type.  Window k of W = max(1, ceil(end_time / bin_s)) covers [k * bin_s, (k + 1) * bin_s); a job
+ * finishing at t goes to window min(floor(t / bin_s), W - 1) (f64; finishes at end_time and in the 1e-9 slack behind it
+ * fold into the last window), and every job also to row W, the whole run.  Per replica and cell two f64 sums, added in
+ * finish order: JOBS (count) and LAT_SUM (sum of finish - start, the latency_s column).  Device layout
+ * [W + 1][DCSIM_JENS_STORED][n_dc][2 jtypes][n_replicas] doubles, replica fastest (the reductions read it coalesced), and
+ * a per-DC job-latency histogram [n_replicas][n_dc][2][DCSIM_LAT_BINS] u32 (the bin rule of the batch histogram above;
+ * summed over DCs it is that histogram's row of the replica).  The reductions add a third, derived field: MEAN_LATENCY =
+ * LAT_SUM / JOBS, over the replicas with at least one job in the cell.  A replica whose status is not 0 counts in no
+ * column and no histogram. */
+enum {
+  DCSIM_JENS_JOBS = 0,         /* jobs finished in the cell */
+  DCSIM_JENS_LAT_SUM = 1,      /* sum of their latencies [s] */
+  DCSIM_JENS_STORED = 2,       /* fields the recorder stores per replica */
+  DCSIM_JENS_MEAN_LATENCY = 2, /* LAT_SUM / JOBS (reductions only) */
+  DCSIM_JENS_FIELDS = 3        /* fields of the reductions' columns */
+};
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  bin_s = 0: log_interval.
+ * DCSIM_E_INVALID when bin_s is negative or not finite, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when
+ * the buffers do not fit, DCSIM_E_STATE after the first advance. */
+int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s);
+/* W, the number of finish windows (0 = not enabled); the rows are W + 1. */
+int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out);
+/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][STORED][n_dc][2][n_replicas] doubles,
+ * `hist` [n_replicas][n_dc][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than its array is
+ * DCSIM_E_INVALID.  For tests and small batches. */
+int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
+/* Pass 1, per column (row, field, dc, jtype) over the valid replicas: dev_out = [4][(W + 1) * JENS_FIELDS * n_dc * 2]
+ * doubles {n, sum, min, max}, the same contract as dcsim_ensemble_moments.  Pass 2: as dcsim_ensemble_spread; JOBS is
+ * the integer field (unit bins when its range allows).  Both run on the handle's stream, with device pointers. */
+int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out);
+int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                              double* dev_m2_out, uint64_t* dev_hist_out);
+/* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
+int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
+
 /* Word source of the replicas' random streams (before the first advance of a batch; stays across dcsim_reset).
  *   DCSIM_RNG_PHILOX   (default) Philox4x32-10, key = base_seed + replica id: counter-based, no state.
  *   DCSIM_RNG_MT19937  CPython's own Mersenne Twister seeded like random.seed(base_seed + replica id)
