@@ -25,6 +25,7 @@ EXPORTS = (
     "dcsim_ensemble_moments", "dcsim_ensemble_spread",
     "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_job_ensemble_moments",
     "dcsim_job_ensemble_spread", "dcsim_fetch_dc_latency_histogram",
+    "dcsim_arrivals_compatible", "dcsim_create_shared", "dcsim_paired_moments", "dcsim_paired_spread",
 )
 
 _lib = None
@@ -118,6 +119,15 @@ def load():
         L.dcsim_job_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
         L.dcsim_fetch_dc_latency_histogram.restype = i32
         L.dcsim_fetch_dc_latency_histogram.argtypes = [vp, vp, C.c_size_t]
+    if hasattr(L, "dcsim_create_shared"):
+        L.dcsim_arrivals_compatible.restype = i32
+        L.dcsim_arrivals_compatible.argtypes = [vp, C.c_size_t, vp, C.c_size_t, C.POINTER(i32)]
+        L.dcsim_create_shared.restype = i32
+        L.dcsim_create_shared.argtypes = [vp, C.c_size_t, vp, C.POINTER(vp)]
+        L.dcsim_paired_moments.restype = i32
+        L.dcsim_paired_moments.argtypes = [vp, vp, u64, vp]
+        L.dcsim_paired_spread.restype = i32
+        L.dcsim_paired_spread.argtypes = [vp, vp, u64, vp, vp, vp, vp, vp]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

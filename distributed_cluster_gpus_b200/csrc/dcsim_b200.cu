@@ -11,8 +11,11 @@
  *   dcsim_reduce_kernel       [n_replicas][K] summaries -> DCSIM_AGG_K doubles (the only cross-GPU payload).
  *   dcsim_hist_reduce_kernel  per-replica job-latency histograms -> one [2][128] histogram (opt-in); the same for the
  *                             per-DC [n_dc][2][128] histograms of the job-log ensemble.
- *   dcsim_ens_*_kernel        the cluster-log and job-log ensembles (opt-in) -> per-column moments, then spread +
- *                             histograms.
+ *   dcsim_ens_*_kernel        the cluster-log and job-log ensembles (opt-in) and the paired comparison of two batches
+ *                             with the same keys -> per-column moments, then spread + histograms.
+ *
+ * Handles of one group (dcsim_create_shared) share the pre-pass's buffers and the merged lists it leaves: the arrival
+ * lists do not depend on the policy (dcsim_arrival_inputs_equal, dcsim_core.cuh).
  *
  * Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false (see __graft_entry__.build()).
  * -fmad=false matters: the reference is CPython float arithmetic, one rounding per operation.
@@ -199,6 +202,67 @@ struct dcsim_ens_job_src {
   __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JENS_FIELDS == DCSIM_JENS_JOBS; }
 };
 
+/* Paired comparison: column (metric, field) over replica r's summary rows of a base and a variant batch (the same keys).
+ * Counted when both rows have status 0 and the metric is defined in both; fields base, variant, variant - base,
+ * variant < base, variant > base (include/dcsim_b200.h DCSIM_PAIR_*). */
+struct dcsim_ens_pair_src {
+  const double* base;
+  const double* var;
+  int n_dc;
+  struct view {
+    const double* base;
+    const double* var;
+    int metric, field, n_dc;
+    __device__ __forceinline__ static bool value(const double* s, int metric, int n_dc, double& v) {
+      switch (metric) {
+        case DCSIM_PAIR_ENERGY_J: v = s[DCSIM_S_TOTAL_ENERGY_J]; return true;
+        case DCSIM_PAIR_ENERGY_PER_JOB_J:
+          if (!(s[DCSIM_S_JOBS_FINISHED] > 0.0)) return false;
+          v = s[DCSIM_S_TOTAL_ENERGY_J] / s[DCSIM_S_JOBS_FINISHED]; return true;
+        case DCSIM_PAIR_JOBS_INF: v = s[DCSIM_S_FIN_INF]; return true;
+        case DCSIM_PAIR_JOBS_TRN: v = s[DCSIM_S_FIN_TRN]; return true;
+        case DCSIM_PAIR_MEAN_LAT_INF_S:
+          if (!(s[DCSIM_S_FIN_INF] > 0.0)) return false;
+          v = s[DCSIM_S_LAT_SUM_INF] / s[DCSIM_S_FIN_INF]; return true;
+        case DCSIM_PAIR_MEAN_LAT_TRN_S:
+          if (!(s[DCSIM_S_FIN_TRN] > 0.0)) return false;
+          v = s[DCSIM_S_LAT_SUM_TRN] / s[DCSIM_S_FIN_TRN]; return true;
+        case DCSIM_PAIR_UNFINISHED: {
+          double u = 0.0;
+          for (int d = 0; d < n_dc; ++d) {
+            const double* g = s + DCSIM_S_DC0 + d * DCSIM_S_DC_STRIDE;
+            u += g[DCSIM_SD_Q_INF] + g[DCSIM_SD_Q_TRN] + g[DCSIM_SD_RUNNING];
+          }
+          v = u; return true;
+        }
+        default: v = s[DCSIM_S_DC0 + (metric - DCSIM_PAIR_DC_ENERGY_J) * DCSIM_S_DC_STRIDE + DCSIM_SD_ENERGY_J]; return true;
+      }
+    }
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      const double* b = base + r * DCSIM_SUMMARY_K;
+      const double* x = var + r * DCSIM_SUMMARY_K;
+      if (b[DCSIM_S_STATUS] != 0.0 || x[DCSIM_S_STATUS] != 0.0) return false;
+      double vb, vx;
+      if (!value(b, metric, n_dc, vb) || !value(x, metric, n_dc, vx)) return false;
+      switch (field) {
+        case DCSIM_PAIR_BASE: v = vb; break;
+        case DCSIM_PAIR_VARIANT: v = vx; break;
+        case DCSIM_PAIR_DIFF: v = vx - vb; break;
+        case DCSIM_PAIR_LOWER: v = vx < vb ? 1.0 : 0.0; break;
+        default: v = vx > vb ? 1.0 : 0.0; break;
+      }
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const {
+    return view{base, var, (int)(col / DCSIM_PAIR_FIELDS), (int)(col % DCSIM_PAIR_FIELDS), n_dc};
+  }
+  __device__ __forceinline__ bool integral(uint64_t col) const {
+    const int metric = (int)(col / DCSIM_PAIR_FIELDS), field = (int)(col % DCSIM_PAIR_FIELDS);
+    return field >= DCSIM_PAIR_LOWER || metric == DCSIM_PAIR_JOBS_INF || metric == DCSIM_PAIR_JOBS_TRN || metric == DCSIM_PAIR_UNFINISHED;
+  }
+};
+
 __device__ __forceinline__ double dcsim_ens_min(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double dcsim_ens_max(double a, double b) { return b > a ? b : a; }
 
@@ -284,13 +348,54 @@ __global__ void __launch_bounds__(DCSIM_ENS_THREADS) dcsim_ens_spread_kernel(con
 /* ================================================================================================
  * C-ABI
  * ============================================================================================== */
+/* What the handles of one group share: the arrival pre-pass's buffers and the merged lists it leaves, the replica keys,
+ * the RNG kind and the stream every launch of the group goes to (so prepare -> advances -> reset -> prepare stay in
+ * stream order).  A handle made by dcsim_create owns a group of one; dcsim_create_shared adds members whose specs have
+ * the same arrival inputs (dcsim_arrival_inputs_equal).  Released with the last handle. */
+struct dcsim_group {
+  int refs;
+  int device;
+  dcsim_spec_t spec; /* the owner's: the pre-pass runs with it */
+  uint64_t n_replicas, seed0;
+  uint64_t generation; /* bumped by every reset of the owner */
+  cudaStream_t stream, own_stream;
+  int arrivals_ready;
+  int rng_kind;
+  uint32_t cap_arr;
+  double max_transfer;
+  double* d_arr_t;
+  double* d_arr_raw;
+  uint32_t* d_arr_meta;
+  uint32_t* d_arr_pred;
+  double* d_arr_tx;
+  uint32_t* d_arr_fin;
+  double* d_ml_t;
+  double* d_ml_aux;
+  uint32_t* d_ml_meta;
+  dcsim_arrhdr_t* d_arr_hdr;
+  uint32_t* d_mt; /* [624][n_replicas] Mersenne Twister states, rng_kind == DCSIM_RNG_MT19937 only */
+};
+
+static void group_release(dcsim_group* g) {
+  if (!g || --g->refs > 0) return;
+  cudaSetDevice(g->device);
+  if (g->stream) cudaStreamSynchronize(g->stream);
+  cudaFree(g->d_arr_t); cudaFree(g->d_arr_raw); cudaFree(g->d_arr_meta); cudaFree(g->d_arr_pred); cudaFree(g->d_arr_tx);
+  cudaFree(g->d_arr_fin); cudaFree(g->d_ml_t); cudaFree(g->d_ml_aux); cudaFree(g->d_ml_meta); cudaFree(g->d_arr_hdr);
+  cudaFree(g->d_mt);
+  if (g->own_stream) cudaStreamDestroy(g->own_stream);
+  delete g;
+}
+
 struct dcsim {
   dcsim_spec_t spec;
   dcsim_layout_t L;
-  uint64_t n_replicas, seed0;
+  dcsim_group* g;      /* arrival lists, keys, RNG kind, stream (shared with the rest of the group) */
+  int member;          /* 1: made by dcsim_create_shared (owns neither keys nor stream) */
+  uint64_t generation; /* the group generation this handle's batch was (re)set for */
+  uint64_t n_replicas;
   int device, sm_count, warps_per_cta, ctas, smem_bytes, regs, resident_warps;
   int lanes; /* lanes per replica of the advance kernel picked for this handle: 32, 16 or 8 */
-  cudaStream_t stream, own_stream;
   char* d_state;
   char* d_queues;
   double* d_summary;
@@ -307,20 +412,8 @@ struct dcsim {
   int want_job_log;                   /* layout the NEXT batch needs; applied lazily by ensure_layout() */
   int64_t trace_replica, log_replica;
   int launches;
-  int arrivals_ready, mode; /* mode: DCSIM_MODE_* of the advance kernel for this handle's layout */
-  double* d_arr_t;
-  double* d_arr_raw;
-  uint32_t* d_arr_meta;
-  uint32_t* d_arr_pred;
-  double* d_arr_tx;
-  uint32_t* d_arr_fin;
-  double* d_ml_t;
-  double* d_ml_aux;
-  uint32_t* d_ml_meta;
-  dcsim_arrhdr_t* d_arr_hdr;
-  double max_transfer;
+  int mode; /* DCSIM_MODE_* of the advance kernel for this handle's layout */
   uint32_t* d_hist;
-  uint32_t* d_mt; /* [624][n_replicas] Mersenne Twister states, rng_kind == DCSIM_RNG_MT19937 only */
   double* d_ens;       /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble (opt-in) */
   uint32_t* d_ens_nlog; /* [n_replicas] ticks each replica recorded, + 1 word: the largest DCSIM_S_EV_LOG */
   uint32_t ens_cap;
@@ -330,8 +423,6 @@ struct dcsim {
   unsigned long long* d_jens_hist_out; /* [n_dc][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_latency_histogram */
   double jens_bin;
   uint64_t jens_windows;
-  int rng_kind;
-  uint32_t cap_arr;
   unsigned long long events_seen;
   char err[512];
 };
@@ -479,15 +570,17 @@ static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
   dcsim_make_layout(&h->spec, &L, job_log);
   if (L.lean == h->L.lean) return DCSIM_OK;
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
   CUDA_TRY(h, size_launch(h));
   if (h->d_state) { cudaFree(h->d_state); h->d_state = NULL; }
   const size_t state_bytes = (size_t)h->n_replicas * (size_t)h->L.total_bytes;
   CUDA_TRY(h, cudaMalloc(&h->d_state, state_bytes));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, state_bytes, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, state_bytes, h->g->stream));
   return DCSIM_OK;
 }
+
+static int create_handle(const dcsim_spec_t* sp, dcsim_group* g, int member, dcsim_t** out);
 
 int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, uint64_t base_seed,
                  uint64_t first_replica_id, int device, dcsim_t** out) {
@@ -503,23 +596,72 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
   int rc = validate_spec(&sp);
   if (rc != DCSIM_OK) return rc;
 
+  dcsim_group* g = new (std::nothrow) dcsim_group();
+  if (!g) return set_err(NULL, DCSIM_E_NOMEM, "create: host allocation failed%s%lld");
+  memset(g, 0, sizeof(*g));
+  g->refs = 1;
+  g->device = device;
+  g->spec = sp;
+  g->n_replicas = n_replicas;
+  g->seed0 = base_seed + first_replica_id;
+  g->cap_arr = (uint32_t)(sp.cap_arrivals > 0 ? sp.cap_arrivals : 16384);
+  for (int i = 0; i < sp.n_ing; ++i)
+    for (int d = 0; d < sp.n_dc; ++d)
+      for (int jt = 0; jt < 2; ++jt) {
+        const double v = sp.transfer_s[i][d][jt];
+        if (v == v && v < 1e300 && v > g->max_transfer) g->max_transfer = v; /* finite ones only */
+      }
+
+#define GROUP_TRY(call)                                                                   \
+  do {                                                                                    \
+    cudaError_t e_ = (call);                                                              \
+    if (e_ != cudaSuccess) {                                                              \
+      rc = set_err(NULL, e_ == cudaErrorMemoryAllocation ? DCSIM_E_NOMEM : DCSIM_E_CUDA,  \
+                   "CUDA error in create: %s (line %lld)", cudaGetErrorString(e_), (long long)__LINE__); \
+      group_release(g);                                                                   \
+      return rc;                                                                          \
+    }                                                                                     \
+  } while (0)
+
+  GROUP_TRY(cudaSetDevice(device));
+  GROUP_TRY(cudaStreamCreateWithFlags(&g->own_stream, cudaStreamNonBlocking));
+  g->stream = g->own_stream;
+  {
+    const size_t ne = (size_t)n_replicas * (size_t)g->cap_arr;
+    GROUP_TRY(cudaMalloc(&g->d_arr_t, ne * sizeof(double)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_raw, ne * sizeof(double)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_meta, ne * sizeof(uint32_t)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_pred, ne * sizeof(uint32_t)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_tx, ne * sizeof(double)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_fin, ne * sizeof(uint32_t)));
+    GROUP_TRY(cudaMalloc(&g->d_ml_t, 2 * ne * sizeof(double)));
+    GROUP_TRY(cudaMalloc(&g->d_ml_aux, 2 * ne * sizeof(double)));
+    GROUP_TRY(cudaMalloc(&g->d_ml_meta, 2 * ne * sizeof(uint32_t)));
+    GROUP_TRY(cudaMalloc(&g->d_arr_hdr, (size_t)n_replicas * sizeof(dcsim_arrhdr_t)));
+  }
+#undef GROUP_TRY
+  rc = create_handle(&sp, g, /*member=*/0, out);
+  group_release(g); /* the handle holds its own reference (or, on failure, none) */
+  return rc;
+}
+
+/* A handle of group `g` (takes a reference on success): its own state block, queues, summary and scratch. */
+static int create_handle(const dcsim_spec_t* sp, dcsim_group* g, int member, dcsim_t** out) {
+  int rc = DCSIM_OK;
   dcsim_t* h = new (std::nothrow) dcsim();
   if (!h) return set_err(NULL, DCSIM_E_NOMEM, "create: host allocation failed%s%lld");
   memset(h, 0, sizeof(*h));
-  h->spec = sp;
+  h->spec = *sp;
   dcsim_make_layout(&h->spec, &h->L, /*job_log=*/0);
-  h->cap_arr = (uint32_t)(h->spec.cap_arrivals > 0 ? h->spec.cap_arrivals : 16384);
-  for (int i = 0; i < h->spec.n_ing; ++i)
-    for (int d = 0; d < h->spec.n_dc; ++d)
-      for (int jt = 0; jt < 2; ++jt) {
-        const double v = h->spec.transfer_s[i][d][jt];
-        if (v == v && v < 1e300 && v > h->max_transfer) h->max_transfer = v; /* finite ones only */
-      }
-  h->n_replicas = n_replicas;
-  h->seed0 = base_seed + first_replica_id;
-  h->device = device;
+  h->g = g;
+  ++g->refs;
+  h->member = member;
+  h->generation = g->generation;
+  h->n_replicas = g->n_replicas;
+  h->device = g->device;
   h->trace_replica = -1;
   h->log_replica = -1;
+  const uint64_t n_replicas = h->n_replicas;
 
 #define CREATE_TRY(call)                                                                  \
   do {                                                                                    \
@@ -532,11 +674,9 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
     }                                                                                     \
   } while (0)
 
-  CREATE_TRY(cudaSetDevice(device));
-  CREATE_TRY(cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, device));
+  CREATE_TRY(cudaSetDevice(h->device));
+  CREATE_TRY(cudaDeviceGetAttribute(&h->sm_count, cudaDevAttrMultiProcessorCount, h->device));
   CREATE_TRY(size_launch(h));
-  CREATE_TRY(cudaStreamCreateWithFlags(&h->own_stream, cudaStreamNonBlocking));
-  h->stream = h->own_stream;
   const size_t state_bytes = (size_t)n_replicas * (size_t)h->L.total_bytes;
   if (h->L.queue_bytes >= (1ull << 32)) /* the event loop addresses inside one replica's FIFOs with 32 bits */
   {
@@ -548,56 +688,86 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
   CREATE_TRY(cudaMalloc(&h->d_state, state_bytes));
   CREATE_TRY(cudaMalloc(&h->d_queues, queue_bytes ? queue_bytes : 16));
   CREATE_TRY(cudaMalloc(&h->d_summary, (size_t)n_replicas * DCSIM_SUMMARY_K * sizeof(double)));
-  {
-    const size_t ne = (size_t)n_replicas * (size_t)h->cap_arr;
-    CREATE_TRY(cudaMalloc(&h->d_arr_t, ne * sizeof(double)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_raw, ne * sizeof(double)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_meta, ne * sizeof(uint32_t)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_pred, ne * sizeof(uint32_t)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_tx, ne * sizeof(double)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_fin, ne * sizeof(uint32_t)));
-    CREATE_TRY(cudaMalloc(&h->d_ml_t, 2 * ne * sizeof(double)));
-    CREATE_TRY(cudaMalloc(&h->d_ml_aux, 2 * ne * sizeof(double)));
-    CREATE_TRY(cudaMalloc(&h->d_ml_meta, 2 * ne * sizeof(uint32_t)));
-    CREATE_TRY(cudaMalloc(&h->d_arr_hdr, (size_t)n_replicas * sizeof(dcsim_arrhdr_t)));
-  }
   CREATE_TRY(cudaMalloc(&h->d_events, sizeof(unsigned long long)));
   CREATE_TRY(cudaMalloc(&h->d_agg, DCSIM_AGG_K * sizeof(double)));
   CREATE_TRY(cudaMalloc(&h->d_hist_out, 2 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
   CREATE_TRY(cudaMalloc(&h->d_counts, 4 * sizeof(uint32_t)));
-  CREATE_TRY(cudaMemsetAsync(h->d_state, 0, state_bytes, h->stream)); /* hdr.initialized == 0 => fresh replica */
-  CREATE_TRY(cudaMemsetAsync(h->d_summary, 0, (size_t)n_replicas * DCSIM_SUMMARY_K * sizeof(double), h->stream));
-  CREATE_TRY(cudaMemsetAsync(h->d_events, 0, sizeof(unsigned long long), h->stream));
-  CREATE_TRY(cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->stream));
-  CREATE_TRY(cudaStreamSynchronize(h->stream));
+  CREATE_TRY(cudaMemsetAsync(h->d_state, 0, state_bytes, h->g->stream)); /* hdr.initialized == 0 => fresh replica */
+  CREATE_TRY(cudaMemsetAsync(h->d_summary, 0, (size_t)n_replicas * DCSIM_SUMMARY_K * sizeof(double), h->g->stream));
+  CREATE_TRY(cudaMemsetAsync(h->d_events, 0, sizeof(unsigned long long), h->g->stream));
+  CREATE_TRY(cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->g->stream));
+  CREATE_TRY(cudaStreamSynchronize(h->g->stream));
 #undef CREATE_TRY
   *out = h;
   return DCSIM_OK;
 }
 
+/* A blob of the right size holding a valid spec, copied into *sp. */
+static int spec_from_blob(const void* spec_blob, size_t spec_bytes, dcsim_spec_t* sp) {
+  if (!spec_blob || spec_bytes != sizeof(dcsim_spec_t))
+    return set_err(NULL, DCSIM_E_INVALID, "spec blob must be %s%lld bytes", "", (long long)sizeof(dcsim_spec_t));
+  memcpy(sp, spec_blob, sizeof(*sp));
+  return validate_spec(sp);
+}
+
+int dcsim_arrivals_compatible(const void* spec_a, size_t a_bytes, const void* spec_b, size_t b_bytes, int* equal_out) {
+  if (!equal_out) return set_err(NULL, DCSIM_E_INVALID, "arrivals_compatible: equal_out is NULL%s%lld");
+  *equal_out = 0;
+  dcsim_spec_t a, b;
+  int rc = spec_from_blob(spec_a, a_bytes, &a);
+  if (rc == DCSIM_OK) rc = spec_from_blob(spec_b, b_bytes, &b);
+  if (rc != DCSIM_OK) return DCSIM_E_INVALID;
+  *equal_out = dcsim_arrival_inputs_equal(&a, &b) ? 1 : 0;
+  return DCSIM_OK;
+}
+
+int dcsim_create_shared(const void* spec_blob, size_t spec_bytes, dcsim_t* owner, dcsim_t** out) {
+  if (!out) return set_err(NULL, DCSIM_E_INVALID, "create_shared: out is NULL%s%lld");
+  *out = NULL;
+  if (!owner) return set_err(NULL, DCSIM_E_INVALID, "create_shared: owner is NULL%s%lld");
+  if (owner->member) return set_err(NULL, DCSIM_E_INVALID, "create_shared: the owner is itself a member of a group%s%lld");
+  dcsim_spec_t sp;
+  int rc = spec_from_blob(spec_blob, spec_bytes, &sp);
+  if (rc != DCSIM_OK) return rc;
+  const char* field = NULL;
+  if (!dcsim_arrival_inputs_equal(&owner->g->spec, &sp, &field)) {
+    snprintf(g_create_err, sizeof(g_create_err), "create_shared: the spec draws other arrivals than the owner's (%s differs)", field);
+    return DCSIM_E_INVALID;
+  }
+  return create_handle(&sp, owner->g, /*member=*/1, out);
+}
+
 int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
   if (!h) return DCSIM_E_INVALID;
+  if (h->member && base_seed + first_replica_id != h->g->seed0)
+    return set_err(h, DCSIM_E_INVALID, "reset: a member must pass the owner's keys (base_seed + first_replica_id = %s%lld)", "",
+                   (long long)h->g->seed0);
   CUDA_TRY(h, cudaSetDevice(h->device));
   /* hdr.initialized == 0 marks a fresh replica; the FIFOs need no clearing (head == tail == 0) */
-  CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, (size_t)h->n_replicas * (size_t)h->L.total_bytes, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->stream));
-  if (h->d_hist) CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t), h->stream));
-  if (h->d_ens) CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, ens_bytes(h, h->ens_cap), h->stream)); /* NaN: not recorded */
+  CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, (size_t)h->n_replicas * (size_t)h->L.total_bytes, h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->g->stream));
+  if (h->d_hist) CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t), h->g->stream));
+  if (h->d_ens) CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, ens_bytes(h, h->ens_cap), h->g->stream)); /* NaN: not recorded */
   if (h->d_jens) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, (h->jens_windows + 1) * jens_row_bytes(h), h->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, (h->jens_windows + 1) * jens_row_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
   }
-  h->seed0 = base_seed + first_replica_id;
-  h->arrivals_ready = 0;
+  if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
+    h->g->seed0 = base_seed + first_replica_id;
+    h->g->arrivals_ready = 0;
+    ++h->g->generation;
+  }
+  h->generation = h->g->generation;
   h->launches = 0; /* a reset batch is "fresh": recorders may be re-targeted before its first advance */
   return DCSIM_OK;
 }
 
 int dcsim_set_stream(dcsim_t* h, void* cuda_stream) {
   if (!h) return DCSIM_E_INVALID;
+  if (h->member) return set_err(h, DCSIM_E_STATE, "set_stream on a member: the group's stream is the owner's%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
-  h->stream = cuda_stream ? (cudaStream_t)cuda_stream : h->own_stream;
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  h->g->stream = cuda_stream ? (cudaStream_t)cuda_stream : h->g->own_stream;
   return DCSIM_OK;
 }
 
@@ -647,62 +817,75 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->rec.trace_cap = h->trace_cap; P->rec.jobs_cap = h->jobs_cap; P->rec.cluster_cap = h->cluster_cap;
   P->rec.trace_replica = h->trace_replica; P->rec.log_replica = h->log_replica;
   P->n_replicas = h->n_replicas;
-  P->seed0 = h->seed0;
+  P->seed0 = h->g->seed0;
   P->max_events = max_events;
   P->budget32 = (max_events == 0ull || max_events > 0xfffffffeull) ? 0xffffffffu : (uint32_t)max_events;
   P->state = h->d_state; P->queues = h->d_queues; P->summary = h->d_summary;
   P->end_eps = h->spec.end_time + 1e-9; /* SIM:161 */
-  P->arr_t = h->d_arr_t; P->arr_raw = h->d_arr_raw; P->arr_meta = h->d_arr_meta; P->arr_pred = h->d_arr_pred;
-  P->arr_tx = h->d_arr_tx; P->arr_fin = h->d_arr_fin;
-  P->ml_t = h->d_ml_t; P->ml_aux = h->d_ml_aux; P->ml_meta = h->d_ml_meta;
-  P->arr_hdr = h->d_arr_hdr; P->cap_arr = h->cap_arr;
-  P->max_transfer = h->max_transfer;
+  P->arr_t = h->g->d_arr_t; P->arr_raw = h->g->d_arr_raw; P->arr_meta = h->g->d_arr_meta; P->arr_pred = h->g->d_arr_pred;
+  P->arr_tx = h->g->d_arr_tx; P->arr_fin = h->g->d_arr_fin;
+  P->ml_t = h->g->d_ml_t; P->ml_aux = h->g->d_ml_aux; P->ml_meta = h->g->d_ml_meta;
+  P->arr_hdr = h->g->d_arr_hdr; P->cap_arr = h->g->cap_arr;
+  P->max_transfer = h->g->max_transfer;
   P->lat_hist = h->d_hist;
-  P->mt_state = h->d_mt;
+  P->mt_state = h->g->d_mt;
   P->ens = h->d_ens; P->ens_cap = h->ens_cap;
   P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
   P->finish_rec = (P->lat_hist || P->jens) ? 1u : 0u;
 }
 
+/* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */
+static int check_generation(dcsim_t* h) {
+  if (h->generation == h->g->generation) return DCSIM_OK;
+  return set_err(h, DCSIM_E_STATE, "arrival source was reset: reset this member with the owner's keys%s%lld");
+}
+
 int dcsim_prepare(dcsim_t* h) {
   if (!h) return DCSIM_E_INVALID;
+  int rc = check_generation(h);
+  if (rc != DCSIM_OK) return rc;
   CUDA_TRY(h, cudaSetDevice(h->device));
   if (h->launches == 0) { const int rc0 = relayout(h, h->want_job_log); if (rc0 != DCSIM_OK) return rc0; }
-  if (h->arrivals_ready) return DCSIM_OK;
+  if (h->g->arrivals_ready) return DCSIM_OK;
   dcsim_kparams_t P;
   fill_kparams(h, &P, 0);
+  /* the owner's launch parameters: its spec and the layout it implies (the merge checks the seq ring against it); both
+   * give what this handle's would (dcsim_arrival_inputs_equal, dcsim_create_shared) */
+  P.spec = h->g->spec;
+  dcsim_make_layout(&h->g->spec, &P.L, /*job_log=*/0);
   const int nb = (int)((h->n_replicas + DCSIM_ARRIVALS_THREADS - 1) / DCSIM_ARRIVALS_THREADS);
   const size_t scratch = dcsim_arrivals_scratch_bytes(h->spec.n_ing); /* 52 KB at 8 ingresses: above the 48 KB default */
-  if (h->rng_kind == DCSIM_RNG_MT19937) {
+  if (h->g->rng_kind == DCSIM_RNG_MT19937) {
     CUDA_TRY(h, cudaFuncSetAttribute(dcsim_arrivals_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scratch));
-    dcsim_arrivals_kernel<true><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
+    dcsim_arrivals_kernel<true><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->g->stream>>>(P);
   } else {
     CUDA_TRY(h, cudaFuncSetAttribute(dcsim_arrivals_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scratch));
-    dcsim_arrivals_kernel<false><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->stream>>>(P);
+    dcsim_arrivals_kernel<false><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->g->stream>>>(P);
   }
   CUDA_TRY(h, cudaGetLastError());
   const int wpb = DCSIM_MERGE_THREADS / 32;
-  dcsim_merge_kernel<<<(int)((h->n_replicas + wpb - 1) / wpb), DCSIM_MERGE_THREADS, 0, h->stream>>>(P);
+  dcsim_merge_kernel<<<(int)((h->n_replicas + wpb - 1) / wpb), DCSIM_MERGE_THREADS, 0, h->g->stream>>>(P);
   CUDA_TRY(h, cudaGetLastError());
-  h->arrivals_ready = 1;
+  h->g->arrivals_ready = 1;
   h->launches += 2;
   return DCSIM_OK;
 }
 
 int dcsim_advance(dcsim_t* h, uint64_t max_events_per_replica, uint64_t* total_events_out) {
   if (!h) return DCSIM_E_INVALID;
+  if (check_generation(h) != DCSIM_OK) return DCSIM_E_STATE;
   CUDA_TRY(h, cudaSetDevice(h->device));
   if (h->launches == 0) { const int rc0 = relayout(h, h->want_job_log); if (rc0 != DCSIM_OK) return rc0; }
-  int rc = dcsim_prepare(h); /* once per (re)seeded batch: the arrival lists of all replicas */
+  int rc = dcsim_prepare(h); /* once per (re)seeded batch of the group: the arrival lists of all replicas */
   if (rc != DCSIM_OK) return rc;
   dcsim_kparams_t P;
   fill_kparams(h, &P, max_events_per_replica);
-  CUDA_TRY(h, adv_launch_for(h->lanes)(&P, h->d_events, h->L.cap_stale != 0, h->mode, h->ctas, h->warps_per_cta * 32, h->smem_bytes, h->stream));
+  CUDA_TRY(h, adv_launch_for(h->lanes)(&P, h->d_events, h->L.cap_stale != 0, h->mode, h->ctas, h->warps_per_cta * 32, h->smem_bytes, h->g->stream));
   h->launches++;
   if (total_events_out) {
     unsigned long long total = 0;
-    CUDA_TRY(h, cudaMemcpyAsync(&total, h->d_events, sizeof(total), cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(&total, h->d_events, sizeof(total), cudaMemcpyDeviceToHost, h->g->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
     *total_events_out = (uint64_t)(total - h->events_seen);
     h->events_seen = total;
   }
@@ -715,8 +898,8 @@ int dcsim_fetch_summary(dcsim_t* h, double* out, size_t out_bytes) {
   if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_summary: buffer too small (need %s%lld bytes)", "", (long long)need);
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "fetch_summary before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_summary, need, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_summary, need, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
@@ -727,8 +910,8 @@ int dcsim_fetch_summary_host(dcsim_t* h, const double** host_ptr_out) {
   CUDA_TRY(h, cudaSetDevice(h->device));
   const size_t need = (size_t)h->n_replicas * DCSIM_SUMMARY_K * sizeof(double);
   if (!h->h_summary_pinned) CUDA_TRY(h, cudaHostAlloc(&h->h_summary_pinned, need, cudaHostAllocDefault));
-  CUDA_TRY(h, cudaMemcpyAsync(h->h_summary_pinned, h->d_summary, need, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(h->h_summary_pinned, h->d_summary, need, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   *host_ptr_out = h->h_summary_pinned;
   return DCSIM_OK;
 }
@@ -748,8 +931,8 @@ int dcsim_all_done(dcsim_t* h, int* done_out) {
   int rc = dcsim_reduce_summary(h, agg);
   double host[DCSIM_AGG_K];
   if (rc == DCSIM_OK) {
-    cudaError_t e = cudaMemcpyAsync(host, agg, sizeof(host), cudaMemcpyDeviceToHost, h->stream);
-    if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+    cudaError_t e = cudaMemcpyAsync(host, agg, sizeof(host), cudaMemcpyDeviceToHost, h->g->stream);
+    if (e == cudaSuccess) e = cudaStreamSynchronize(h->g->stream);
     if (e != cudaSuccess) rc = set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
   }
   if (rc != DCSIM_OK) return rc;
@@ -762,10 +945,10 @@ int dcsim_reduce_summary(dcsim_t* h, double* dev_out) {
   if (!h || !dev_out) return DCSIM_E_INVALID;
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "reduce_summary before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(dev_out, 0, DCSIM_AGG_K * sizeof(double), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(dev_out, 0, DCSIM_AGG_K * sizeof(double), h->g->stream));
   int blocks = (int)((h->n_replicas + 255) / 256);
   if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_reduce_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, dev_out);
+  dcsim_reduce_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, dev_out);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
 }
@@ -789,21 +972,22 @@ int dcsim_allreduce_summary(dcsim_t* h, void* nccl_comm, double* out) {
   }
   int rc = dcsim_reduce_summary(h, h->d_agg);
   if (rc != DCSIM_OK) return rc;
-  const int nccl_rc = fn(h->d_agg, h->d_agg, DCSIM_AGG_K, /*ncclFloat64*/ 8, /*ncclSum*/ 0, nccl_comm, h->stream);
+  const int nccl_rc = fn(h->d_agg, h->d_agg, DCSIM_AGG_K, /*ncclFloat64*/ 8, /*ncclSum*/ 0, nccl_comm, h->g->stream);
   if (nccl_rc != 0) return set_err(h, DCSIM_E_CUDA, "allreduce_summary: ncclAllReduce failed with code %s%lld", "", (long long)nccl_rc);
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_agg, DCSIM_AGG_K * sizeof(double), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_agg, DCSIM_AGG_K * sizeof(double), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
 int dcsim_set_rng(dcsim_t* h, int rng_kind) {
   if (!h) return DCSIM_E_INVALID;
   if (rng_kind != DCSIM_RNG_PHILOX && rng_kind != DCSIM_RNG_MT19937) return set_err(h, DCSIM_E_INVALID, "set_rng: unknown rng kind %s%lld", "", (long long)rng_kind);
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "set_rng must precede the first advance%s%lld");
+  if (h->member) return set_err(h, DCSIM_E_STATE, "set_rng on a member: the group's RNG kind is the owner's%s%lld");
+  if (h->launches || h->g->arrivals_ready) return set_err(h, DCSIM_E_STATE, "set_rng must precede the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  if (rng_kind == DCSIM_RNG_MT19937 && !h->d_mt)
-    CUDA_TRY(h, cudaMalloc(&h->d_mt, (size_t)h->n_replicas * DCSIM_MT_N * sizeof(uint32_t)));
-  h->rng_kind = rng_kind;
+  if (rng_kind == DCSIM_RNG_MT19937 && !h->g->d_mt)
+    CUDA_TRY(h, cudaMalloc(&h->g->d_mt, (size_t)h->n_replicas * DCSIM_MT_N * sizeof(uint32_t)));
+  h->g->rng_kind = rng_kind;
   return DCSIM_OK;
 }
 
@@ -814,7 +998,7 @@ int dcsim_enable_latency_histogram(dcsim_t* h) {
   CUDA_TRY(h, cudaSetDevice(h->device));
   const size_t bytes = (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t);
   CUDA_TRY(h, cudaMalloc(&h->d_hist, bytes));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, bytes, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, bytes, h->g->stream));
   return DCSIM_OK;
 }
 
@@ -826,15 +1010,15 @@ int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "fetch_latency_histogram before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
   unsigned long long* d_out = h->d_hist_out;
-  cudaError_t e = cudaMemsetAsync(d_out, 0, need, h->stream);
+  cudaError_t e = cudaMemsetAsync(d_out, 0, need, h->g->stream);
   if (e == cudaSuccess) {
     int blocks = 8 * h->sm_count;
     if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
-    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->stream>>>(h->d_hist, h->n_replicas, 2 * DCSIM_LAT_BINS, NULL, d_out);
+    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->g->stream>>>(h->d_hist, h->n_replicas, 2 * DCSIM_LAT_BINS, NULL, d_out);
     e = cudaGetLastError();
   }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, need, cudaMemcpyDeviceToHost, h->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->stream);
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, need, cudaMemcpyDeviceToHost, h->g->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->g->stream);
   if (e != cudaSuccess) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
   return DCSIM_OK;
 }
@@ -857,7 +1041,7 @@ int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks) {
                    (long long)bytes);
   }
   h->ens_cap = ticks;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, bytes, h->stream)); /* NaN: not recorded */
+  CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, bytes, h->g->stream)); /* NaN: not recorded */
   return DCSIM_OK;
 }
 
@@ -872,14 +1056,14 @@ static int ens_counts(dcsim_t* h) {
   if (!h->d_ens) return set_err(h, DCSIM_E_STATE, "cluster ensemble not enabled (dcsim_enable_cluster_ensemble)%s%lld");
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "cluster ensemble read before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_ens_nlog + h->n_replicas, 0, sizeof(uint32_t), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_ens_nlog + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
   int blocks = (int)((h->n_replicas + 255) / 256);
   if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_EV_LOG, h->d_ens_nlog);
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_EV_LOG, h->d_ens_nlog);
   CUDA_TRY(h, cudaGetLastError());
   uint32_t most = 0u;
-  CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   if (most > h->ens_cap) {
     snprintf(h->err, sizeof(h->err), "cluster ensemble overflow: a replica recorded %u log ticks, capacity %u", most, h->ens_cap);
     return DCSIM_E_STATE;
@@ -895,8 +1079,8 @@ int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes) {
   size_t ticks = out_bytes / tick_bytes;
   if (ticks > h->ens_cap) ticks = h->ens_cap;
   if (ticks) {
-    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_ens, ticks * tick_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_ens, ticks * tick_bytes, cudaMemcpyDeviceToHost, h->g->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   }
   return DCSIM_OK;
 }
@@ -911,7 +1095,7 @@ int dcsim_ensemble_moments(dcsim_t* h, double* dev_out) {
   const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
   if (!n_cols) return DCSIM_OK;
   const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_out);
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
 }
@@ -925,9 +1109,44 @@ int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_
   const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
   if (!n_cols) return DCSIM_OK;
   const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
                                                                                     dev_m2_out, (unsigned long long*)dev_hist_out);
   CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+static int pair_check(dcsim_t* base, const double* dev_variant_summary, uint64_t n) {
+  if (!base || !dev_variant_summary) return DCSIM_E_INVALID;
+  if (n != base->n_replicas)
+    return set_err(base, DCSIM_E_INVALID, "paired reduction: n must be the base handle's replica count (%s%lld)", "", (long long)base->n_replicas);
+  if (!base->launches) return set_err(base, DCSIM_E_STATE, "paired reduction before the base handle's first advance%s%lld");
+  CUDA_TRY(base, cudaSetDevice(base->device));
+  return DCSIM_OK;
+}
+
+static uint64_t pair_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PAIR_DC_ENERGY_J + h->spec.n_dc) * DCSIM_PAIR_FIELDS; }
+
+int dcsim_paired_moments(dcsim_t* base, const double* dev_variant_summary, uint64_t n, double* dev_out) {
+  if (!dev_out) return DCSIM_E_INVALID;
+  const int rc = pair_check(base, dev_variant_summary, n);
+  if (rc != DCSIM_OK) return rc;
+  const uint64_t n_cols = pair_cols(base);
+  const dcsim_ens_pair_src src{base->d_summary, dev_variant_summary, base->spec.n_dc};
+  dcsim_ens_moments_kernel<<<ens_grid(base, n_cols), DCSIM_ENS_THREADS, 0, base->g->stream>>>(src, n, n_cols, dev_out);
+  CUDA_TRY(base, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_paired_spread(dcsim_t* base, const double* dev_variant_summary, uint64_t n, const double* dev_mean,
+                        const double* dev_lo, const double* dev_hi, double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = pair_check(base, dev_variant_summary, n);
+  if (rc != DCSIM_OK) return rc;
+  const uint64_t n_cols = pair_cols(base);
+  const dcsim_ens_pair_src src{base->d_summary, dev_variant_summary, base->spec.n_dc};
+  dcsim_ens_spread_kernel<<<ens_grid(base, n_cols), DCSIM_ENS_THREADS, 0, base->g->stream>>>(src, n, n_cols, dev_mean, dev_lo, dev_hi,
+                                                                                          dev_m2_out, (unsigned long long*)dev_hist_out);
+  CUDA_TRY(base, cudaGetLastError());
   return DCSIM_OK;
 }
 
@@ -958,8 +1177,8 @@ int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
     return set_err(h, DCSIM_E_NOMEM, "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)", "", need_ll);
   }
   h->jens_bin = bin; h->jens_windows = windows;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, rows_bytes, h->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, rows_bytes, h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
   return DCSIM_OK;
 }
 
@@ -974,10 +1193,10 @@ static int jens_status(dcsim_t* h) {
   if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "job ensemble not enabled (dcsim_enable_job_ensemble)%s%lld");
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "job ensemble read before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_status + h->n_replicas, 0, sizeof(uint32_t), h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_status + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
   int blocks = (int)((h->n_replicas + 255) / 256);
   if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_jens_status);
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_jens_status);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
 }
@@ -990,9 +1209,9 @@ int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32
   if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
     return set_err(h, DCSIM_E_INVALID, "fetch_job_ensemble: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
   CUDA_TRY(h, cudaSetDevice(h->device));
-  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jens, need_rows, cudaMemcpyDeviceToHost, h->stream));
-  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jens_hist, need_hist, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jens, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
+  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jens_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
@@ -1003,7 +1222,7 @@ int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out) {
   const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
   const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
   const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_out);
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
 }
@@ -1016,7 +1235,7 @@ int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* 
   const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
   const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
   const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
                                                                                     dev_m2_out, (unsigned long long*)dev_hist_out);
   CUDA_TRY(h, cudaGetLastError());
   return DCSIM_OK;
@@ -1029,14 +1248,14 @@ int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes
   if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_latency_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
   const int rc = jens_status(h);
   if (rc != DCSIM_OK) return rc;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist_out, 0, need, h->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist_out, 0, need, h->g->stream));
   int blocks = 8 * h->sm_count;
   if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
-  dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->stream>>>(h->d_jens_hist, h->n_replicas, row_len, h->d_jens_status,
+  dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->g->stream>>>(h->d_jens_hist, h->n_replicas, row_len, h->d_jens_status,
                                                                          h->d_jens_hist_out);
   CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_jens_hist_out, need, cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_jens_hist_out, need, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
@@ -1044,8 +1263,8 @@ int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {
   if (!h || !out3) return DCSIM_E_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
   uint32_t counts[4];
-  CUDA_TRY(h, cudaMemcpyAsync(counts, h->d_counts, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(counts, h->d_counts, sizeof(counts), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   out3[0] = counts[0]; out3[1] = counts[1]; out3[2] = counts[2];
   return DCSIM_OK;
 }
@@ -1057,13 +1276,13 @@ static int fetch_records(dcsim_t* h, const void* dev, size_t rec_bytes, uint32_t
   if (!dev) return DCSIM_OK;
   CUDA_TRY(h, cudaSetDevice(h->device));
   uint32_t counts[4];
-  CUDA_TRY(h, cudaMemcpyAsync(counts, h->d_counts, sizeof(counts), cudaMemcpyDeviceToHost, h->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(counts, h->d_counts, sizeof(counts), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   uint32_t n = counts[which] < dev_cap ? counts[which] : dev_cap;
   if (n > capacity) n = capacity;
   if (n && out) {
-    CUDA_TRY(h, cudaMemcpyAsync(out, dev, (size_t)n * rec_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->stream));
+    CUDA_TRY(h, cudaMemcpyAsync(out, dev, (size_t)n * rec_bytes, cudaMemcpyDeviceToHost, h->g->stream));
+    CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   }
   *n_out = n;
   return DCSIM_OK;
@@ -1090,7 +1309,7 @@ int dcsim_launch_info(dcsim_t* h, dcsim_launch_info_t* out) {
   out->hbm_bytes_queues = (uint64_t)h->n_replicas * h->L.queue_bytes;
   out->arrivals_prepass = 1;
   /* per arrival: pre-pass output 24 B + merge scratch 12 B + two list entries of 20 B */
-  out->hbm_bytes_arrivals = (uint64_t)h->n_replicas * ((uint64_t)h->cap_arr * 76ull + sizeof(dcsim_arrhdr_t));
+  out->hbm_bytes_arrivals = h->member ? 0ull : (uint64_t)h->n_replicas * ((uint64_t)h->g->cap_arr * 76ull + sizeof(dcsim_arrhdr_t));
   out->staging_mode = h->mode; out->state_block_bytes = h->L.total_bytes;
   out->staged_bytes_per_replica = h->warps_per_cta ? h->smem_bytes / (h->warps_per_cta * (32 / h->lanes)) : 0;
   out->lanes_per_replica = h->lanes;
@@ -1102,17 +1321,14 @@ const char* dcsim_last_error(const dcsim_t* h) { return h ? h->err : g_create_er
 void dcsim_destroy(dcsim_t* h) {
   if (!h) return;
   cudaSetDevice(h->device);
-  if (h->own_stream) { cudaStreamSynchronize(h->stream); }
+  if (h->g && h->g->stream) cudaStreamSynchronize(h->g->stream);
   cudaFree(h->d_state); cudaFree(h->d_queues); cudaFree(h->d_summary); cudaFree(h->d_events); cudaFree(h->d_counts);
   cudaFree(h->d_trace); cudaFree(h->d_jobs); cudaFree(h->d_cluster);
   cudaFree(h->d_hist); cudaFree(h->d_agg); cudaFree(h->d_hist_out);
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
-  cudaFree(h->d_mt);
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_status); cudaFree(h->d_jens_hist_out);
-  cudaFree(h->d_arr_t); cudaFree(h->d_arr_raw); cudaFree(h->d_arr_meta); cudaFree(h->d_arr_pred); cudaFree(h->d_arr_tx);
-  cudaFree(h->d_arr_fin); cudaFree(h->d_ml_t); cudaFree(h->d_ml_aux); cudaFree(h->d_ml_meta); cudaFree(h->d_arr_hdr);
-  if (h->own_stream) cudaStreamDestroy(h->own_stream);
+  group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }
 

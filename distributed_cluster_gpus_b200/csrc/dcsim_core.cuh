@@ -347,6 +347,14 @@ enum : int32_t {
 };
 
 /* Host-side: sizes the state block from the spec's capacities. */
+/* Entries of a replica's seq ring of in-flight transfers (see dcsim_make_layout): a power of two >= 2 * cap_xfer. */
+static inline int32_t dcsim_xring_entries(const dcsim_spec_t* sp) {
+  const int32_t cx = sp->cap_xfer > 0 ? sp->cap_xfer : 64;
+  int32_t ring = 8;
+  while (ring < 2 * cx) ring <<= 1;
+  return ring;
+}
+
 static inline void dcsim_make_layout(const dcsim_spec_t* sp, dcsim_layout_t* L, int job_log) {
   memset(L, 0, sizeof(*L));
   const bool bandit = sp->xfer_rule == DCSIM_START_BANDIT || sp->deq_rule == DCSIM_START_BANDIT;
@@ -354,7 +362,6 @@ static inline void dcsim_make_layout(const dcsim_spec_t* sp, dcsim_layout_t* L, 
   /* size (job_log.csv, cap re-timing), f (job_log.csv, bandit reward, cap) and jid (job_log.csv) of a running job
      are dead weight in the state block unless one of those readers exists: 60 -> 40 bytes per record. */
   L->lean = (job_log || bandit || cap) ? 0 : 1;
-  int32_t cx = sp->cap_xfer > 0 ? sp->cap_xfer : 64;
   int32_t cr = sp->cap_run > 0 ? sp->cap_run : 16;
   cr = (cr + 3) & ~3;
   L->cap_run = cr;
@@ -367,8 +374,7 @@ static inline void dcsim_make_layout(const dcsim_spec_t* sp, dcsim_layout_t* L, 
    * cursor gets there.  cap_xfer bounds the transfers in flight; an xfer entry lies at most (arrivals + transfers in
    * between) ahead of its arrival — the merge kernel measures that distance and flags DCSIM_ST_XFER_OVERFLOW when the
    * ring is too small for it, so the bound is checked, not assumed. */
-  int32_t ring = 8;
-  while (ring < 2 * cx) ring <<= 1;
+  const int32_t ring = dcsim_xring_entries(sp);
   L->xring = DCSIM_OFF_XRING;
   L->xring_mask = ring - 1;
   int32_t o = dcsim_align16(DCSIM_OFF_XRING + ring * 4);
@@ -881,6 +887,48 @@ DCSIM_DEV void dcsim_arr_flush(const dcsim_kparams_t* P, const dcsim_arr_stage_t
   }
 }
 #endif
+
+/* Whether two specs give every replica the same merged {arrival, xfer_done} list and list header (the same keys and RNG
+ * kind assumed): true when every spec field that dcsim_generate_arrivals and dcsim_merge_arrivals read is equal, doubles
+ * bit for bit, and so is every launch parameter derived from the spec that they read — the seq-ring size of the layout
+ * (dcsim_xring_entries of cap_xfer), against which the merge flags DCSIM_ST_XFER_OVERFLOW in the shared header.  The
+ * event loop only reads that list and header, so handles whose specs pass this can share one pre-pass
+ * (dcsim_create_shared).  ANY NEW SPEC FIELD OR LAYOUT FIELD THE PRE-PASS OR THE MERGE READS MUST BE ADDED HERE.  `field_out` (or NULL): the first field that
+ * differs, NULL when equal. */
+static inline bool dcsim_arrival_inputs_equal(const dcsim_spec_t* a, const dcsim_spec_t* b, const char** field_out = NULL) {
+  const char* diff = NULL;
+#define DCSIM_AIE(name, x, y) \
+  if (!diff && memcmp(&(x), &(y), sizeof(x)) != 0) diff = name
+  DCSIM_AIE("n_ing", a->n_ing, b->n_ing);
+  DCSIM_AIE("n_dc", a->n_dc, b->n_dc);
+  DCSIM_AIE("end_time", a->end_time, b->end_time);
+  for (int k = 0; k < 2; ++k) {
+    DCSIM_AIE(k ? "arr[1].mode" : "arr[0].mode", a->arr[k].mode, b->arr[k].mode);
+    DCSIM_AIE(k ? "arr[1].rate" : "arr[0].rate", a->arr[k].rate, b->arr[k].rate);
+    DCSIM_AIE(k ? "arr[1].amp" : "arr[0].amp", a->arr[k].amp, b->arr[k].amp);
+    DCSIM_AIE(k ? "arr[1].period" : "arr[0].period", a->arr[k].period, b->arr[k].period);
+  }
+  DCSIM_AIE("pareto_xm", a->pareto_xm, b->pareto_xm);
+  DCSIM_AIE("pareto_inv_alpha", a->pareto_inv_alpha, b->pareto_inv_alpha);
+  DCSIM_AIE("lognorm_mu", a->lognorm_mu, b->lognorm_mu);
+  DCSIM_AIE("lognorm_sigma", a->lognorm_sigma, b->lognorm_sigma);
+  DCSIM_AIE("lognorm_floor", a->lognorm_floor, b->lognorm_floor);
+  DCSIM_AIE("uniform_floor", a->uniform_floor, b->uniform_floor);
+  DCSIM_AIE("nv_magicconst", a->nv_magicconst, b->nv_magicconst);
+  DCSIM_AIE("two_pi", a->two_pi, b->two_pi);
+  DCSIM_AIE("route_rule", a->route_rule, b->route_rule);
+  DCSIM_AIE("cap_arrivals", a->cap_arrivals, b->cap_arrivals);
+  if (!diff && dcsim_xring_entries(a) != dcsim_xring_entries(b)) diff = "cap_xfer";
+  if (!diff && a->n_ing >= 1 && a->n_ing <= DCSIM_MAX_ING && a->n_dc >= 1 && a->n_dc <= DCSIM_MAX_DC) { /* the entries in use */
+    for (int i = 0; i < a->n_ing; ++i)
+      for (int d = 0; d < a->n_dc; ++d) DCSIM_AIE("transfer_s", a->transfer_s[i][d], b->transfer_s[i][d]);
+    if (a->route_rule == DCSIM_ROUTE_ECO) /* random routing draws the DC and never reads E_unit */
+      for (int d = 0; d < a->n_dc; ++d) DCSIM_AIE("eco_e_unit", a->dc[d].eco_e_unit, b->dc[d].eco_e_unit);
+  }
+#undef DCSIM_AIE
+  if (field_out) *field_out = diff;
+  return diff == NULL;
+}
 
 /* One replica's arrival list.  Per-thread scratch, element s of each array at [s * stride] ([slot][thread] in shared
  * memory): `next_t` the 2*n_ing stream clocks, `last_idx` the list index of each stream's latest arrival, `ring` the

@@ -68,29 +68,52 @@ class BatchedEngine:
     """
 
     def __init__(self, spec: S.Spec, n_replicas: int, base_seed: int, first_replica_id: int = 0, device: int = 0,
-                 cuda_stream: int = 0):
+                 cuda_stream: int = 0, _owner=None):
         self._lib = N.load()
         self._h = C.c_void_p()
-        self.n_replicas = int(n_replicas)
-        self.device = int(device)
         self.spec = spec
         blob = spec.to_bytes()
         self._blob = C.create_string_buffer(blob, len(blob))
-        N.check(self._lib.dcsim_create(self._blob, len(blob), self.n_replicas, base_seed & (2**64 - 1),
-                                       first_replica_id, device, C.byref(self._h)))
+        self.owner = _owner
+        if _owner is None:
+            self.n_replicas, self.device = int(n_replicas), int(device)
+            self.keys = (base_seed + first_replica_id) & (2**64 - 1)
+            N.check(self._lib.dcsim_create(self._blob, len(blob), self.n_replicas, base_seed & (2**64 - 1),
+                                           first_replica_id, device, C.byref(self._h)))
+        else:
+            self.n_replicas, self.device = _owner.n_replicas, _owner.device
+            self.keys = _owner.keys
+            N.check(self._lib.dcsim_create_shared(self._blob, len(blob), _owner._h, C.byref(self._h)))
         if cuda_stream:
             self.set_stream(cuda_stream)
         self._trace_cap = self._jobs_cap = self._cluster_cap = 0
         self._ens_cap = 0
         self._jens_windows, self._jens_bin = 0, None
 
+    @classmethod
+    def shared(cls, spec: S.Spec, owner: "BatchedEngine") -> "BatchedEngine":
+        """A member of ``owner``'s group: the same replicas and keys, reading the owner's arrival lists (one pre-pass for
+        the group, common random numbers).  ``spec`` must draw the same arrivals (``arrivals_compatible``); its
+        ``reset(seed, first)`` forwards the owner's current keys.  The owner may be closed first."""
+        return cls(spec, 0, 0, _owner=owner)
+
+    @property
+    def is_member(self) -> bool:
+        return self.owner is not None
+
     # -- configuration ---------------------------------------------------------------------------
     def set_stream(self, cuda_stream: int):
         N.check(self._lib.dcsim_set_stream(self._h, C.c_void_p(cuda_stream)), self._h)
 
-    def reset(self, base_seed: int, first_replica_id: int = 0):
-        """All replicas back to t = 0 with new keys; allocations are kept."""
+    def reset(self, base_seed=None, first_replica_id: int = 0):
+        """All replicas back to t = 0 with new keys; allocations are kept.  A member (``shared``) takes its owner's
+        current keys (``base_seed=None``); the library refuses any other keys for it."""
+        if base_seed is None:
+            if self.owner is None:
+                raise ValueError("reset: base_seed is required for an engine that owns its keys")
+            base_seed, first_replica_id = self.owner.keys, 0
         N.check(self._lib.dcsim_reset(self._h, base_seed & (2**64 - 1), first_replica_id), self._h)
+        self.keys = (base_seed + first_replica_id) & (2**64 - 1)
 
     def set_rng(self, kind: str = "philox"):
         """Word source of the replicas' random streams: "philox" (default; key = seed) or "mt19937" (CPython's own
@@ -249,6 +272,20 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_dc_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
 
+    # -- paired reductions (compare.py) ------------------------------------------------------------------------------
+    def paired_moments_into(self, variant_summary_ptr: int, device_ptr: int):
+        """Pass 1 on this (base) handle's stream against a variant's [n_replicas, SUMMARY_K] summaries on the device:
+        [4][(PAIR_DC_ENERGY_J + n_dc) * PAIR_FIELDS] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_paired_moments(self._h, C.c_void_p(variant_summary_ptr), self.n_replicas,
+                                               C.c_void_p(device_ptr)), self._h)
+
+    def paired_spread_into(self, variant_summary_ptr: int, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int,
+                           hist_ptr: int):
+        """Pass 2 on this handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_paired_spread(self._h, C.c_void_p(variant_summary_ptr), self.n_replicas,
+                                              C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                              C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
     # -- recorders -------------------------------------------------------------------------------
     def recorder_counts(self):
         """(trace, job_log, cluster_log) rows the recorders WOULD have written: more than a recorder's capacity means
@@ -296,6 +333,16 @@ class BatchedEngine:
             self.close()
         except Exception:
             pass
+
+
+def arrivals_compatible(spec_a: S.Spec, spec_b: S.Spec) -> bool:
+    """True when the two specs give every replica the same arrival list (the library's dcsim_arrivals_compatible): their
+    batches can share one arrival pre-pass (``BatchedEngine.shared``)."""
+    lib = N.load()
+    a, b = spec_a.to_bytes(), spec_b.to_bytes()
+    eq = C.c_int(0)
+    N.check(lib.dcsim_arrivals_compatible(a, len(a), b, len(b), C.byref(eq)))
+    return bool(eq.value)
 
 
 _COPY_POOL = None
@@ -459,18 +506,24 @@ def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, d
         if bits == 0:
             return eng, summ
         eng.close()
-        raisable = S.ST_RUN_OVERFLOW | S.ST_XFER_OVERFLOW | S.ST_ARRIVALS_OVERFLOW | S.ST_QUEUE_OVERFLOW | S.ST_STALE_OVERFLOW
-        if bits & ~raisable or attempt == max_retries:   # a status no capacity can cure (or out of attempts): fail now
-            raise RuntimeError(f"replicas stopped: {describe_status(bits)}")
-        g_max = max(sp.dc[d].total_gpus for d in range(sp.n_dc))
-        if bits & S.ST_RUN_OVERFLOW:
-            caps["cap_run"] = g_max
-        if bits & S.ST_XFER_OVERFLOW:
-            caps["cap_xfer"] = 2 * sp.cap_xfer
-        if bits & S.ST_ARRIVALS_OVERFLOW:
-            caps["cap_arrivals"] = 2 * sp.cap_arrivals
-        if bits & S.ST_QUEUE_OVERFLOW:
-            caps["cap_q_inf"], caps["cap_q_trn"] = 2 * sp.cap_q_inf, 2 * sp.cap_q_trn
-        if bits & S.ST_STALE_OVERFLOW:                   # cap_greedy: superseded job_finish events still in the event set
-            caps["cap_stale"] = 2 * max(64, sp.cap_stale)
+        raise_caps(bits, sp, caps, last_attempt=attempt == max_retries)
     raise AssertionError("unreachable")
+
+
+def raise_caps(bits, sp, caps, last_attempt=False):
+    """The capacity retry rule: raises in ``caps`` every capacity of ``sp`` that a replica overflowed (status ``bits``).
+    RuntimeError when a status no capacity can cure is set, or on the last attempt."""
+    raisable = S.ST_RUN_OVERFLOW | S.ST_XFER_OVERFLOW | S.ST_ARRIVALS_OVERFLOW | S.ST_QUEUE_OVERFLOW | S.ST_STALE_OVERFLOW
+    if bits & ~raisable or last_attempt:             # a status no capacity can cure (or out of attempts): fail now
+        raise RuntimeError(f"replicas stopped: {describe_status(bits)}")
+    g_max = max(sp.dc[d].total_gpus for d in range(sp.n_dc))
+    if bits & S.ST_RUN_OVERFLOW:
+        caps["cap_run"] = g_max
+    if bits & S.ST_XFER_OVERFLOW:
+        caps["cap_xfer"] = 2 * sp.cap_xfer
+    if bits & S.ST_ARRIVALS_OVERFLOW:
+        caps["cap_arrivals"] = 2 * sp.cap_arrivals
+    if bits & S.ST_QUEUE_OVERFLOW:
+        caps["cap_q_inf"], caps["cap_q_trn"] = 2 * sp.cap_q_inf, 2 * sp.cap_q_trn
+    if bits & S.ST_STALE_OVERFLOW:                   # cap_greedy: superseded job_finish events still in the event set
+        caps["cap_stale"] = 2 * max(64, sp.cap_stale)

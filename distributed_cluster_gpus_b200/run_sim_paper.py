@@ -66,6 +66,13 @@ def parse_args(argv=None):
                         "latencies per job type over all replicas (long format), and per-DC latency quantiles, to this file")
     p.add_argument("--job-ensemble-bin", type=float, default=None, metavar="SECONDS",
                    help="finish-window width of --job-ensemble-csv (default: --log-interval)")
+    p.add_argument("--compare-algos", type=str, default=None, metavar="A,B,...",
+                   help="run every listed algo on the scenario of the other flags, on the same replica keys, and compare "
+                        "each with the FIRST (the baseline) replica by replica; algos that draw the same arrivals share "
+                        "one arrival pre-pass.  cluster_log.csv / job_log.csv are not written in this mode")
+    p.add_argument("--compare-csv", type=str, default=None, metavar="PATH",
+                   help="with --compare-algos: write the paired statistics (long format, one row per algo and metric) "
+                        "to this file")
     p.add_argument("--gpus", type=int, default=1,
                    help="shard the replicas over this many GPUs of the node (one process per GPU; the only collective is "
                         "the all-reduce of the end-of-run statistics over NCCL).  Under torchrun the world size wins.")
@@ -121,6 +128,8 @@ def main(argv=None):
         if rc != 0:
             raise SystemExit(rc)
         return None
+    if args.compare_algos:
+        return _main_compare(args, world, rank)
     if world > 1:
         return _main_sharded(args, world, rank)
     sim = build_simulator(args)
@@ -215,6 +224,79 @@ def _main_sharded(args, world, rank):
     dist.destroy_process_group()
     sim.batch_stats = stats
     return sim
+
+
+def _main_compare(args, world, rank):
+    """--compare-algos A,B,...: every algo on the same scenario and replica keys (compare.compare_variants), paired with
+    the first.  Single-process or one rank of --gpus N (replicas sharded by global id; rank 0 writes)."""
+    from . import compare
+    algos = [a.strip() for a in args.compare_algos.split(",") if a.strip()]
+    if len(algos) < 2 or len(set(algos)) != len(algos):
+        raise SystemExit("--compare-algos needs at least two distinct algos")
+    unknown = [a for a in algos if a not in ALGOS]
+    if unknown:
+        raise SystemExit(f"--compare-algos: unknown algo(s) {unknown}; choose from {ALGOS}")
+    if args.ensemble_csv or args.job_ensemble_csv:
+        raise SystemExit("--ensemble-csv / --job-ensemble-csv are not available with --compare-algos (run each algo "
+                         "on its own for its cluster-log and job-log ensembles)")
+    dist = None
+    first, count, device = 0, args.replicas, args.device
+    if world > 1:
+        import torch
+        import torch.distributed as dist
+        from . import sharding
+        backend = os.environ.get("DCSIM_DIST_BACKEND", "nccl")
+        device = int(os.environ.get("LOCAL_RANK", str(rank))) % max(1, torch.cuda.device_count())
+        torch.cuda.set_device(device)
+        if not dist.is_initialized():
+            if backend == "nccl":
+                dist.init_process_group("nccl", device_id=torch.device("cuda", device))
+            else:
+                dist.init_process_group(backend)
+        first, count = sharding.shard(args.replicas, rank, world)
+        if count == 0:
+            raise SystemExit("--compare-algos needs at least one replica per rank")
+    sims = {a: build_simulator(argparse.Namespace(**dict(vars(args), algo=a)), replicas=count, first_replica_id=first,
+                               device=device, write_logs=False) for a in algos}
+    res = compare.compare_variants({a: sims[a]._flatten for a in algos}, algos[0], count, args.seed, first, device, rng=args.rng)
+    dc_names = [dc.name for dc in sims[algos[0]].dcs.values()]
+    per_algo = {}
+    for a in algos:
+        summ = res.summaries[a]
+        if dist is not None:                                   # every rank's rows, in global replica order
+            import torch
+            width = -(-args.replicas // world)
+            mine = torch.full((width, S.SUMMARY_K), float("nan"), dtype=torch.float64)
+            mine[:count] = torch.from_numpy(summ)
+            gathered = [torch.empty_like(mine) for _ in range(world)]
+            if backend == "gloo":
+                dist.all_gather(gathered, mine)
+            else:
+                dev = torch.device("cuda", device)
+                gathered = [g.to(dev) for g in gathered]
+                dist.all_gather(gathered, mine.to(dev))
+            rows = torch.cat(gathered).cpu().numpy()
+            summ = rows[~np.isnan(rows[:, S.S_STATUS])]
+        per_algo[a] = batch_statistics(summ)
+    if rank == 0:
+        if args.compare_csv:
+            res.to_csv(args.compare_csv, dc_names)
+        if args.summary_json:
+            with open(args.summary_json, "w") as f:
+                json.dump({"baseline": algos[0], "algos": per_algo, "comparison": res.rows(dc_names)}, f, indent=1)
+        for a in algos:
+            st = per_algo[a]
+            print(f"Done. ({a}) replicas={st['replicas']} events={st['events_total']:.0f} mean energy="
+                  f"{st['energy_j_mean']:.6g} J (+-{st['energy_j_ci95']:.3g}) mean latency={st['mean_latency_s_mean']:.6g} s")
+        for a in algos[1:]:
+            st = res.stats[a]
+            print(f"  {a} - {algos[0]}: energy {st.diff_mean[0]:+.6g} J [{st.diff_ci95_lo[0]:+.4g}, {st.diff_ci95_hi[0]:+.4g}] "
+                  f"({100 * st.rel_change[0]:+.3f} %), var_ratio {st.var_ratio[0]:.3g}, shared arrivals "
+                  f"{res.shared_arrivals[a]}")
+    if dist is not None:
+        dist.barrier()
+        dist.destroy_process_group()
+    return res
 
 
 def batch_statistics(summary: np.ndarray) -> dict:

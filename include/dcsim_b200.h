@@ -9,7 +9,8 @@
  * Ownership / threading
  *   - host buffers are caller-owned; device memory is library-owned;
  *   - one handle <-> one CUDA device <-> one stream; calls on one handle are not thread-safe,
- *     distinct handles are independent;
+ *     distinct handles are independent — except the members of one group (dcsim_create_shared), which share
+ *     the owner's arrival lists and stream and are driven from one thread;
  *   - nothing throws across the boundary: every entry point returns DCSIM_OK or a negative code and
  *     dcsim_last_error() returns the message.
  */
@@ -235,8 +236,36 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
  * keeping all device allocations.  Asynchronous on the handle's stream. */
 int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id);
 
-/* Launch on a caller-provided cudaStream_t (e.g. torch's current stream) instead of the handle's own. */
+/* Launch on a caller-provided cudaStream_t (e.g. torch's current stream) instead of the handle's own.  On the owner of a
+ * group it sets the stream of every handle of the group; on a member DCSIM_E_STATE. */
 int dcsim_set_stream(dcsim_t* h, void* cuda_stream);
+
+/* ---- policy comparisons on common random numbers ------------------------------------------------------------------
+ * Arrivals do not depend on the policy: the arrival pre-pass and the list merge read only the spec's arrival inputs
+ * (arr[2], n_ing, n_dc, end_time, the sampler constants, transfer_s, route_rule, cap_arrivals, and eco_e_unit when
+ * route_rule is ECO), the replica keys / RNG kind, and the size of the seq ring of in-flight transfers that cap_xfer
+ * implies (the merge flags DCSIM_ST_XFER_OVERFLOW in the list header when a transfer lies too far ahead for it); the
+ * event loop never writes the list or the header they leave.  So batches
+ * of specs that differ in algo, policy, power cap, DVFS thresholds, prices, carbon, nf tables ... can share ONE pre-pass,
+ * and replica r of each sees the same jobs at the same instants: the per-replica difference of two policies has far
+ * less variance than the difference of two independent batches.
+ *
+ * dcsim_arrivals_compatible: *equal_out = 1 when the two specs give every replica the same arrival list (host only;
+ * DCSIM_E_INVALID for a malformed blob).
+ *
+ * dcsim_create_shared: a MEMBER of the owner's group.  It takes replica count, keys, RNG kind, device and stream from
+ * the owner, allocates its own state, queues and summary, and reads the group's arrival lists (no pre-pass buffers of
+ * its own: dcsim_launch_info reports hbm_bytes_arrivals = 0).  DCSIM_E_INVALID when the arrival inputs differ (the
+ * message names the first differing field) or the owner is itself a member.
+ *   - The first dcsim_prepare / dcsim_advance of ANY handle of the group runs the pre-pass, once.
+ *   - dcsim_reset(owner, ...) draws new keys: the group's next prepare / advance re-runs the pre-pass.  A member must
+ *     then be reset with the owner's keys (base_seed + first_replica_id equal; DCSIM_E_INVALID otherwise) before it
+ *     advances again: until then dcsim_advance returns DCSIM_E_STATE ("arrival source was reset").
+ *   - dcsim_set_stream and dcsim_set_rng on a member: DCSIM_E_STATE (set them on the owner, before the group's first
+ *     prepare).
+ *   - Handles may be destroyed in any order: the lists live until the group's last handle is destroyed. */
+int dcsim_arrivals_compatible(const void* spec_a, size_t a_bytes, const void* spec_b, size_t b_bytes, int* equal_out);
+int dcsim_create_shared(const void* spec_blob, size_t spec_bytes, dcsim_t* owner, dcsim_t** out);
 
 /* Record the first `capacity` processed events of local replica `replica` (debug aid; 0 disables). */
 int dcsim_set_trace(dcsim_t* h, uint64_t replica, uint32_t capacity);
@@ -371,6 +400,29 @@ int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* 
                               double* dev_m2_out, uint64_t* dev_hist_out);
 /* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
+
+/* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant
+ * batch with the same keys (a member's dcsim_summary_device_ptr or a copy of it: [n][DCSIM_SUMMARY_K] doubles on the
+ * base's device).  Replica r counts in a column when both rows have status 0 and the metric is defined in both (a
+ * per-job or latency metric needs a finished job of that kind).  n_cols = (DCSIM_PAIR_DC_ENERGY_J + n_dc) *
+ * DCSIM_PAIR_FIELDS.  The same two passes and contract as dcsim_ensemble_moments / _spread, on the base's stream; n
+ * must be the base's replica count.  JOBS_*, UNFINISHED and their differences, and LOWER / HIGHER, are integer columns
+ * (unit bins when their range allows). */
+enum {
+  DCSIM_PAIR_ENERGY_J = 0,         /* total energy [J] */
+  DCSIM_PAIR_ENERGY_PER_JOB_J = 1, /* total energy / jobs finished */
+  DCSIM_PAIR_JOBS_INF = 2,         /* inference jobs finished */
+  DCSIM_PAIR_JOBS_TRN = 3,
+  DCSIM_PAIR_MEAN_LAT_INF_S = 4,   /* mean latency of the finished inference jobs */
+  DCSIM_PAIR_MEAN_LAT_TRN_S = 5,
+  DCSIM_PAIR_UNFINISHED = 6,       /* sum over DCs of queued (both types) + running jobs at the end */
+  DCSIM_PAIR_DC_ENERGY_J = 7       /* + dc: energy of each DC */
+};
+enum { DCSIM_PAIR_BASE = 0, DCSIM_PAIR_VARIANT = 1, DCSIM_PAIR_DIFF = 2 /* variant - base */, DCSIM_PAIR_LOWER = 3 /* 1: variant < base */,
+       DCSIM_PAIR_HIGHER = 4, DCSIM_PAIR_FIELDS = 5 };
+int dcsim_paired_moments(dcsim_t* base, const double* dev_variant_summary, uint64_t n, double* dev_out);
+int dcsim_paired_spread(dcsim_t* base, const double* dev_variant_summary, uint64_t n, const double* dev_mean,
+                        const double* dev_lo, const double* dev_hi, double* dev_m2_out, uint64_t* dev_hist_out);
 
 /* Word source of the replicas' random streams (before the first advance of a batch; stays across dcsim_reset).
  *   DCSIM_RNG_PHILOX   (default) Philox4x32-10, key = base_seed + replica id: counter-based, no state.
