@@ -163,13 +163,20 @@ gw_alphabet_dict = dict(zip((f"gw-{n}" for n in ("us-west", "us-east", "eu-west"
 
 
 def build_scenario(n_dc: int = 8, gpus_per_dc: Optional[int] = None, freq_levels: Optional[Iterable[float]] = None,
-                   gpus_list: Optional[Sequence[int]] = None):
+                   gpus_list: Optional[Sequence[int]] = None, wan: Optional[Dict[str, float]] = None):
     """The (D, G) sub-setting rule of SURVEY.md §8(d).
 
     Keeps the first ``n_dc`` DCs of build_dcs() (dict order) with their GPUType, overrides ``total_gpus``
     (``gpus_per_dc`` for all, or ``gpus_list`` per DC) and ``freq_levels``, keeps the gateways ``gw-<dc>`` of
     those DCs and the WAN edges with both endpoints kept.  Returns (ingresses, dcs, graph, coeffs_map).
+
+    ``wan`` (optional) overrides every kept edge: ``latency_ms`` and/or ``capacity_gbps``.  A finite capacity adds
+    payload / capacity to every transfer (SIM:487-495: 5 GB of training data over 1 Gbps is 5 s); latency 0 with
+    capacity 0 (no bandwidth term) makes every transfer instantaneous, so each xfer_done falls on its arrival's instant.
     """
+    wan = dict(wan or {})
+    if set(wan) - {"latency_ms", "capacity_gbps"}:
+        raise ValueError(f"wan: unknown keys {sorted(set(wan) - {'latency_ms', 'capacity_gbps'})}")
     if not 1 <= n_dc <= len(DC_TABLE):
         raise ValueError(f"n_dc must be in 1..{len(DC_TABLE)}")
     levels = list(freq_levels) if freq_levels is not None else list(FREQ_LEVELS_8)
@@ -190,5 +197,6 @@ def build_scenario(n_dc: int = 8, gpus_per_dc: Optional[int] = None, freq_levels
         if u in nodes:
             for e in edges:
                 if e.to in nodes:
-                    graph.add_edge(u, e.to, e.latency_ms, e.capacity_gbps, e.cost_per_GB)
+                    graph.add_edge(u, e.to, wan.get("latency_ms", e.latency_ms), wan.get("capacity_gbps", e.capacity_gbps),
+                                   e.cost_per_GB)
     return ingresses, dcs, graph, build_paper_coeffs(dcs)

@@ -374,6 +374,9 @@ struct dcsim_group {
   uint32_t* d_ml_meta;
   dcsim_arrhdr_t* d_arr_hdr;
   uint32_t* d_mt; /* [624][n_replicas] Mersenne Twister states, rng_kind == DCSIM_RNG_MT19937 only */
+#ifdef DCSIM_TEST_HOOKS
+  double test_quantum; /* the time quantum of dcsim_test_set_time_quantum when the group was made */
+#endif
 };
 
 static void group_release(dcsim_group* g) {
@@ -459,6 +462,20 @@ extern "C" {
 size_t dcsim_sizeof_spec(void) { return sizeof(dcsim_spec_t); }
 uint32_t dcsim_abi_version(void) { return DCSIM_ABI_VERSION; }
 int dcsim_summary_k(void) { return DCSIM_SUMMARY_K; }
+
+#ifdef DCSIM_TEST_HOOKS
+/* TEST-ONLY (the library built with -DDCSIM_TEST_HOOKS; not declared in include/dcsim_b200.h, not in the product
+ * library): handles created after this call round every arrival and xfer_done instant up to a multiple of q (0 = off),
+ * like the oracle's and the host build's hook, so that same-instant events become common on the device.  The quantum
+ * reaches the pre-pass and the merge through one __device__ variable, written in stream order by each group's prepare:
+ * groups with different quanta must not prepare concurrently. */
+static double g_test_time_quantum = 0.0;
+int dcsim_test_set_time_quantum(double q) {
+  if (!(q >= 0.0 && q <= DBL_MAX)) return set_err(NULL, DCSIM_E_INVALID, "test_set_time_quantum: q must be finite and >= 0%s%lld");
+  g_test_time_quantum = q;
+  return DCSIM_OK;
+}
+#endif
 
 static int validate_spec(const dcsim_spec_t* sp) {
   if (sp->magic != DCSIM_SPEC_MAGIC) return set_err(NULL, DCSIM_E_INVALID, "spec: bad magic%s%lld");
@@ -611,6 +628,10 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
         const double v = sp.transfer_s[i][d][jt];
         if (v == v && v < 1e300 && v > g->max_transfer) g->max_transfer = v; /* finite ones only */
       }
+#ifdef DCSIM_TEST_HOOKS
+  g->test_quantum = g_test_time_quantum;
+  g->max_transfer += g->test_quantum; /* a rounded-up xfer_done instant may lie up to one quantum past t + transfer_s */
+#endif
 
 #define GROUP_TRY(call)                                                                   \
   do {                                                                                    \
@@ -855,6 +876,10 @@ int dcsim_prepare(dcsim_t* h) {
   dcsim_make_layout(&h->g->spec, &P.L, /*job_log=*/0);
   const int nb = (int)((h->n_replicas + DCSIM_ARRIVALS_THREADS - 1) / DCSIM_ARRIVALS_THREADS);
   const size_t scratch = dcsim_arrivals_scratch_bytes(h->spec.n_ing); /* 52 KB at 8 ingresses: above the 48 KB default */
+#ifdef DCSIM_TEST_HOOKS
+  CUDA_TRY(h, cudaMemcpyToSymbolAsync(dcsim_test_time_quantum_dev, &h->g->test_quantum, sizeof(double), 0, cudaMemcpyHostToDevice,
+                                      h->g->stream));
+#endif
   if (h->g->rng_kind == DCSIM_RNG_MT19937) {
     CUDA_TRY(h, cudaFuncSetAttribute(dcsim_arrivals_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)scratch));
     dcsim_arrivals_kernel<true><<<nb, DCSIM_ARRIVALS_THREADS, scratch, h->g->stream>>>(P);

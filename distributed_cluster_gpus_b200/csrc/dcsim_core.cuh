@@ -840,12 +840,20 @@ DCSIM_DEV double dcsim_size_from_raw(const dcsim_spec_t& sp, double raw, int jt)
   return v > sp.lognorm_floor ? v : sp.lognorm_floor;
 }
 
-/* TEST HOOK, host build only (see oracle/dcsim_oracle.c g_test_time_quantum): rounds arrival and xfer_done instants up
- * to a multiple of a quantum so that same-instant events become common and the tie-breaking below is exercised. */
+/* TEST HOOK, host build and the test-only GPU build with DCSIM_TEST_HOOKS (see oracle/dcsim_oracle.c
+ * g_test_time_quantum): rounds arrival and xfer_done instants up to a multiple of a quantum so that same-instant events
+ * become common and the tie-breaking below is exercised.  Only the pre-pass and the merge read it; the product library
+ * has neither the variable nor the rounding. */
 #ifdef DCSIM_HOST_EMU
 static double dcsim_test_time_quantum = 0.0;
 static inline double dcsim_test_quantize(double t) {
   return (dcsim_test_time_quantum > 0.0 && !(t == DCSIM_INF)) ? ceil(t / dcsim_test_time_quantum) * dcsim_test_time_quantum : t;
+}
+#elif defined(DCSIM_TEST_HOOKS)
+static __device__ double dcsim_test_time_quantum_dev = 0.0; /* set from the host before the pre-pass (dcsim_b200.cu) */
+DCSIM_DEV double dcsim_test_quantize(double t) {
+  const double q = dcsim_test_time_quantum_dev;
+  return (q > 0.0 && !(t == DCSIM_INF)) ? ceil(t / q) * q : t;
 }
 #else
 #define dcsim_test_quantize(t) (t)

@@ -14,15 +14,20 @@ SIN10 = dict(mode="sinusoid", rate=10.0, amp=0.6, period=3600.0)
 SIN6 = dict(mode="sinusoid", rate=6.0, amp=0.6, period=3600.0)
 POI = lambda r: dict(mode="poisson", rate=float(r), amp=0.0, period=3600.0)  # noqa: E731
 OFF = dict(mode="off", rate=0.0, amp=0.0, period=3600.0)
+ZERO_WAN = dict(latency_ms=0.0, capacity_gbps=0.0)
+SLOW_WAN = dict(capacity_gbps=1.0)
 
 
 def scenario(name, n_dc, gpus_per_dc, inf, trn, duration, freq_levels=None, algo="default_policy",
              policy="energy_aware", log_interval=5.0, power_cap=0.0, num_fixed_gpus=1, fixed_freq=None,
-             gpus_list=None):
-    return {"name": name, "n_dc": n_dc, "gpus_per_dc": gpus_per_dc, "gpus_list": gpus_list,
-            "freq_levels": list(freq_levels or FREQ8), "inf": dict(inf), "trn": dict(trn),
-            "duration": float(duration), "algo": algo, "policy": policy, "log_interval": float(log_interval),
-            "power_cap": float(power_cap), "num_fixed_gpus": int(num_fixed_gpus), "fixed_freq": fixed_freq}
+             gpus_list=None, wan=None):
+    sc = {"name": name, "n_dc": n_dc, "gpus_per_dc": gpus_per_dc, "gpus_list": gpus_list,
+          "freq_levels": list(freq_levels or FREQ8), "inf": dict(inf), "trn": dict(trn),
+          "duration": float(duration), "algo": algo, "policy": policy, "log_interval": float(log_interval),
+          "power_cap": float(power_cap), "num_fixed_gpus": int(num_fixed_gpus), "fixed_freq": fixed_freq}
+    if wan is not None:   # only when given: every scenario without it keeps the reference's own WAN (and its fixture)
+        sc["wan"] = {k: float(v) for k, v in wan.items()}
+    return sc
 
 
 # BASELINE.json configs, with the durations fixed once here (SURVEY.md §8(d) caveat iii)
@@ -66,6 +71,13 @@ GOLDEN_SCENARIOS = [
              dict(mode="poisson", rate=0.3, amp=0.0, period=3600.0), 180.0, FREQ8, gpus_list=[16, 32, 256, 16, 128, 16, 512, 512]),
     scenario("cli_defaults_8dc_joint_nf_60s", 8, None, dict(mode="sinusoid", rate=6.0, amp=0.6, period=300.0),
              dict(mode="poisson", rate=0.3, amp=0.0, period=3600.0), 60.0, FREQ8, algo="joint_nf", gpus_list=[16, 32, 256, 16, 128, 16, 512, 512]),
+    # WAN overrides (paper_config.build_scenario `wan`).  Zero latency and no bandwidth term: transfer_s == 0, so every
+    # arrival ties with the xfer_done it pushes at its own instant.  1 Gbps links: a training job's 5 GB
+    # take 5 s (SIM:489), hundreds of arrivals lie within one max_transfer and the list merge leaves its shared-memory ring.
+    scenario("zero_xfer_4x64_sin10_60s", 4, 64, SIN10, POI(1.0), 60.0, FREQ8, wan=ZERO_WAN),
+    scenario("slow_wan_1g_4x64_sin10_60s", 4, 64, SIN10, POI(1.0), 60.0, FREQ8, wan=SLOW_WAN),
+    scenario("zero_xfer_cap_greedy_4x64_60s", 4, 64, SIN10, POI(1.0), 60.0, FREQ8, algo="cap_greedy", power_cap=20000.0,
+             wan=ZERO_WAN),
 ]
 BY_NAME = {s["name"]: s for s in GOLDEN_SCENARIOS}
 
@@ -79,7 +91,8 @@ CSV_SCENARIOS = {
 
 def build_inputs(sc):
     """Scenario -> kwargs of MultiIngressPaperSimulator / spec.flatten (product builders)."""
-    ingresses, dcs, graph, coeffs = _pc.build_scenario(sc["n_dc"], sc["gpus_per_dc"], sc["freq_levels"], sc.get("gpus_list"))
+    ingresses, dcs, graph, coeffs = _pc.build_scenario(sc["n_dc"], sc["gpus_per_dc"], sc["freq_levels"], sc.get("gpus_list"),
+                                                       sc.get("wan"))
     return dict(ingresses=ingresses, dcs=dcs, graph=graph, arrival_inf=ArrivalConfig(**sc["inf"]),
                 arrival_train=ArrivalConfig(**sc["trn"]), coeffs_map=coeffs,
                 carbon_intensity=_pc.build_carbon_intensity(), energy_price=_pc.build_energy_price(),

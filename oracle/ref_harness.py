@@ -85,13 +85,15 @@ def build_reference_inputs(sc):
     all_ing, full_graph = pc.build_ingresses_and_topology()
     ingresses = {f"gw-{k}": all_ing[f"gw-{k}"] for k in keep}
     nodes = set(keep) | set(ingresses)
+    wan = sc.get("wan") or {}   # optional: overrides latency_ms / capacity_gbps of every kept edge
     graph = Graph()
     for u, edges in full_graph.adj.items():
         if u not in nodes:
             continue
         for e in edges:
             if e.to in nodes:
-                graph.add_edge(u, e.to, e.latency_ms, e.capacity_gbps, e.cost_per_GB)
+                graph.add_edge(u, e.to, wan.get("latency_ms", e.latency_ms), wan.get("capacity_gbps", e.capacity_gbps),
+                               e.cost_per_GB)
     arr_inf = ArrivalConfig(**sc["inf"])
     arr_trn = ArrivalConfig(**sc["trn"])
     return dict(

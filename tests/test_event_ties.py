@@ -6,8 +6,12 @@ and in the host build of the device core rounds every arrival and xfer_done inst
 The oracle then resolves the ties with its heap; the device core has to reproduce that order from list indices alone —
 in the arrival pre-pass (two streams due at the same instant) and in the list merge (arrival vs xfer_done, xfer_done
 vs xfer_done).  Everything must stay bit-identical: summaries, the seq of every traced event, both logs."""
+import os
+
 import numpy as np
 import pytest
+
+from conftest import ROOT
 
 from distributed_cluster_gpus_b200 import scenarios as SC, spec as S
 from distributed_cluster_gpus_b200.engine import CLUSTER_DTYPE, JOB_DTYPE
@@ -64,11 +68,13 @@ def test_chunked_resume_with_ties(oracle, hostemu, quantum):
     assert np.array_equal(whole["summary"], parts["summary"]) and whole["events"] == parts["events"]
 
 
-@pytest.mark.parametrize("name", ["cfg3_4x64_sinusoid_120s", "cfg5_8x256_sinusoid_60s", "ragged_3dc_12_5_40", "sweep_eco_route"])
+@pytest.mark.parametrize("name", ["cfg3_4x64_sinusoid_120s", "cfg5_8x256_sinusoid_60s", "ragged_3dc_12_5_40", "sweep_eco_route",
+                                  "slow_wan_1g_4x64_sin10_60s"])
 @pytest.mark.parametrize("q", [0.0, 0.25])
 def test_merge_fallback_paths(oracle, hostemu, quantum, name, q):
     """The list merge keeps a sliding window of arrivals in shared memory and reads HBM where a scan leaves it.  A host
-    build with a ring of ONE chunk sends nearly every scan down that path; results must not change."""
+    build with a ring of ONE chunk sends nearly every scan down that path; results must not change.  The slow WAN
+    (5 s transfers, hundreds of arrivals per max_transfer) leaves the ring even at full size."""
     sc = dict(SC.BY_NAME[name])
     sc["duration"] = min(sc["duration"], 40.0)
     blob = SC.to_spec(sc, caps={"cap_xfer": 4096}).to_bytes()
@@ -78,3 +84,17 @@ def test_merge_fallback_paths(oracle, hostemu, quantum, name, q):
     a, b = got["summary"].copy(), want.copy()
     a[:, HIGH_WATER] = b[:, HIGH_WATER] = 0
     assert got["events"] == total and np.array_equal(a, b)
+
+
+def test_time_quantum_hook_only_in_the_test_build():
+    """The GPU build with the hook (tests/gpuhooks, -DDCSIM_TEST_HOOKS) exports its setter; the product library does not."""
+    import ctypes as C
+    import __graft_entry__ as G
+    from distributed_cluster_gpus_b200 import _native
+    if not os.path.exists(G.HOOK_LIB):
+        G.build()
+    assert not hasattr(C.CDLL(_native.LIB_PATH), "dcsim_test_set_time_quantum")
+    hook = C.CDLL(G.HOOK_LIB)
+    assert hasattr(hook, "dcsim_test_set_time_quantum")
+    with open(os.path.join(ROOT, "include", "dcsim_b200.h")) as f:
+        assert "dcsim_test_set_time_quantum" not in f.read()
