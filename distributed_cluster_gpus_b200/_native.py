@@ -26,6 +26,8 @@ EXPORTS = (
     "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_job_ensemble_moments",
     "dcsim_job_ensemble_spread", "dcsim_fetch_dc_latency_histogram",
     "dcsim_arrivals_compatible", "dcsim_create_shared", "dcsim_paired_moments", "dcsim_paired_spread",
+    "dcsim_enable_power_profile", "dcsim_power_profile_range", "dcsim_fetch_power_profile", "dcsim_power_profile_moments",
+    "dcsim_power_profile_spread",
 )
 
 _lib = None
@@ -128,6 +130,17 @@ def load():
         L.dcsim_paired_moments.argtypes = [vp, vp, u64, vp]
         L.dcsim_paired_spread.restype = i32
         L.dcsim_paired_spread.argtypes = [vp, vp, u64, vp, vp, vp, vp, vp]
+    if hasattr(L, "dcsim_enable_power_profile"):
+        L.dcsim_enable_power_profile.restype = i32
+        L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]
+        L.dcsim_power_profile_range.restype = i32
+        L.dcsim_power_profile_range.argtypes = [vp, C.POINTER(C.c_double)]
+        L.dcsim_fetch_power_profile.restype = i32
+        L.dcsim_fetch_power_profile.argtypes = [vp, vp, C.c_size_t]
+        L.dcsim_power_profile_moments.restype = i32
+        L.dcsim_power_profile_moments.argtypes = [vp, vp]
+        L.dcsim_power_profile_spread.restype = i32
+        L.dcsim_power_profile_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

@@ -36,7 +36,9 @@ extern __shared__ __align__(16) char dcsim_smem[];
  *                      leave the SM below its 32 warps (8 DC x 256: 17 kB -> 12 warps/SM; head ~4 kB -> 32);
  *   DCSIM_MODE_INPLACE nothing is staged (even the head exceeds a CTA's shared memory): same core on the HBM copy. */
 enum { DCSIM_MODE_INPLACE = 0, DCSIM_MODE_STAGED = 1, DCSIM_MODE_HEAD = 2 };
-template <bool CAP, int MODE>
+/* PP = the power-profile recorder is compiled in (launched when it is enabled): the kernels without it keep their
+ * registers, spills and code. */
+template <bool CAP, int MODE, bool PP>
 __global__ void __launch_bounds__(DCSIM_MAX_WARPS_PER_CTA * 32, DCSIM_MIN_CTAS_PER_SM)
 DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsigned long long* __restrict__ events_total) {
   /* one replica per group of DCSIM_LANES lanes: a whole warp, or an aligned quarter / half of one */
@@ -63,7 +65,7 @@ DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsig
     for (int i = lane; i < bytes / 16; i += DCSIM_LANES) dst[i] = src[i];
   }
   dcsim_warp_sync();
-  const uint32_t n = dcsim_replica_step<CAP, MODE != DCSIM_MODE_STAGED>(&P, r, blk, rec, fresh, ghost);
+  const uint32_t n = dcsim_replica_step<CAP, MODE != DCSIM_MODE_STAGED, PP>(&P, r, blk, rec, fresh, ghost);
   dcsim_warp_sync();
   if (MODE != DCSIM_MODE_INPLACE && !ghost) {
     const uint4* src = reinterpret_cast<const uint4*>(blk);
@@ -75,29 +77,34 @@ DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsig
 
 
 typedef void (*DCSIM_ADV(dcsim_advance_fn))(const dcsim_kparams_t, unsigned long long*);
-static DCSIM_ADV(dcsim_advance_fn) DCSIM_ADV(dcsim_pick_kernel)(bool cap, int mode) {
-  static const DCSIM_ADV(dcsim_advance_fn) table[6] = {
-      DCSIM_ADV(dcsim_advance_kernel)<false, 0>, DCSIM_ADV(dcsim_advance_kernel)<false, 1>, DCSIM_ADV(dcsim_advance_kernel)<false, 2>,
-      DCSIM_ADV(dcsim_advance_kernel)<true, 0>,  DCSIM_ADV(dcsim_advance_kernel)<true, 1>,  DCSIM_ADV(dcsim_advance_kernel)<true, 2>};
-  return table[(cap ? 3 : 0) + mode];
+static DCSIM_ADV(dcsim_advance_fn) DCSIM_ADV(dcsim_pick_kernel)(bool cap, int mode, bool pp) {
+  static const DCSIM_ADV(dcsim_advance_fn) table[12] = {
+      DCSIM_ADV(dcsim_advance_kernel)<false, 0, false>, DCSIM_ADV(dcsim_advance_kernel)<false, 1, false>, DCSIM_ADV(dcsim_advance_kernel)<false, 2, false>,
+      DCSIM_ADV(dcsim_advance_kernel)<true, 0, false>,  DCSIM_ADV(dcsim_advance_kernel)<true, 1, false>,  DCSIM_ADV(dcsim_advance_kernel)<true, 2, false>,
+      DCSIM_ADV(dcsim_advance_kernel)<false, 0, true>,  DCSIM_ADV(dcsim_advance_kernel)<false, 1, true>,  DCSIM_ADV(dcsim_advance_kernel)<false, 2, true>,
+      DCSIM_ADV(dcsim_advance_kernel)<true, 0, true>,   DCSIM_ADV(dcsim_advance_kernel)<true, 1, true>,   DCSIM_ADV(dcsim_advance_kernel)<true, 2, true>};
+  return table[(pp ? 6 : 0) + (cap ? 3 : 0) + mode];
 }
 
 /* Resident CTAs per SM this build's register budget was chosen for (its __launch_bounds__). */
 int DCSIM_ADV(dcsim_adv_min_ctas)(void) { return DCSIM_MIN_CTAS_PER_SM; }
 
-/* Launch on `stream`: `ctas` CTAs of `threads` threads (threads / DCSIM_LANES replicas each), `smem` dynamic bytes. */
+/* Launch on `stream`: `ctas` CTAs of `threads` threads (threads / DCSIM_LANES replicas each), `smem` dynamic bytes.  The
+ * instantiation with the power-profile recorder when P->pp is set. */
 cudaError_t DCSIM_ADV(dcsim_adv_launch)(const dcsim_kparams_t* P, unsigned long long* events, int cap, int mode, int ctas, int threads,
                                         int smem, cudaStream_t stream) {
-  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode)<<<ctas, threads, smem, stream>>>(*P, events);
+  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
   return cudaGetLastError();
 }
 
-/* Registers per thread and resident CTAs per SM of the instantiation for (cap, mode) at that CTA shape; also raises the
- * kernel's dynamic shared-memory limit to `smem_optin`. */
+/* Registers per thread and resident CTAs per SM of the instantiation for (cap, mode) at that CTA shape (the one without
+ * the power-profile recorder); also raises the dynamic shared-memory limit of both to `smem_optin`. */
 cudaError_t DCSIM_ADV(dcsim_adv_attrs)(int cap, int mode, int threads, int smem, int smem_optin, int* regs, int* blocks_per_sm,
                                        int* min_ctas_per_sm) {
-  const DCSIM_ADV(dcsim_advance_fn) kern = DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode);
+  const DCSIM_ADV(dcsim_advance_fn) kern = DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, false);
   cudaError_t e;
+  if ((e = cudaFuncSetAttribute(DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, true), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                smem_optin)) != cudaSuccess) return e;
   if ((e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin)) != cudaSuccess) return e;
   cudaFuncAttributes fa;
   if ((e = cudaFuncGetAttributes(&fa, kern)) != cudaSuccess) return e;

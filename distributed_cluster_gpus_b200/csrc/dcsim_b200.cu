@@ -263,6 +263,27 @@ struct dcsim_ens_pair_src {
   }
 };
 
+/* Power profile: column c = n contiguous doubles ([DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n]), counted by the replicas
+ * with status 0. */
+struct dcsim_ens_pp_src {
+  const double* pp;
+  const uint32_t* status;
+  uint64_t n;
+  struct view {
+    const double* x;
+    const uint32_t* status;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (status[r] != 0u) return false;
+      v = x[r];
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const { return view{pp + col * n, status}; }
+  __device__ __forceinline__ bool integral(uint64_t col) const {
+    return col == DCSIM_PP_EXCURSIONS || col == DCSIM_PP_OUT_OF_RANGE;
+  }
+};
+
 __device__ __forceinline__ double dcsim_ens_min(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double dcsim_ens_max(double a, double b) { return b > a ? b : a; }
 
@@ -426,6 +447,10 @@ struct dcsim {
   unsigned long long* d_jens_hist_out; /* [n_dc][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_latency_histogram */
   double jens_bin;
   uint64_t jens_windows;
+  double* d_pp;            /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile (opt-in) */
+  double* d_pp_work;       /* [n_replicas][DCSIM_PPW_N] its working state */
+  uint32_t* d_pp_status;   /* [n_replicas] status words (+ 1 word), refreshed by every reduction */
+  double pp_threshold;
   unsigned long long events_seen;
   char err[512];
 };
@@ -442,6 +467,10 @@ static size_t jens_row_bytes(const dcsim_t* h) { /* one row (window) of the job-
 static size_t jens_hist_bytes(const dcsim_t* h) {
   return (size_t)h->n_replicas * (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(uint32_t);
 }
+
+static uint64_t pp_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc + DCSIM_PP_BINS); }
+static size_t pp_bytes(const dcsim_t* h) { return (size_t)pp_cols(h) * (size_t)h->n_replicas * sizeof(double); }
+static size_t pp_work_bytes(const dcsim_t* h) { return (size_t)h->n_replicas * DCSIM_PPW_N * sizeof(double); }
 
 static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", long long b = 0) {
   char* dst = h ? h->err : g_create_err;
@@ -773,6 +802,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, (h->jens_windows + 1) * jens_row_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
   }
+  if (h->d_pp) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
+  }
   if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
     h->g->seed0 = base_seed + first_replica_id;
     h->g->arrivals_ready = 0;
@@ -853,6 +886,8 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->ens = h->d_ens; P->ens_cap = h->ens_cap;
   P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
   P->finish_rec = (P->lat_hist || P->jens) ? 1u : 0u;
+  P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
+  P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
 }
 
 /* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */
@@ -1284,6 +1319,87 @@ int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes
   return DCSIM_OK;
 }
 
+int dcsim_enable_power_profile(dcsim_t* h, double threshold_w) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!(threshold_w >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_power_profile: the threshold must be >= 0 (+inf: none)%s%lld");
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_power_profile on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_power_profile must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_pp) {
+    const size_t need = pp_bytes(h) + pp_work_bytes(h);
+    cudaError_t e = cudaMalloc(&h->d_pp, pp_bytes(h));
+    if (e == cudaSuccess) e = cudaMalloc(&h->d_pp_work, pp_work_bytes(h));
+    if (e == cudaSuccess && !h->d_pp_status) e = cudaMalloc(&h->d_pp_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t));
+    if (e != cudaSuccess) {
+      cudaFree(h->d_pp); cudaFree(h->d_pp_work);
+      h->d_pp = NULL; h->d_pp_work = NULL;
+      if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
+      cudaGetLastError();
+      return set_err(h, DCSIM_E_NOMEM, "enable_power_profile: %s%lld bytes of device memory do not fit (run fewer replicas)", "",
+                     (long long)need);
+    }
+  }
+  h->pp_threshold = threshold_w;
+  CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_power_profile_range(dcsim_t* h, double* hi_out) {
+  if (!h || !hi_out) return DCSIM_E_INVALID;
+  *hi_out = dcsim_pp_range(&h->spec);
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  if (!h->d_pp) return set_err(h, DCSIM_E_STATE, "power profile not enabled (dcsim_enable_power_profile)%s%lld");
+  if (!h->launches) return set_err(h, DCSIM_E_STATE, "power profile read before the first advance%s%lld");
+  if (out_bytes < pp_bytes(h))
+    return set_err(h, DCSIM_E_INVALID, "fetch_power_profile: buffer too small (need %s%lld bytes)", "", (long long)pp_bytes(h));
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_pp, pp_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+/* Every replica's status word into d_pp_status (on the stream, ahead of the reduction that reads it). */
+static int pp_status(dcsim_t* h) {
+  if (!h->d_pp) return set_err(h, DCSIM_E_STATE, "power profile not enabled (dcsim_enable_power_profile)%s%lld");
+  if (!h->launches) return set_err(h, DCSIM_E_STATE, "power profile read before the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_pp_status + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
+  int blocks = (int)((h->n_replicas + 255) / 256);
+  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_pp_status);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_power_profile_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = pp_status(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint64_t n_cols = pp_cols(h);
+  const dcsim_ens_pp_src src{h->d_pp, h->d_pp_status, h->n_replicas};
+  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                               double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = pp_status(h);
+  if (rc != DCSIM_OK) return rc;
+  const uint64_t n_cols = (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc); /* the bins need no spread */
+  const dcsim_ens_pp_src src{h->d_pp, h->d_pp_status, h->n_replicas};
+  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
+                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
 int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {
   if (!h || !out3) return DCSIM_E_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
@@ -1353,6 +1469,7 @@ void dcsim_destroy(dcsim_t* h) {
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_status); cudaFree(h->d_jens_hist_out);
+  cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_pp_status);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }

@@ -482,6 +482,10 @@ struct dcsim_kparams_t {
   uint32_t* jens_hist;  /* [n_replicas][n_dc][2][DCSIM_LAT_BINS] per-DC job-latency histograms (with jens) */
   double jens_bin;      /* finish-window width [s] */
   uint64_t jens_windows; /* W */
+  double* pp;           /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile, or NULL */
+  double* pp_work;      /* [n_replicas][DCSIM_PPW_N] its working state (with pp) */
+  double pp_threshold;  /* [W], +inf: none */
+  double pp_hi;         /* upper end of the histogram range (dcsim_pp_range) */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -497,6 +501,8 @@ struct dcsim_ctx_t {
   dcsim_hdr_t* H;
   int lane;
   bool is_traced, is_logged;
+  bool pp;               /* the power-profile recorder runs: a compile-time false in the instantiations without it
+                            (dcsim_replica_step<..., PP>), so their code does not change */
   /* Hot scalars kept in registers and written back to the header when the launch ends.  seq: lane 0's copy is
    * authoritative (only lane 0 runs handlers); the others are warp-uniform. */
   uint32_t seq;          /* successful pushes (SIM:163) */
@@ -1389,12 +1395,121 @@ DCSIM_DEV int dcsim_argmin_cand(dcsim_ctx_t& c, dcsim_omin_t& om, double* t_out,
 /* SIM:160-163: an event later than end_time + 1e-9 (or at +inf) is never scheduled and takes no seq. */
 DCSIM_DEV bool dcsim_schedulable(const dcsim_ctx_t& c, double t) { return !(t == DCSIM_INF) && !(t > c.P->end_eps); }
 
+/* ---- power profile (opt-in: P->pp; layout and definitions in include/dcsim_b200.h) ---------------------------------
+ * DF_POWER is what the per-event accrual integrates, and it is written only at init and by dcsim_refresh_power (job
+ * start, job finish, the cap controller).  So the state that held over (last change point, now] is still in DF_POWER
+ * when the first write of a later instant comes: the recorder hangs off those writes and the tail, with no per-event
+ * work.  Its working state is a row of DCSIM_PPW_N doubles per replica in HBM (zeroed by enable / reset); every
+ * instant in it is > 0 once set, so 0.0 reads as "not yet". */
+enum {
+  DCSIM_PPW_TC = 0,   /* last change point: the profile is accounted up to here */
+  DCSIM_PPW_LVL_S,    /* start of the open level (0: none opened yet) */
+  DCSIM_PPW_LVL_P,    /* its power */
+  DCSIM_PPW_RUN_S,    /* start of the open run of levels above the threshold (0: none) */
+  DCSIM_PPW_PEAK, DCSIM_PPW_T_PEAK, DCSIM_PPW_OVER_S, DCSIM_PPW_OVER_J, DCSIM_PPW_EXC, DCSIM_PPW_LONGEST, DCSIM_PPW_OOR,
+  DCSIM_PPW_LEVELS,   /* levels closed */
+  DCSIM_PPW_DC_PEAK,  /* + d */
+  DCSIM_PPW_N = DCSIM_PPW_DC_PEAK + DCSIM_MAX_DC
+};
+
+/* Host code: the histogram's upper end (include/dcsim_b200.h dcsim_power_profile_range). */
+static inline double dcsim_pp_range(const dcsim_spec_t* sp) {
+  double total = 0.0;
+  for (int d = 0; d < sp->n_dc; ++d) {
+    const dcsim_dc_t& cfg = sp->dc[d];
+    double fs[DCSIM_MAX_FREQ + 3 + 2 * DCSIM_HOURS * 2 + 2];
+    int nf = 0;
+    fs[nf++] = sp->dvfs_low; fs[nf++] = sp->dvfs_high; fs[nf++] = cfg.default_freq;
+    for (int q = 0; q < cfg.n_freq; ++q) fs[nf++] = cfg.freq_levels[q];
+    for (int jt = 0; jt < 2; ++jt) {
+      for (int hr = 0; hr < DCSIM_HOURS; ++hr) fs[nf++] = cfg.nf_xfer[jt][hr].f;
+      fs[nf++] = cfg.nf_deq[jt].f;
+    }
+    double m = cfg.power_gating ? cfg.p_sleep : cfg.p_idle;
+    for (int i = 0; i < nf; ++i) {
+      const double f = fs[i] > 0.0 ? fs[i] : 0.0;
+      for (int jt = 0; jt < 2; ++jt) {
+        const dcsim_coeffs_t& k = cfg.coeffs[jt];
+        const double busy = k.alpha_p * f * f * f + k.beta_p * f + k.gamma_p; /* energy_paper.py:4-6, one GPU */
+        m = busy > m ? busy : m;
+      }
+      const double tail = cfg.p_idle + cfg.p_peak * pow(fs[i], cfg.alpha); /* models.py:88, one active GPU */
+      m = tail > m ? tail : m;
+    }
+    total += (double)cfg.total_gpus * m;
+  }
+  total *= 1.0 + 1.0 / 1048576.0;
+  return total > 0.0 ? total : 1.0;
+}
+
+DCSIM_DEV bool dcsim_same_bits(double a, double b) { return dcsim_hi(a) == dcsim_hi(b) && dcsim_lo(a) == dcsim_lo(b); }
+
+/* Level [s, e] of power p closes: its histogram bin (a fire-and-forget RED; one writer per replica, so each bin is the
+ * sequential sum in level order), the peak, the threshold-run bookkeeping. */
+DCSIM_DEV void dcsim_pp_close(const dcsim_kparams_t* P, double* w, uint32_t r, double s, double e, double p) {
+  const double len = e - s, hi = P->pp_hi;
+  const double f = floor(p / (hi * (1.0 / (double)DCSIM_PP_BINS)));
+  int b = f >= (double)(DCSIM_PP_BINS - 1) ? DCSIM_PP_BINS - 1 : (f > 0.0 ? (int)f : 0);
+  if (!(p >= 0.0 && p <= hi)) w[DCSIM_PPW_OOR] += 1.0;
+  double* cell = P->pp + (uint64_t)(DCSIM_PP_FIELDS + P->spec.n_dc + b) * P->n_replicas + r;
+#ifdef DCSIM_HOST_EMU
+  *cell += len;
+#else
+  atomicAdd(cell, len);
+#endif
+  if (w[DCSIM_PPW_LEVELS] == 0.0 || p > w[DCSIM_PPW_PEAK]) { w[DCSIM_PPW_PEAK] = p; w[DCSIM_PPW_T_PEAK] = s; }
+  w[DCSIM_PPW_LEVELS] += 1.0;
+  const double thr = P->pp_threshold;
+  if (p > thr) {
+    w[DCSIM_PPW_OVER_S] += len;
+    w[DCSIM_PPW_OVER_J] += (p - thr) * len;
+    if (w[DCSIM_PPW_RUN_S] == 0.0) { w[DCSIM_PPW_RUN_S] = s; w[DCSIM_PPW_EXC] += 1.0; }
+  } else if (w[DCSIM_PPW_RUN_S] != 0.0) {
+    const double l = s - w[DCSIM_PPW_RUN_S];
+    if (l > w[DCSIM_PPW_LONGEST]) w[DCSIM_PPW_LONGEST] = l;
+    w[DCSIM_PPW_RUN_S] = 0.0;
+  }
+}
+
+/* The interval (TC, now] had per-DC power pd[0, n_dc) (their DC-order sum p): extend the open level or close it and
+ * open the next one at TC.  Nothing when the interval is empty. */
+DCSIM_DEV void dcsim_pp_segment(const dcsim_kparams_t* P, double* w, uint32_t r, double now, double p, const double* pd) {
+  const double tc = w[DCSIM_PPW_TC];
+  if (!(now > tc)) return;
+  const bool first = w[DCSIM_PPW_LVL_S] == 0.0;
+  for (int d = 0; d < P->spec.n_dc; ++d)
+    if (first || pd[d] > w[DCSIM_PPW_DC_PEAK + d]) w[DCSIM_PPW_DC_PEAK + d] = pd[d];
+  if (first) {
+    w[DCSIM_PPW_LVL_S] = tc; w[DCSIM_PPW_LVL_P] = p;
+  } else if (!dcsim_same_bits(p, w[DCSIM_PPW_LVL_P])) {
+    dcsim_pp_close(P, w, r, w[DCSIM_PPW_LVL_S], tc, w[DCSIM_PPW_LVL_P]);
+    w[DCSIM_PPW_LVL_S] = tc; w[DCSIM_PPW_LVL_P] = p;
+  }
+  w[DCSIM_PPW_TC] = now;
+}
+
+/* Lane 0, before a DF_POWER write at instant `now`: the state in DF_POWER held over (TC, now].  Before the first
+ * processed event (DF_UTIL_BEGIN still 0.0) nothing accrues, so nothing is recorded. */
+DCSIM_COLD void dcsim_pp_touch(const dcsim_kparams_t* P, char* blk, uint32_t r, double now) {
+  const struct { char* blk; } v = {blk};
+  const double t0 = DCF(v, DF_UTIL_BEGIN)[0];
+  if (t0 == 0.0) return;
+  double* w = P->pp_work + (uint64_t)r * DCSIM_PPW_N;
+  if (w[DCSIM_PPW_TC] == 0.0) w[DCSIM_PPW_TC] = t0;
+  if (!(now > w[DCSIM_PPW_TC])) return;
+  const double* pd = DCF(v, DF_POWER);
+  double p = 0.0;
+  for (int d = 0; d < P->spec.n_dc; ++d) p += pd[d];
+  dcsim_pp_segment(P, w, r, now, p, pd);
+}
+
 /* Lane 0.  DC d's estimated power as SIM:168-179 computes it on every event: the running jobs' powers summed in
  * dict (= start) order from 0.0 — kept in DF_PSUM, see there — then the idle term. */
 DCSIM_DEV void dcsim_refresh_power(dcsim_ctx_t& c, int d) {
   const dcsim_dc_t& cfg = c.P->spec.dc[d];
   const int idle = cfg.total_gpus - DCI(c, DI_BUSY)[d];
   const double p_idle = (double)idle * (cfg.power_gating ? cfg.p_sleep : cfg.p_idle);
+  if (c.pp) dcsim_pp_touch(c.P, c.blk, c.r, c.now);
   DCF(c, DF_POWER)[d] = DCF(c, DF_PSUM)[d] + p_idle;
 }
 
@@ -2156,6 +2271,14 @@ DCSIM_DEV void dcsim_replica_init(dcsim_ctx_t& c) {
   dcsim_list_wait();
 }
 
+/* models.py:82-91: DC d's instantaneous_power_w() with `busy` GPUs active at frequency f (the tail's power). */
+DCSIM_DEV double dcsim_tail_power(const dcsim_dc_t& cfg, int busy, double f) {
+  const double fa = cfg.alpha == 3.0 ? dcsim_cube(f) : pow(f, cfg.alpha);
+  const double p_active = (double)busy * (cfg.p_idle + cfg.p_peak * fa);
+  const double p_idle = (double)(cfg.total_gpus - busy) * (cfg.power_gating ? cfg.p_sleep : cfg.p_idle);
+  return p_active + p_idle;
+}
+
 /* SIM:469-475: util to end_time, then accrue_energy(end_time) WITHOUT power_fn => models.py:82-91. */
 DCSIM_DEV void dcsim_replica_tail(dcsim_ctx_t& c) {
   const dcsim_spec_t& sp = c.P->spec;
@@ -2167,15 +2290,51 @@ DCSIM_DEV void dcsim_replica_tail(dcsim_ctx_t& c) {
     if (0.0 < last && last < end) DCF(c, DF_UTIL_TIME)[d] += (double)busy * (end - last); /* SIM:471-474 */
     if (last != 0.0) { /* models.py:100-106 with power_fn=None */
       double dt = end - last; dt = dt > 0.0 ? dt : 0.0;
-      const double f = DCF(c, DF_CUR_FREQ)[d];
-      const double fa = cfg.alpha == 3.0 ? dcsim_cube(f) : pow(f, cfg.alpha);
-      const double p_active = (double)busy * (cfg.p_idle + cfg.p_peak * fa);
-      const double p_idle = (double)(cfg.total_gpus - busy) * (cfg.power_gating ? cfg.p_sleep : cfg.p_idle);
-      DCF(c, DF_ENERGY)[d] += (p_active + p_idle) * dt;
+      DCF(c, DF_ENERGY)[d] += dcsim_tail_power(cfg, busy, DCF(c, DF_CUR_FREQ)[d]) * dt;
     }
     DCF(c, DF_LAST_T)[d] = end;
   }
   dcsim_warp_sync();
+}
+
+/* Lane 0, once, after the tail: the power profile's last state up to the last event (`last`), then the tail interval
+ * with the tail's own power; closes the open level and run at end_time and writes the replica's columns. */
+DCSIM_COLD void dcsim_pp_tail(const dcsim_kparams_t* P, char* blk, uint32_t r, double last) {
+  const struct { char* blk; } v = {blk};
+  const dcsim_spec_t& sp = P->spec;
+  double* w = P->pp_work + (uint64_t)r * DCSIM_PPW_N;
+  double profile = 0.0;
+  if (last != 0.0) { /* an event was processed: the profile runs from the first one to end_time */
+    const double t0 = DCF(v, DF_UTIL_BEGIN)[0];
+    if (w[DCSIM_PPW_TC] == 0.0) w[DCSIM_PPW_TC] = t0;
+    const double* pd = DCF(v, DF_POWER);
+    double p = 0.0;
+    for (int d = 0; d < sp.n_dc; ++d) p += pd[d];
+    dcsim_pp_segment(P, w, r, last, p, pd);
+    double pt[DCSIM_MAX_DC];
+    p = 0.0;
+    for (int d = 0; d < sp.n_dc; ++d) { pt[d] = dcsim_tail_power(sp.dc[d], DCI(v, DI_BUSY)[d], DCF(v, DF_CUR_FREQ)[d]); p += pt[d]; }
+    dcsim_pp_segment(P, w, r, sp.end_time, p, pt);
+    const double end = w[DCSIM_PPW_TC];
+    if (w[DCSIM_PPW_LVL_S] != 0.0) dcsim_pp_close(P, w, r, w[DCSIM_PPW_LVL_S], end, w[DCSIM_PPW_LVL_P]);
+    if (w[DCSIM_PPW_RUN_S] != 0.0) {
+      const double l = end - w[DCSIM_PPW_RUN_S];
+      if (l > w[DCSIM_PPW_LONGEST]) w[DCSIM_PPW_LONGEST] = l;
+      w[DCSIM_PPW_RUN_S] = 0.0;
+    }
+    profile = sp.end_time - t0;
+  }
+  const uint64_t n = P->n_replicas;
+  double* o = P->pp + r;
+  o[DCSIM_PP_PROFILE_S * n] = profile;
+  o[DCSIM_PP_PEAK_W * n] = w[DCSIM_PPW_PEAK];
+  o[DCSIM_PP_T_PEAK_S * n] = w[DCSIM_PPW_T_PEAK];
+  o[DCSIM_PP_OVER_S * n] = w[DCSIM_PPW_OVER_S];
+  o[DCSIM_PP_OVER_J * n] = w[DCSIM_PPW_OVER_J];
+  o[DCSIM_PP_EXCURSIONS * n] = w[DCSIM_PPW_EXC];
+  o[DCSIM_PP_LONGEST_OVER_S * n] = w[DCSIM_PPW_LONGEST];
+  o[DCSIM_PP_OUT_OF_RANGE * n] = w[DCSIM_PPW_OOR];
+  for (int d = 0; d < sp.n_dc; ++d) o[(uint64_t)(DCSIM_PP_FIELDS + d) * n] = w[DCSIM_PPW_DC_PEAK + d];
 }
 
 /* One popped event (SIM:429-467) of a replica that is `on`: the per-DC accrual with the state before the event, then
@@ -2306,6 +2465,7 @@ DCSIM_DEV uint32_t dcsim_replica_run(dcsim_ctx_t& c, bool live) {
 #endif
   if (finished && c.H->done == 0u) {
     dcsim_replica_tail(c);
+    if (c.lane == 0 && c.pp) dcsim_pp_tail(c.P, c.blk, c.r, c.now);
     if (c.lane == 0) c.H->done = 1u;
     dcsim_warp_sync();
   }
@@ -2355,14 +2515,17 @@ DCSIM_DEV void dcsim_write_summary(dcsim_ctx_t& c, double* out) {
 
 /* One replica, one launch: (init |) resume -> run -> summary.  `blk` is the working copy of the state
  * block (shared memory on the GPU), already loaded unless `fresh`; `rec` is the base the running-job record offsets
- * apply to (== blk when the records were staged with it, the block's home in HBM when only the head was: RECG). */
-template <bool CAP, bool RECG>
+ * apply to (== blk when the records were staged with it, the block's home in HBM when only the head was: RECG).
+ * PP: the power-profile recorder is compiled in (it runs when P->pp is set); a separate instantiation, so that the
+ * kernels without it keep their registers and code. */
+template <bool CAP, bool RECG, bool PP = false>
 DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char* blk, char* rec, bool fresh, bool ghost = false) {
   dcsim_ctx_t c;
   c.P = P; c.blk = blk; c.rec = rec; c.H = reinterpret_cast<dcsim_hdr_t*>(blk); c.lane = dcsim_lane();
   c.r = (uint32_t)r; /* n_replicas < 2^32 (checked by dcsim_create) */
   c.is_traced = !ghost && ((int64_t)r == P->rec.trace_replica);
   c.is_logged = !ghost && ((int64_t)r == P->rec.log_replica);
+  c.pp = PP && !ghost && P->pp != nullptr;
   if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing */
     c.seq = 0u; c.now = 0.0; c.cursor = 0u;
     return dcsim_replica_run<CAP, RECG>(c, false);

@@ -272,6 +272,48 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_dc_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
 
+    # -- power profile (ensemble.power_profile turns it into batch statistics) ----------------------------------------
+    def enable_power_profile(self, threshold=None):
+        """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records its
+        cluster power step function — peak, time and energy over ``threshold`` watts (None: no threshold), per-DC peaks
+        and a time-weighted power histogram (include/dcsim_b200.h DCSIM_PP_*).  Runs the event-loop instantiation with
+        the recorder compiled in."""
+        N.check(self._lib.dcsim_enable_power_profile(self._h, float("inf") if threshold is None else float(threshold)),
+                self._h)
+        self._pp_threshold = None if threshold is None else float(threshold)
+        self._pp_on = True
+
+    @property
+    def power_profile_enabled(self) -> bool:
+        return getattr(self, "_pp_on", False)
+
+    @property
+    def power_threshold(self):
+        """The threshold [W] of the enabled profile (None: none)."""
+        return getattr(self, "_pp_threshold", None)
+
+    def power_profile_range(self) -> float:
+        """hi [W]: the power histogram covers [0, hi] in PP_BINS bins (the library's bound, dcsim_power_profile_range)."""
+        hi = C.c_double(0.0)
+        N.check(self._lib.dcsim_power_profile_range(self._h, C.byref(hi)), self._h)
+        return float(hi.value)
+
+    def power_profile_rows(self) -> np.ndarray:
+        """[PP_FIELDS + n_dc + PP_BINS, n_replicas] float64: every replica's raw profile.  For tests and small batches."""
+        rows = np.empty((S.PP_FIELDS + self.spec.n_dc + S.PP_BINS, self.n_replicas), dtype=np.float64)
+        N.check(self._lib.dcsim_fetch_power_profile(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
+        return rows
+
+    def power_profile_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][PP_FIELDS + n_dc + PP_BINS] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_power_profile_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def power_profile_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream over the first PP_FIELDS + n_dc columns: sum (x - mean)^2 and an ENS_BINS
+        histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_power_profile_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                     C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
     # -- paired reductions (compare.py) ------------------------------------------------------------------------------
     def paired_moments_into(self, variant_summary_ptr: int, device_ptr: int):
         """Pass 1 on this (base) handle's stream against a variant's [n_replicas, SUMMARY_K] summaries on the device:
@@ -387,9 +429,14 @@ def _job_bin(sp, job_ensemble, job_ensemble_bin):
     return float(job_ensemble_bin or sp.log_interval) if job_ensemble else None
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None):
+def _pp_key(power_profile, power_threshold):
+    """The power profile's threshold as the engine cache sees it: None when the profile is off, +inf for no threshold."""
+    return (float("inf") if power_threshold is None else float(power_threshold)) if power_profile else None
+
+
+def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None):
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            bool(cluster_ensemble), job_bin)
+            bool(cluster_ensemble), job_bin, pp)
 
 
 def _drop_parked_batch_engine():
@@ -399,12 +446,13 @@ def _drop_parked_batch_engine():
 
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
-                   job_ensemble=False, job_ensemble_bin=None):
+                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
-    ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval).  A parked engine is only reused
-    by a caller that asks for the same recorders."""
+    ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
+    power-profile recorder on, threshold ``power_threshold`` watts (None: none).  A parked engine is only reused by a
+    caller that asks for the same recorders."""
     job_bin = _job_bin(sp, job_ensemble, job_ensemble_bin)
-    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin)
+    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold))
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -419,6 +467,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_cluster_ensemble()
         if job_bin is not None:
             eng.enable_job_ensemble(job_bin)
+        if power_profile:
+            eng.enable_power_profile(power_threshold)
     except BaseException:
         eng.close()
         raise
@@ -431,7 +481,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     every run() its allocations)."""
     _drop_parked_batch_engine()
     _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
-                                                        eng.job_ensemble_bin)
+                                                        eng.job_ensemble_bin,
+                                                        _pp_key(eng.power_profile_enabled, eng.power_threshold))
 
 
 def free_cached_engine():
@@ -480,18 +531,19 @@ class LoggedReplica:
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
-                      job_ensemble_bin=None):
+                      job_ensemble_bin=None, power_profile=False, power_threshold=None):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
     kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
     ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
-    window width, None = log_interval)."""
+    window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
+    None = no threshold)."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
-                             job_ensemble, job_ensemble_bin)
+                             job_ensemble, job_ensemble_bin, power_profile, power_threshold)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

@@ -478,3 +478,201 @@ def job_ensemble_from_rows(rows: np.ndarray, hist: np.ndarray, status: np.ndarra
                                                                   width_of(lo.numpy(), hi.numpy())),
                                                       (np.float64, np.int64))),
                        lat_hist, n_dc, bin_s, end_time, quantiles)
+
+
+# ---- power profile ---------------------------------------------------------------------------------------------------
+PP_FIELDS = ("profile_s", "peak_w", "t_peak_s", "over_s", "over_j", "excursions", "longest_over_s", "out_of_range")
+PP_INTEGER_FIELDS = (5, 7)                             # excursions, out_of_range: unit bins, exact quantiles
+PP_BINS = 1024                                         # DCSIM_PP_BINS
+PP_CURVE_LEVELS = (0.5, 0.1, 0.01, 0.001)              # shares of the pooled time the CSV's power_w_time row reports
+PP_CSV_HEADER = ["dc", "field", "n", "mean", "std", "min", "p05", "p25", "p50", "p75", "p95", "p99", "max"]
+PP_CSV_QUANTILES = (0.05, 0.25, 0.5, 0.75, 0.95, 0.99)
+
+
+def _pp_integral(n_cols: int) -> np.ndarray:
+    return np.isin(np.arange(n_cols), PP_INTEGER_FIELDS)
+
+
+def pp_bin_edges(hi: float) -> np.ndarray:
+    """Edges of the power histogram: PP_BINS bins of hi / PP_BINS watts over [0, hi]."""
+    return np.arange(PP_BINS + 1, dtype=np.float64) * (float(hi) / PP_BINS)
+
+
+@dataclass
+class PowerProfileResult:
+    """Batch statistics of the power profile over the replicas with status 0.  ``n`` ... ``max`` and ``quantiles``
+    ([Q, columns]) cover the columns ``columns`` — the per-replica fields (PP_FIELDS), then ``dc_peak_w`` per DC.
+    ``duration_curve``: (bin edges [PP_BINS + 1] W, pooled seconds [PP_BINS]) summed over the replicas — how long the
+    pooled simulated time spent in each power bin."""
+    columns: Tuple[Tuple[str, int], ...]               # (field, dc); dc = -1 for the per-replica fields
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray
+    hi: float
+    threshold: float                                   # +inf: none
+    duration_curve: Tuple[np.ndarray, np.ndarray]
+    pooled_energy_j: float                             # sum of the replicas' total energy
+
+    def column(self, field: str, dc: int = -1) -> int:
+        return self.columns.index((field, dc))
+
+    @property
+    def replicas(self) -> int:
+        return int(self.n[0]) if len(self.n) else 0
+
+    @property
+    def pooled_time_s(self) -> float:
+        return float(self.duration_curve[1].sum())
+
+    @property
+    def mean_power_w(self) -> float:
+        """Pooled energy / pooled profile time."""
+        t = self.pooled_time_s
+        return self.pooled_energy_j / t if t > 0 else float("nan")
+
+    @property
+    def over_share(self) -> float:
+        """Share of the pooled time above the threshold (NaN without one)."""
+        if not math.isfinite(self.threshold):
+            return float("nan")
+        t = self.pooled_time_s
+        s = float(self.mean[self.column("over_s")]) * self.replicas
+        return s / t if t > 0 else float("nan")
+
+    def time_quantiles(self, shares: Sequence[float]) -> np.ndarray:
+        """The power levels exceeded for the given shares of the pooled time (0.01: the level the cluster was at or
+        above for 1 % of the time), read off the pooled curve: the centre of the bin where the share is crossed, within
+        one bin width."""
+        edges, sec = self.duration_curve
+        total = sec.sum()
+        out = np.full(len(shares), np.nan)
+        if total <= 0:
+            return out
+        above = np.cumsum(sec[::-1])[::-1]             # time at or above the bottom of each bin
+        for i, s in enumerate(shares):
+            k = np.nonzero(above >= float(s) * total)[0]
+            b = int(k.max()) if len(k) else 0
+            out[i] = 0.5 * (edges[b] + edges[b + 1])
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """Long format: dc,field,n,mean,std,min,p05,p25,p50,p75,p95,p99,max — one row per field (dc empty), one per DC
+        for dc_peak_w; with no threshold the threshold columns are left empty.  A last ``power_w_time`` row holds the
+        pooled curve: n = replicas, mean = pooled energy / pooled time, std empty, min / max the lowest / highest occupied
+        bin's centre, the quantiles the power levels exceeded for 95 / 75 / 50 / 25 / 5 / 1 % of the pooled time."""
+        thr_fields = ("over_s", "over_j", "excursions", "longest_over_s")
+        fmt = lambda x: repr(float(x))  # noqa: E731
+        with open(path, "w", newline="") as f:
+            w = csv.writer(f)
+            w.writerow(PP_CSV_HEADER)
+            for c, (field, d) in enumerate(self.columns):
+                dc = dc_names[d] if d >= 0 else ""
+                if field in thr_fields and not math.isfinite(self.threshold):
+                    w.writerow([dc, field] + [""] * (len(PP_CSV_HEADER) - 2))
+                    continue
+                w.writerow([dc, field, int(self.n[c]), fmt(self.mean[c]), fmt(self.std[c]), fmt(self.min[c])]
+                           + [fmt(self.quantiles[j, c]) for j in range(len(self.q))] + [fmt(self.max[c])])
+            edges, sec = self.duration_curve
+            occ = np.nonzero(sec > 0)[0]
+            centre = lambda b: 0.5 * (edges[b] + edges[b + 1])  # noqa: E731
+            lo = centre(occ.min()) if len(occ) else float("nan")
+            hi = centre(occ.max()) if len(occ) else float("nan")
+            tq = self.time_quantiles([1.0 - q for q in PP_CSV_QUANTILES])
+            w.writerow(["", "power_w_time", self.replicas, fmt(self.mean_power_w), "", fmt(lo)]
+                       + [fmt(v) for v in tq] + [fmt(hi)])
+
+
+def pp_finalize(mom, m2, hist, n_dc: int, hi: float, threshold: float, energy: float,
+                quantiles: Sequence[float] = PP_CSV_QUANTILES) -> PowerProfileResult:
+    """All-reduced moments [4, PP_FIELDS + n_dc + PP_BINS], m2 and histograms over the first PP_FIELDS + n_dc columns,
+    and the pooled energy -> statistics."""
+    n_all, s, lo, mx = (np.asarray(a, dtype=np.float64) for a in mom)
+    c = len(PP_FIELDS) + n_dc
+    n, s_c, lo_c, mx_c, m2 = n_all[:c], s[:c], lo[:c], mx[:c], np.asarray(m2, dtype=np.float64)[:c]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mean = np.where(n > 0, s_c / n, np.nan)
+        std = np.where(n > 1, np.sqrt(m2 / (n - 1)), np.where(n == 1, 0.0, np.nan))
+    empty = n == 0
+    integral = _pp_integral(c)
+    qv = hist_quantiles(np.asarray(hist)[:c], n, lo_c, mx_c, bin_widths_for(lo_c, mx_c, integral), integral, quantiles)
+    columns = tuple((f, -1) for f in PP_FIELDS) + tuple(("dc_peak_w", d) for d in range(n_dc))
+    return PowerProfileResult(columns=columns, n=n.astype(np.int64), mean=mean, std=std,
+                              min=np.where(empty, np.nan, lo_c), max=np.where(empty, np.nan, mx_c),
+                              q=tuple(float(q) for q in quantiles), quantiles=qv, hi=float(hi), threshold=float(threshold),
+                              duration_curve=(pp_bin_edges(hi), s[c:c + PP_BINS].copy()), pooled_energy_j=float(energy))
+
+
+def _pp_passes(moments_fn, spread_fn, energy, n_dc, hi, threshold, quantiles):
+    """The two passes, then the pooled energy (a float64 torch scalar tensor) all-reduced."""
+    import torch.distributed as dist
+    mom, m2, hist = two_passes(moments_fn, spread_fn)
+    e = float(_allreduce(energy, dist.ReduceOp.SUM).cpu().numpy().reshape(-1)[0])
+    return pp_finalize(mom, m2, hist, n_dc, hi, threshold, e, quantiles)
+
+
+def _good_energy(summary: np.ndarray):
+    import torch
+    from . import spec as S
+    s = np.asarray(summary)
+    good = s[:, S.S_STATUS] == 0
+    return torch.tensor([float(s[good, S.S_TOTAL_ENERGY_J].sum())], dtype=torch.float64)
+
+
+def power_profile(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES, summary=None) -> PowerProfileResult:
+    """Statistics of the power profile of ``engine`` (a finished BatchedEngine with enable_power_profile()), over all
+    ranks when torch.distributed runs with world > 1 (every rank calls this).  ``summary``: the engine's summary rows if
+    the caller has them already (they give the pooled energy)."""
+    import torch
+    if not engine.power_profile_enabled:
+        raise RuntimeError("power profile not enabled (enable_power_profile)")
+    dev = torch.device("cuda", engine.device)
+    n_dc = engine.spec.n_dc
+    cols, stat_cols = len(PP_FIELDS) + n_dc + PP_BINS, len(PP_FIELDS) + n_dc
+
+    def moments():
+        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
+        torch.cuda.synchronize(dev)                    # the library runs on the handle's stream, torch on its own
+        engine.power_profile_moments_into(out.data_ptr())
+        torch.cuda.synchronize(dev)
+        return out
+
+    def spread(mean, lo, hi):
+        m2 = torch.zeros(stat_cols, dtype=torch.float64, device=dev)
+        hist = torch.zeros((stat_cols, BINS), dtype=torch.int64, device=dev)
+        torch.cuda.synchronize(dev)
+        engine.power_profile_spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
+        torch.cuda.synchronize(dev)
+        return m2, hist
+
+    energy = _good_energy(engine.summary() if summary is None else summary).to(dev)
+    thr = engine.power_threshold
+    return _pp_passes(moments, spread, energy, n_dc, engine.power_profile_range(),
+                      float("inf") if thr is None else thr, quantiles)
+
+
+def power_profile_from_rows(rows: np.ndarray, summary: np.ndarray, hi: float, threshold=None,
+                            quantiles: Sequence[float] = PP_CSV_QUANTILES) -> PowerProfileResult:
+    """The same statistics from host rows [PP_FIELDS + n_dc + PP_BINS, R] (BatchedEngine.power_profile_rows) and the
+    summary rows [R, SUMMARY_K] through the numpy mirror of both passes; replicas with status != 0 are left out.
+    All-reduced over the ranks like power_profile."""
+    import torch
+    from . import spec as S
+    rows = np.asarray(rows, dtype=np.float64)
+    n_dc = rows.shape[0] - len(PP_FIELDS) - PP_BINS
+    stat_cols = len(PP_FIELDS) + n_dc
+    good = np.asarray(summary)[:, S.S_STATUS] == 0
+    ok = np.broadcast_to(good[None, :], rows.shape)
+    integral = _pp_integral(stat_cols)
+    return _pp_passes(lambda: torch.from_numpy(moments_cols(rows, ok)),
+                      lambda mean, lo, hi_: tuple(torch.from_numpy(np.ascontiguousarray(a).astype(dt)) for a, dt in
+                                                  zip(spread_cols(rows[:stat_cols], ok[:stat_cols], mean.numpy()[:stat_cols],
+                                                                  lo.numpy()[:stat_cols],
+                                                                  hi_.numpy()[:stat_cols],
+                                                                  bin_widths_for(lo.numpy()[:stat_cols], hi_.numpy()[:stat_cols],
+                                                                                 integral)),
+                                                      (np.float64, np.int64))),
+                      _good_energy(summary), n_dc, hi, float("inf") if threshold is None else float(threshold), quantiles)

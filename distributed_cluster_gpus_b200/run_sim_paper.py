@@ -66,6 +66,12 @@ def parse_args(argv=None):
                         "latencies per job type over all replicas (long format), and per-DC latency quantiles, to this file")
     p.add_argument("--job-ensemble-bin", type=float, default=None, metavar="SECONDS",
                    help="finish-window width of --job-ensemble-csv (default: --log-interval)")
+    p.add_argument("--power-profile-csv", type=str, default=None, metavar="PATH",
+                   help="write batch statistics of every replica's cluster power over time — peak, time and energy over "
+                        "--power-threshold, longest excursion, per-DC peaks — and the pooled power-duration curve's "
+                        "quantiles (long format) to this file")
+    p.add_argument("--power-threshold", type=float, default=None, metavar="W",
+                   help="threshold of --power-profile-csv (default: --power-cap when it is > 0, else none)")
     p.add_argument("--compare-algos", type=str, default=None, metavar="A,B,...",
                    help="run every listed algo on the scenario of the other flags, on the same replica keys, and compare "
                         "each with the FIRST (the baseline) replica by replica; algos that draw the same arrivals share "
@@ -107,8 +113,16 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         replicas=args.replicas if replicas is None else replicas, first_replica_id=first_replica_id,
         device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
         cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
-        job_ensemble_bin=args.job_ensemble_bin)
+        job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
+        power_threshold=power_threshold(args))
     return sim
+
+
+def power_threshold(args):
+    """--power-threshold, else --power-cap when it is > 0, else None (no threshold)."""
+    if args.power_threshold is not None:
+        return float(args.power_threshold)
+    return float(args.power_cap) if args.power_cap > 0 else None
 
 
 def _launch_workers(args, argv):
@@ -137,6 +151,7 @@ def main(argv=None):
     _write_ensemble(args, sim)
     stats = batch_statistics(sim.summary)
     _add_latency_quantiles(stats, sim.latency_histogram)
+    _add_power_profile(stats, sim.power_profile)
     _report(args, stats)
     return sim
 
@@ -146,6 +161,24 @@ def _write_ensemble(args, sim):
         sim.cluster_ensemble.to_csv(args.ensemble_csv, [dc.name for dc in sim.dcs.values()])
     if args.job_ensemble_csv:
         sim.job_ensemble.to_csv(args.job_ensemble_csv, [dc.name for dc in sim.dcs.values()])
+    if args.power_profile_csv:
+        sim.power_profile.to_csv(args.power_profile_csv, [dc.name for dc in sim.dcs.values()])
+
+
+def _add_power_profile(stats, res):
+    """The batch figures of the power profile for --summary-json."""
+    if res is None:
+        return
+    col = lambda f: res.column(f)  # noqa: E731
+    thr = res.threshold if np.isfinite(res.threshold) else None
+    out = {"replicas": res.replicas, "threshold_w": thr, "hi_w": res.hi, "mean_power_w": res.mean_power_w,
+           "peak_w_mean": float(res.mean[col("peak_w")]), "peak_w_max": float(res.max[col("peak_w")]),
+           "power_w_exceeded_50_10_1_0.1pct": [float(v) for v in res.time_quantiles([0.5, 0.1, 0.01, 0.001])]}
+    if thr is not None:
+        out.update({"over_s_mean": float(res.mean[col("over_s")]), "over_j_mean": float(res.mean[col("over_j")]),
+                    "excursions_mean": float(res.mean[col("excursions")]),
+                    "longest_over_s_max": float(res.max[col("longest_over_s")]), "over_share": res.over_share})
+    stats["power_profile"] = out
 
 
 def _add_latency_quantiles(stats, hist):
@@ -186,6 +219,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--ensemble-csv needs at least one replica per rank")
     if args.job_ensemble_csv and count == 0:
         raise SystemExit("--job-ensemble-csv needs at least one replica per rank")
+    if args.power_profile_csv and count == 0:
+        raise SystemExit("--power-profile-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -219,6 +254,7 @@ def _main_sharded(args, world, rank):
                  "mean_latency_s_mean": stats["mean_latency_s_mean"], "mean_latency_s_ci95": ci(stats["mean_latency_s_var"]),
                  "mean_latency_s_p05_p50_p95": [float(q) for q in np.percentile(cols[1][keep], [5, 50, 95])]}
         _add_latency_quantiles(stats, hist.cpu().numpy().astype(np.uint64))
+        _add_power_profile(stats, sim.power_profile)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -236,6 +272,9 @@ def _main_compare(args, world, rank):
     unknown = [a for a in algos if a not in ALGOS]
     if unknown:
         raise SystemExit(f"--compare-algos: unknown algo(s) {unknown}; choose from {ALGOS}")
+    if args.power_profile_csv or args.power_threshold is not None:
+        raise SystemExit("--power-profile-csv / --power-threshold are not available with --compare-algos (run each algo "
+                         "on its own)")
     if args.ensemble_csv or args.job_ensemble_csv:
         raise SystemExit("--ensemble-csv / --job-ensemble-csv are not available with --compare-algos (run each algo "
                          "on its own for its cluster-log and job-log ensembles)")

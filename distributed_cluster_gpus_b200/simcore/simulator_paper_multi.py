@@ -60,7 +60,8 @@ class MultiIngressPaperSimulator:
                  # --- batched-engine additions (keyword only in spirit; defaults reproduce one trajectory) ---
                  replicas: int = 1, device: int = 0, first_replica_id: int = 0, write_logs: bool = True,
                  cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
-                 job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None):
+                 job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None, power_profile: bool = False,
+                 power_threshold: Optional[float] = None):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -103,6 +104,11 @@ class MultiIngressPaperSimulator:
         # ensemble.JobEnsembleResult
         self._want_job_ensemble, self._job_ensemble_bin = bool(job_ensemble), job_ensemble_bin
         self.job_ensemble = None
+        # power_profile=True: after run(), batch statistics of every replica's cluster power step function — peak, time
+        # and energy over power_threshold watts (None: no threshold), per-DC peaks and the pooled power-duration curve
+        # (all ranks, as above), ensemble.PowerProfileResult
+        self._want_power_profile, self._power_threshold = bool(power_profile), power_threshold
+        self.power_profile = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -154,7 +160,8 @@ class MultiIngressPaperSimulator:
             eng, summ = run_to_completion(self._flatten, self.replicas, self.rng_seed, self.first_replica_id, self.device,
                                           self.cuda_stream, configure=configure, while_running=while_running,
                                           cluster_ensemble=self._want_ensemble, job_ensemble=self._want_job_ensemble,
-                                          job_ensemble_bin=self._job_ensemble_bin)
+                                          job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
+                                          power_threshold=self._power_threshold)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -169,6 +176,9 @@ class MultiIngressPaperSimulator:
             if self._want_job_ensemble:
                 from ..ensemble import job_ensemble
                 self.job_ensemble = job_ensemble(eng)
+            if self._want_power_profile:
+                from ..ensemble import power_profile
+                self.power_profile = power_profile(eng, summary=summ)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

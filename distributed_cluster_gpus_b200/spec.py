@@ -40,6 +40,9 @@ ST_ARRIVALS_OVERFLOW, ST_ARRIVAL_TIE, ST_SEQ_OVERFLOW = 32, 64, 128
 A_REPLICAS, A_FAILED, A_EVENTS, A_JOBS, A_ENERGY, A_ENERGY_SQ, A_LAT_SUM, A_MEANLAT_SUM, A_MEANLAT_SQ, A_RNG_WORDS = range(10)
 A_RUNNING = 11
 AGG_K = 16
+# power-profile columns (DCSIM_PP_*): the fields, then DC_PEAK_W per DC, then PP_BINS histogram bins
+PP_PROFILE_S, PP_PEAK_W, PP_T_PEAK_S, PP_OVER_S, PP_OVER_J, PP_EXCURSIONS, PP_LONGEST_OVER_S, PP_OUT_OF_RANGE = range(8)
+PP_FIELDS, PP_BINS = 8, 1024
 
 
 class Coeffs(C.Structure):

@@ -401,6 +401,51 @@ int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* 
 /* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
+/* Power profile: for EVERY replica, the cluster power P(t) its total energy integrates, as a step function, and what a
+ * site is sized by — peak, time and energy over a threshold, a time-weighted power histogram.
+ *   - Each inter-event interval (t_{k-1}, t_k] of positive length has power sum_d P_d, summed in DC order from 0.0,
+ *     P_d being the estimate the per-event accrual uses (SIM:168-179, 437) as it stood after event k-1; the tail
+ *     (t_last, end_time] has the tail's own power (instantaneous_power_w at current_freq, models.py:82-91, SIM:475).
+ *   - The profile starts at the first processed event (DCSIM_S_UTIL_BEGIN); a replica without one has an empty profile
+ *     (every field 0).  Zero-length intervals are ignored.
+ *   - Consecutive intervals of bitwise-equal power form one LEVEL, whose length is its end minus its start.
+ * Per replica (threshold compared with a strict >, +inf = none):
+ *   PROFILE_S        end_time - the first event's instant
+ *   PEAK_W           largest level power;  T_PEAK_S  start of the first level at it
+ *   OVER_S / OVER_J  total length of the levels above the threshold / sum (power - threshold) * length over them
+ *   EXCURSIONS       maximal runs of consecutive levels above the threshold;  LONGEST_OVER_S  the longest, end - start
+ *   OUT_OF_RANGE     levels outside the histogram range [0, hi], clamped into the end bins: must be 0, never silent
+ *   then DC_PEAK_W[d] largest P_d over the positive-length intervals (tail included), then DCSIM_PP_BINS bins of
+ *   seconds over [0, hi]: bin = min(BINS - 1, floor(P / (hi / BINS))), each level adding its length to its bin in level
+ *   order.
+ * Device layout [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] doubles, replica fastest. */
+enum {
+  DCSIM_PP_PROFILE_S = 0, DCSIM_PP_PEAK_W = 1, DCSIM_PP_T_PEAK_S = 2, DCSIM_PP_OVER_S = 3, DCSIM_PP_OVER_J = 4,
+  DCSIM_PP_EXCURSIONS = 5, DCSIM_PP_LONGEST_OVER_S = 6, DCSIM_PP_OUT_OF_RANGE = 7,
+  DCSIM_PP_FIELDS = 8 /* then n_dc DC_PEAK_W columns, then DCSIM_PP_BINS histogram columns */
+};
+#define DCSIM_PP_BINS 1024
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  threshold_w = +inf: no
+ * threshold (the OVER_* / EXCURSIONS fields stay 0).  DCSIM_E_INVALID for a NaN or negative threshold, DCSIM_E_STATE
+ * after the first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error)
+ * when the rows do not fit. */
+int dcsim_enable_power_profile(dcsim_t* h, double threshold_w);
+/* hi: the histogram's upper end, an upper bound on the cluster power of any state the spec allows — sum over DCs of
+ * total_gpus * max(idle or sleep power, per-GPU busy power at every (job type, frequency) a job can run at, the tail
+ * formula's per-GPU active power at those frequencies), times (1 + 2^-20) for the rounding of the sums.  Host only;
+ * works whether or not the profile is enabled. */
+int dcsim_power_profile_range(dcsim_t* h, double* hi_out);
+/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
+int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes);
+/* Pass 1 over every column (the fields, DC_PEAK_W, the bins) and the replicas with status 0: dev_out =
+ * [4][DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS] {n, sum, min, max}; the bins' sums are the pooled power-duration curve.
+ * Pass 2 over the first DCSIM_PP_FIELDS + n_dc columns only (the bins need no spread): m2 and histograms, the contract
+ * of dcsim_ensemble_spread; EXCURSIONS and OUT_OF_RANGE are the integer columns.  Both on the handle's stream, with
+ * device pointers. */
+int dcsim_power_profile_moments(dcsim_t* h, double* dev_out);
+int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                               double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant
  * batch with the same keys (a member's dcsim_summary_device_ptr or a copy of it: [n][DCSIM_SUMMARY_K] doubles on the
  * base's device).  Replica r counts in a column when both rows have status 0 and the metric is defined in both (a

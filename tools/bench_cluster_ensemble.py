@@ -1,9 +1,9 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job, the job-log ensemble) at bench size: the event loop with
+"""Cost of the cluster-log ensemble (or, with --recorder job / power, the job-log ensemble / the power profile) at bench size: the event loop with
 the recorder off and on, the two reduction kernels, the recorder's bytes per replica.  One JSON line on stdout; writes
 nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
@@ -28,7 +28,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -47,6 +47,8 @@ def main():
         e = BatchedEngine(sp, n, base_seed=seed, cuda_stream=stream.cuda_stream)
         if arm == "on" and args.recorder == "job":
             e.enable_job_ensemble()
+        elif arm == "on" and args.recorder == "power":
+            e.enable_power_profile(sp.power_cap if sp.power_cap > 0 else None)
         elif arm == "on":
             e.enable_cluster_ensemble()
         return e
@@ -64,7 +66,11 @@ def main():
     try:
         on.advance(0)
         events = float(on.summary()[:, S.S_EVENTS].sum())
-        if args.recorder == "job":
+        if args.recorder == "power":
+            cols = S.PP_FIELDS + sp.n_dc + S.PP_BINS
+            moments_into, spread_into = on.power_profile_moments_into, on.power_profile_spread_into
+            rows, recorder_bytes = cols, cols * 8 + 20 * 8      # columns + the working row (DCSIM_PPW_N doubles)
+        elif args.recorder == "job":
             cols = (on.job_ensemble_windows + 1) * len(EN.JOB_FIELDS) * sp.n_dc * 2
             moments_into, spread_into = on.job_ensemble_moments_into, on.job_ensemble_spread_into
             rows, recorder_bytes = on.job_ensemble_windows + 1, ((on.job_ensemble_windows + 1) * 2 * sp.n_dc * 2 * 8
