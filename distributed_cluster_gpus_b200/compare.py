@@ -12,6 +12,7 @@ counts when both runs ended with status 0 and the metric is defined in both.  ``
 mirror of the two kernels (csrc dcsim_ens_pair_src).
 """
 import csv
+import functools
 from dataclasses import dataclass
 from typing import Callable, Dict, Sequence, Tuple
 
@@ -107,15 +108,13 @@ def paired_finalize(mom, m2, hist, n_dc: int, quantiles: Sequence[float] = EN.DE
     F = len(PAIR_FIELDS)
     mom = np.asarray(mom, dtype=np.float64)
     m2 = np.asarray(m2, dtype=np.float64)
-    n_all, s, lo, hi = mom
-    M = n_all.size // F
-    with np.errstate(invalid="ignore", divide="ignore"):
-        mean = np.where(n_all > 0, s / n_all, np.nan).reshape(M, F)
-        var = np.where(n_all > 1, m2 / (n_all - 1), np.where(n_all == 1, 0.0, np.nan)).reshape(M, F)
-    n = n_all.reshape(M, F)[:, DIFF]
+    st = EN.column_stats(mom, m2, hist, _integral(n_dc), quantiles)
+    M = st.n.size // F
+    mean, var = st.mean.reshape(M, F), st.var.reshape(M, F)
+    n = st.n.reshape(M, F)[:, DIFF]
     mb, mv, md = mean[:, BASE], mean[:, VARIANT], mean[:, DIFF]
     vb, vv, vd = var[:, BASE], var[:, VARIANT], var[:, DIFF]
-    sd = np.sqrt(vd)
+    sd = st.std.reshape(M, F)[:, DIFF]
     with np.errstate(invalid="ignore", divide="ignore"):
         half = np.where(n > 1, 1.96 * sd / np.sqrt(np.maximum(n, 1)), 0.0)
         rel = mv / mb - 1.0
@@ -123,13 +122,11 @@ def paired_finalize(mom, m2, hist, n_dc: int, quantiles: Sequence[float] = EN.DE
         var_rel = (vv / mb ** 2 - 2.0 * mv * cov / mb ** 3 + mv ** 2 * vb / mb ** 4) / np.maximum(n, 1)
         rel_half = np.where(n > 1, 1.96 * np.sqrt(np.maximum(var_rel, 0.0)), 0.0)
         var_ratio = vd / (vb + vv)
-    integral = _integral(n_dc)
-    width = EN.bin_widths_for(lo, hi, integral)
-    qv = EN.hist_quantiles(np.asarray(hist), n_all, lo, hi, width, integral, quantiles).reshape(len(quantiles), M, F)
-    return PairedStats(metrics=metric_names(n_dc), n=n.astype(np.int64), base_mean=mb, variant_mean=mv, diff_mean=md,
+    qv = st.quantiles.reshape(len(quantiles), M, F)
+    return PairedStats(metrics=metric_names(n_dc), n=n, base_mean=mb, variant_mean=mv, diff_mean=md,
                        diff_std=sd, diff_ci95_lo=md - half, diff_ci95_hi=md + half, rel_change=rel,
                        rel_ci95_lo=rel - rel_half, rel_ci95_hi=rel + rel_half, frac_lower=mean[:, LOWER],
-                       frac_higher=mean[:, HIGHER], var_ratio=var_ratio, q=tuple(float(x) for x in quantiles),
+                       frac_higher=mean[:, HIGHER], var_ratio=var_ratio, q=st.q,
                        diff_quantiles=qv[:, :, DIFF], moments=mom, m2=m2, hist=np.asarray(hist))
 
 
@@ -138,21 +135,13 @@ def paired_from_summaries(base: np.ndarray, variant: np.ndarray, quantiles: Sequ
     """The same statistics from host summary rows [R, SUMMARY_K] of the two runs (the same replica keys, row r = replica
     r) through the numpy mirror of both passes, all-reduced over the ranks like ``compare_variants``.  ``n_dc``: the
     scenario's DC count (None: the DC groups that are not all zero in either run)."""
-    import torch
     base, variant = np.asarray(base, dtype=np.float64), np.asarray(variant, dtype=np.float64)
     if n_dc is None:
         groups = np.abs(np.concatenate([base, variant]))[:, S.S_DC0:].reshape(-1, S.MAX_DC, S.S_DC_STRIDE)
         used = np.nonzero(groups.sum(axis=(0, 2)) > 0)[0]
         n_dc = int(used.max()) + 1 if used.size else 1
     x, ok = pair_columns(base, variant, n_dc)
-    integral = _integral(n_dc)
-    mom, m2, hist = EN.two_passes(
-        lambda: torch.from_numpy(EN.moments_cols(x, ok)),
-        lambda mean, lo, hi: tuple(torch.from_numpy(np.ascontiguousarray(a).astype(dt)) for a, dt in
-                                   zip(EN.spread_cols(x, ok, mean.numpy(), lo.numpy(), hi.numpy(),
-                                                      EN.bin_widths_for(lo.numpy(), hi.numpy(), integral)),
-                                       (np.float64, np.int64))))
-    return paired_finalize(mom, m2, hist, n_dc, quantiles)
+    return paired_finalize(*EN.host_passes(x, ok, _integral(n_dc)), n_dc, quantiles)
 
 
 @dataclass
@@ -310,23 +299,7 @@ def compare_variants(variants: Dict[str, Callable], baseline: str, n_replicas: i
 
 def _paired_on_device(base, variant_summary, n_dc, dev, quantiles):
     """The two passes of the paired kernels on the base engine's stream, all-reduced over the ranks."""
-    import torch
-    cols = n_columns(n_dc)
     vptr = variant_summary.data_ptr()
-
-    def moments():
-        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
-        torch.cuda.synchronize(dev)                    # the library runs on the handle's stream, torch on its own
-        base.paired_moments_into(vptr, out.data_ptr())
-        torch.cuda.synchronize(dev)
-        return out
-
-    def spread(mean, lo, hi):
-        m2 = torch.zeros(cols, dtype=torch.float64, device=dev)
-        hist = torch.zeros((cols, EN.BINS), dtype=torch.int64, device=dev)
-        torch.cuda.synchronize(dev)
-        base.paired_spread_into(vptr, mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
-        torch.cuda.synchronize(dev)
-        return m2, hist
-
-    return paired_finalize(*EN.two_passes(moments, spread), n_dc, quantiles)
+    passes = EN.device_passes(dev, n_columns(n_dc), functools.partial(base.paired_moments_into, vptr),
+                              functools.partial(base.paired_spread_into, vptr))
+    return paired_finalize(*passes, n_dc, quantiles)

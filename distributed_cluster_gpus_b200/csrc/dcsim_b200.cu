@@ -443,14 +443,14 @@ struct dcsim {
   uint32_t ens_cap;
   double* d_jens;          /* [jens_windows + 1][DCSIM_JENS_STORED][n_dc][2][n_replicas] job-log ensemble (opt-in) */
   uint32_t* d_jens_hist;   /* [n_replicas][n_dc][2][DCSIM_LAT_BINS] its per-DC latency histograms */
-  uint32_t* d_jens_status; /* [n_replicas] status words (+ 1 word: their maximum), refreshed by every reduction */
   unsigned long long* d_jens_hist_out; /* [n_dc][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_latency_histogram */
   double jens_bin;
   uint64_t jens_windows;
   double* d_pp;            /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile (opt-in) */
   double* d_pp_work;       /* [n_replicas][DCSIM_PPW_N] its working state */
-  uint32_t* d_pp_status;   /* [n_replicas] status words (+ 1 word), refreshed by every reduction */
   double pp_threshold;
+  uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the job ensemble and power profile
+                         reductions, refreshed on the stream ahead of every one of them (status_words) */
   unsigned long long events_seen;
   char err[512];
 };
@@ -485,6 +485,82 @@ static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", lo
       return set_err(h, e_ == cudaErrorMemoryAllocation ? DCSIM_E_NOMEM : DCSIM_E_CUDA,    \
                      "CUDA error: %s (line %lld)", cudaGetErrorString(e_), (long long)__LINE__); \
   } while (0)
+
+/* The device buffers of an opt-in recorder: *a and, when b is given, *b — both or neither.  Running out of device memory
+ * is DCSIM_E_NOMEM with `need` bytes in the message `nomem_fmt`, and clears the sticky error: the handle stays usable. */
+static int recorder_alloc(dcsim_t* h, void** a, size_t a_bytes, void** b, size_t b_bytes, const char* nomem_fmt, long long need) {
+  cudaError_t e = cudaMalloc(a, a_bytes);
+  if (e != cudaSuccess) *a = NULL;
+  else if (b && (e = cudaMalloc(b, b_bytes)) != cudaSuccess) { cudaFree(*a); *a = NULL; *b = NULL; }
+  if (e == cudaSuccess) return DCSIM_OK;
+  if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
+  cudaGetLastError();
+  return set_err(h, DCSIM_E_NOMEM, nomem_fmt, "", need);
+}
+
+/* A read of an opt-in recorder (`rec`; NULL: not enabled) needs it enabled and the batch advanced. */
+static int recorder_ready(dcsim_t* h, const void* rec, const char* what, const char* enable_fn) {
+  if (!rec) { snprintf(h->err, sizeof(h->err), "%s not enabled (%s)", what, enable_fn); return DCSIM_E_STATE; }
+  if (!h->launches) { snprintf(h->err, sizeof(h->err), "%s read before the first advance", what); return DCSIM_E_STATE; }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  return DCSIM_OK;
+}
+
+/* Column `field` of every replica's summary row into out[0, n_replicas), their maximum into out[n_replicas]. */
+static int summary_counts(dcsim_t* h, int field, uint32_t* out) {
+  CUDA_TRY(h, cudaMemsetAsync(out + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
+  int blocks = (int)((h->n_replicas + 255) / 256);
+  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
+  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, field, out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+/* Before a reduction over the job ensemble or the power profile (`rec`, checked as by recorder_ready): every replica's
+ * status word into d_status, on the stream, where the reduction that reads it follows. */
+static int status_words(dcsim_t* h, const void* rec, const char* what, const char* enable_fn) {
+  const int rc = recorder_ready(h, rec, what, enable_fn);
+  return rc != DCSIM_OK ? rc : summary_counts(h, DCSIM_S_STATUS, h->d_status);
+}
+
+/* Sums the per-replica histogram rows hist[n_replicas][row_len] (without the replicas whose `status` word is not 0, when
+ * given) into the device scratch `sum`, then copies that to the host `out`; synchronises. */
+static cudaError_t hist_reduce(dcsim_t* h, const uint32_t* hist, uint32_t row_len, const uint32_t* status,
+                               unsigned long long* sum, uint64_t* out) {
+  const size_t bytes = (size_t)row_len * sizeof(uint64_t);
+  cudaError_t e = cudaMemsetAsync(sum, 0, bytes, h->g->stream);
+  if (e == cudaSuccess) {
+    int blocks = 8 * h->sm_count;
+    if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
+    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->g->stream>>>(hist, h->n_replicas, row_len, status, sum);
+    e = cudaGetLastError();
+  }
+  if (e == cudaSuccess) e = cudaMemcpyAsync(out, sum, bytes, cudaMemcpyDeviceToHost, h->g->stream);
+  if (e == cudaSuccess) e = cudaStreamSynchronize(h->g->stream);
+  return e;
+}
+
+/* The two passes of a batch-wide statistic over the n_cols columns of `src` (n replicas) on the handle's stream: one CTA
+ * per column, at most 2^20 CTAs (the kernels stride over the rest). */
+static int ens_grid(uint64_t n_cols) { return (int)(n_cols < (1ull << 20) ? n_cols : (1ull << 20)); }
+
+template <class Src>
+static int ens_moments(dcsim_t* h, const Src& src, uint64_t n, uint64_t n_cols, double* dev_out) {
+  if (!n_cols) return DCSIM_OK;
+  dcsim_ens_moments_kernel<<<ens_grid(n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, n, n_cols, dev_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
+
+template <class Src>
+static int ens_spread(dcsim_t* h, const Src& src, uint64_t n, uint64_t n_cols, const double* dev_mean, const double* dev_lo,
+                      const double* dev_hi, double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!n_cols) return DCSIM_OK;
+  dcsim_ens_spread_kernel<<<ens_grid(n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, n, n_cols, dev_mean, dev_lo, dev_hi,
+                                                                                   dev_m2_out, (unsigned long long*)dev_hist_out);
+  CUDA_TRY(h, cudaGetLastError());
+  return DCSIM_OK;
+}
 
 extern "C" {
 
@@ -1069,16 +1145,7 @@ int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_latency_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
   if (!h->launches) return set_err(h, DCSIM_E_STATE, "fetch_latency_histogram before the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  unsigned long long* d_out = h->d_hist_out;
-  cudaError_t e = cudaMemsetAsync(d_out, 0, need, h->g->stream);
-  if (e == cudaSuccess) {
-    int blocks = 8 * h->sm_count;
-    if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
-    dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->g->stream>>>(h->d_hist, h->n_replicas, 2 * DCSIM_LAT_BINS, NULL, d_out);
-    e = cudaGetLastError();
-  }
-  if (e == cudaSuccess) e = cudaMemcpyAsync(out, d_out, need, cudaMemcpyDeviceToHost, h->g->stream);
-  if (e == cudaSuccess) e = cudaStreamSynchronize(h->g->stream);
+  const cudaError_t e = hist_reduce(h, h->d_hist, 2 * DCSIM_LAT_BINS, NULL, h->d_hist_out, out);
   if (e != cudaSuccess) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
   return DCSIM_OK;
 }
@@ -1092,14 +1159,9 @@ int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks) {
   if (h->d_ens) { cudaFree(h->d_ens); h->d_ens = NULL; h->ens_cap = 0; }
   if (!h->d_ens_nlog) CUDA_TRY(h, cudaMalloc(&h->d_ens_nlog, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
   const size_t bytes = ens_bytes(h, ticks);
-  const cudaError_t e = cudaMalloc(&h->d_ens, bytes ? bytes : sizeof(double));
-  if (e != cudaSuccess) {
-    h->d_ens = NULL;
-    if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
-    cudaGetLastError();
-    return set_err(h, DCSIM_E_NOMEM, "enable_cluster_ensemble: %s%lld bytes of device memory do not fit (run fewer replicas)", "",
-                   (long long)bytes);
-  }
+  const int rc = recorder_alloc(h, (void**)&h->d_ens, bytes ? bytes : sizeof(double), NULL, 0,
+                                "enable_cluster_ensemble: %s%lld bytes of device memory do not fit (run fewer replicas)", (long long)bytes);
+  if (rc != DCSIM_OK) return rc;
   h->ens_cap = ticks;
   CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, bytes, h->g->stream)); /* NaN: not recorded */
   return DCSIM_OK;
@@ -1113,14 +1175,9 @@ int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out) {
 
 /* Every replica's recorded tick count into d_ens_nlog; fails when one of them went past the capacity (synchronises). */
 static int ens_counts(dcsim_t* h) {
-  if (!h->d_ens) return set_err(h, DCSIM_E_STATE, "cluster ensemble not enabled (dcsim_enable_cluster_ensemble)%s%lld");
-  if (!h->launches) return set_err(h, DCSIM_E_STATE, "cluster ensemble read before the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_ens_nlog + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
-  int blocks = (int)((h->n_replicas + 255) / 256);
-  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_EV_LOG, h->d_ens_nlog);
-  CUDA_TRY(h, cudaGetLastError());
+  int rc = recorder_ready(h, h->d_ens, "cluster ensemble", "dcsim_enable_cluster_ensemble");
+  if (rc == DCSIM_OK) rc = summary_counts(h, DCSIM_S_EV_LOG, h->d_ens_nlog);
+  if (rc != DCSIM_OK) return rc;
   uint32_t most = 0u;
   CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
@@ -1145,19 +1202,13 @@ int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
-static int ens_grid(const dcsim_t* h, uint64_t n_cols) { return (int)(n_cols < (1ull << 20) ? (n_cols ? n_cols : 1ull) : (1ull << 20)); }
-
 int dcsim_ensemble_moments(dcsim_t* h, double* dev_out) {
   if (!h || !dev_out) return DCSIM_E_INVALID;
   const int rc = ens_counts(h);
   if (rc != DCSIM_OK) return rc;
   const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
-  const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
-  if (!n_cols) return DCSIM_OK;
   const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  return ens_moments(h, src, h->n_replicas, (uint64_t)h->ens_cap * cols_per_tick, dev_out);
 }
 
 int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
@@ -1166,13 +1217,8 @@ int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_
   const int rc = ens_counts(h);
   if (rc != DCSIM_OK) return rc;
   const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
-  const uint64_t n_cols = (uint64_t)h->ens_cap * cols_per_tick;
-  if (!n_cols) return DCSIM_OK;
   const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
-                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  return ens_spread(h, src, h->n_replicas, (uint64_t)h->ens_cap * cols_per_tick, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
 static int pair_check(dcsim_t* base, const double* dev_variant_summary, uint64_t n) {
@@ -1190,11 +1236,8 @@ int dcsim_paired_moments(dcsim_t* base, const double* dev_variant_summary, uint6
   if (!dev_out) return DCSIM_E_INVALID;
   const int rc = pair_check(base, dev_variant_summary, n);
   if (rc != DCSIM_OK) return rc;
-  const uint64_t n_cols = pair_cols(base);
   const dcsim_ens_pair_src src{base->d_summary, dev_variant_summary, base->spec.n_dc};
-  dcsim_ens_moments_kernel<<<ens_grid(base, n_cols), DCSIM_ENS_THREADS, 0, base->g->stream>>>(src, n, n_cols, dev_out);
-  CUDA_TRY(base, cudaGetLastError());
-  return DCSIM_OK;
+  return ens_moments(base, src, n, pair_cols(base), dev_out);
 }
 
 int dcsim_paired_spread(dcsim_t* base, const double* dev_variant_summary, uint64_t n, const double* dev_mean,
@@ -1202,12 +1245,8 @@ int dcsim_paired_spread(dcsim_t* base, const double* dev_variant_summary, uint64
   if (!dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
   const int rc = pair_check(base, dev_variant_summary, n);
   if (rc != DCSIM_OK) return rc;
-  const uint64_t n_cols = pair_cols(base);
   const dcsim_ens_pair_src src{base->d_summary, dev_variant_summary, base->spec.n_dc};
-  dcsim_ens_spread_kernel<<<ens_grid(base, n_cols), DCSIM_ENS_THREADS, 0, base->g->stream>>>(src, n, n_cols, dev_mean, dev_lo, dev_hi,
-                                                                                          dev_m2_out, (unsigned long long*)dev_hist_out);
-  CUDA_TRY(base, cudaGetLastError());
-  return DCSIM_OK;
+  return ens_spread(base, src, n, pair_cols(base), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
 int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
@@ -1222,20 +1261,13 @@ int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
   const uint64_t windows = dcsim_jens_windows(h->spec.end_time, bin);
   const double need = ((double)windows + 1.0) * (double)jens_row_bytes(h) + (double)jens_hist_bytes(h);
   const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
-  if (windows >= 0xffffffffull || need >= 9.0e18)
-    return set_err(h, DCSIM_E_NOMEM, "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)", "", need_ll);
-  if (!h->d_jens_status) CUDA_TRY(h, cudaMalloc(&h->d_jens_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  const char* nomem = "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)";
+  if (windows >= 0xffffffffull || need >= 9.0e18) return set_err(h, DCSIM_E_NOMEM, nomem, "", need_ll);
+  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
   if (!h->d_jens_hist_out) CUDA_TRY(h, cudaMalloc(&h->d_jens_hist_out, (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
   const size_t rows_bytes = (windows + 1) * jens_row_bytes(h);
-  cudaError_t e = cudaMalloc(&h->d_jens, rows_bytes);
-  if (e == cudaSuccess) e = cudaMalloc(&h->d_jens_hist, jens_hist_bytes(h));
-  if (e != cudaSuccess) {
-    cudaFree(h->d_jens); cudaFree(h->d_jens_hist);
-    h->d_jens = NULL; h->d_jens_hist = NULL;
-    if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
-    cudaGetLastError();
-    return set_err(h, DCSIM_E_NOMEM, "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)", "", need_ll);
-  }
+  const int rc = recorder_alloc(h, (void**)&h->d_jens, rows_bytes, (void**)&h->d_jens_hist, jens_hist_bytes(h), nomem, need_ll);
+  if (rc != DCSIM_OK) return rc;
   h->jens_bin = bin; h->jens_windows = windows;
   CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, rows_bytes, h->g->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
@@ -1248,27 +1280,13 @@ int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out) {
   return DCSIM_OK;
 }
 
-/* Every replica's status word into d_jens_status (on the stream: the reductions that read it follow it there). */
-static int jens_status(dcsim_t* h) {
-  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "job ensemble not enabled (dcsim_enable_job_ensemble)%s%lld");
-  if (!h->launches) return set_err(h, DCSIM_E_STATE, "job ensemble read before the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_status + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
-  int blocks = (int)((h->n_replicas + 255) / 256);
-  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_jens_status);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
-}
-
 int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes) {
   if (!h) return DCSIM_E_INVALID;
-  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "job ensemble not enabled (dcsim_enable_job_ensemble)%s%lld");
-  if (!h->launches) return set_err(h, DCSIM_E_STATE, "job ensemble read before the first advance%s%lld");
+  const int rc = recorder_ready(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
+  if (rc != DCSIM_OK) return rc;
   const size_t need_rows = (h->jens_windows + 1) * jens_row_bytes(h), need_hist = jens_hist_bytes(h);
   if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
     return set_err(h, DCSIM_E_INVALID, "fetch_job_ensemble: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
-  CUDA_TRY(h, cudaSetDevice(h->device));
   if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jens, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
   if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jens_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
@@ -1277,28 +1295,22 @@ int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32
 
 int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out) {
   if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = jens_status(h);
+  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
   if (rc != DCSIM_OK) return rc;
   const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
-  const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  const dcsim_ens_job_src src{h->d_jens, h->d_status, h->n_replicas, cells};
+  return ens_moments(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells, dev_out);
 }
 
 int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                               double* dev_m2_out, uint64_t* dev_hist_out) {
   if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = jens_status(h);
+  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
   if (rc != DCSIM_OK) return rc;
   const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const uint64_t n_cols = (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells;
-  const dcsim_ens_job_src src{h->d_jens, h->d_jens_status, h->n_replicas, cells};
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
-                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  const dcsim_ens_job_src src{h->d_jens, h->d_status, h->n_replicas, cells};
+  return ens_spread(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells, dev_mean, dev_lo, dev_hi,
+                    dev_m2_out, dev_hist_out);
 }
 
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
@@ -1306,16 +1318,9 @@ int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes
   const uint32_t row_len = 2u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
   const size_t need = (size_t)row_len * sizeof(uint64_t);
   if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_latency_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
-  const int rc = jens_status(h);
+  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
   if (rc != DCSIM_OK) return rc;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist_out, 0, need, h->g->stream));
-  int blocks = 8 * h->sm_count;
-  if ((uint64_t)blocks > h->n_replicas) blocks = (int)h->n_replicas;
-  dcsim_hist_reduce_kernel<<<blocks, 2 * DCSIM_LAT_BINS, 0, h->g->stream>>>(h->d_jens_hist, h->n_replicas, row_len, h->d_jens_status,
-                                                                         h->d_jens_hist_out);
-  CUDA_TRY(h, cudaGetLastError());
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_jens_hist_out, need, cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  CUDA_TRY(h, hist_reduce(h, h->d_jens_hist, row_len, h->d_status, h->d_jens_hist_out, out));
   return DCSIM_OK;
 }
 
@@ -1325,19 +1330,12 @@ int dcsim_enable_power_profile(dcsim_t* h, double threshold_w) {
   if (h->member) return set_err(h, DCSIM_E_STATE, "enable_power_profile on a member of a shared group%s%lld");
   if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_power_profile must precede the first advance%s%lld");
   CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
   if (!h->d_pp) {
-    const size_t need = pp_bytes(h) + pp_work_bytes(h);
-    cudaError_t e = cudaMalloc(&h->d_pp, pp_bytes(h));
-    if (e == cudaSuccess) e = cudaMalloc(&h->d_pp_work, pp_work_bytes(h));
-    if (e == cudaSuccess && !h->d_pp_status) e = cudaMalloc(&h->d_pp_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t));
-    if (e != cudaSuccess) {
-      cudaFree(h->d_pp); cudaFree(h->d_pp_work);
-      h->d_pp = NULL; h->d_pp_work = NULL;
-      if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
-      cudaGetLastError();
-      return set_err(h, DCSIM_E_NOMEM, "enable_power_profile: %s%lld bytes of device memory do not fit (run fewer replicas)", "",
-                     (long long)need);
-    }
+    const int rc = recorder_alloc(h, (void**)&h->d_pp, pp_bytes(h), (void**)&h->d_pp_work, pp_work_bytes(h),
+                                  "enable_power_profile: %s%lld bytes of device memory do not fit (run fewer replicas)",
+                                  (long long)(pp_bytes(h) + pp_work_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
   }
   h->pp_threshold = threshold_w;
   CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
@@ -1353,51 +1351,31 @@ int dcsim_power_profile_range(dcsim_t* h, double* hi_out) {
 
 int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes) {
   if (!h || !out) return DCSIM_E_INVALID;
-  if (!h->d_pp) return set_err(h, DCSIM_E_STATE, "power profile not enabled (dcsim_enable_power_profile)%s%lld");
-  if (!h->launches) return set_err(h, DCSIM_E_STATE, "power profile read before the first advance%s%lld");
+  const int rc = recorder_ready(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
+  if (rc != DCSIM_OK) return rc;
   if (out_bytes < pp_bytes(h))
     return set_err(h, DCSIM_E_INVALID, "fetch_power_profile: buffer too small (need %s%lld bytes)", "", (long long)pp_bytes(h));
-  CUDA_TRY(h, cudaSetDevice(h->device));
   CUDA_TRY(h, cudaMemcpyAsync(out, h->d_pp, pp_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
-/* Every replica's status word into d_pp_status (on the stream, ahead of the reduction that reads it). */
-static int pp_status(dcsim_t* h) {
-  if (!h->d_pp) return set_err(h, DCSIM_E_STATE, "power profile not enabled (dcsim_enable_power_profile)%s%lld");
-  if (!h->launches) return set_err(h, DCSIM_E_STATE, "power profile read before the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_pp_status + h->n_replicas, 0, sizeof(uint32_t), h->g->stream));
-  int blocks = (int)((h->n_replicas + 255) / 256);
-  if (blocks > 4 * h->sm_count) blocks = 4 * h->sm_count;
-  dcsim_ens_counts_kernel<<<blocks, 256, 0, h->g->stream>>>(h->d_summary, h->n_replicas, DCSIM_S_STATUS, h->d_pp_status);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
-}
-
 int dcsim_power_profile_moments(dcsim_t* h, double* dev_out) {
   if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = pp_status(h);
+  const int rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
   if (rc != DCSIM_OK) return rc;
-  const uint64_t n_cols = pp_cols(h);
-  const dcsim_ens_pp_src src{h->d_pp, h->d_pp_status, h->n_replicas};
-  dcsim_ens_moments_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  const dcsim_ens_pp_src src{h->d_pp, h->d_status, h->n_replicas};
+  return ens_moments(h, src, h->n_replicas, pp_cols(h), dev_out);
 }
 
 int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                                double* dev_m2_out, uint64_t* dev_hist_out) {
   if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = pp_status(h);
+  const int rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
   if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_pp_src src{h->d_pp, h->d_status, h->n_replicas};
   const uint64_t n_cols = (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc); /* the bins need no spread */
-  const dcsim_ens_pp_src src{h->d_pp, h->d_pp_status, h->n_replicas};
-  dcsim_ens_spread_kernel<<<ens_grid(h, n_cols), DCSIM_ENS_THREADS, 0, h->g->stream>>>(src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi,
-                                                                                    dev_m2_out, (unsigned long long*)dev_hist_out);
-  CUDA_TRY(h, cudaGetLastError());
-  return DCSIM_OK;
+  return ens_spread(h, src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
 int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {
@@ -1468,8 +1446,8 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_hist); cudaFree(h->d_agg); cudaFree(h->d_hist_out);
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
-  cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_status); cudaFree(h->d_jens_hist_out);
-  cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_pp_status);
+  cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
+  cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }

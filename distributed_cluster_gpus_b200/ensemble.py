@@ -9,9 +9,11 @@ The device records, for every replica, the values its cluster_log.csv rows would
   spread   sum (x - mean)^2, histogram   -> all-reduce (SUM), given the GLOBAL mean, min and max
 
 Only n, min, max and the histograms cross GPUs exactly: they, and the quantiles read off the histograms, do not depend
-on the number of GPUs.  Mean and std do only up to summation order.  ``moments_rows`` / ``spread_rows`` are the numpy
+on the number of GPUs.  Mean and std do only up to summation order.  ``moments_cols`` / ``spread_cols`` are the numpy
 mirror of the two kernels (csrc dcsim_ens_moments_kernel / dcsim_ens_spread_kernel), as ``sharding.aggregate_rows``
-mirrors dcsim_reduce_kernel.
+mirrors dcsim_reduce_kernel; they run over a statistic's column view (x, ok) [columns, replicas], the values and which
+of them count.  Every statistic runs its passes through ``device_passes`` or ``host_passes`` and turns the all-reduced
+sums into per-column statistics with ``column_stats``.
 
 The job-log ensemble (``BatchedEngine.enable_job_ensemble``, ``job_ensemble``) runs the same two passes over columns
 (row, field, DC, job type): rows are finish windows of ``bin_s`` seconds plus the whole run, fields ``JOB_FIELDS``.
@@ -58,21 +60,9 @@ def fields_from_cluster_log(cluster, total_gpus: Sequence[int]) -> np.ndarray:
 
 
 # ---- host mirror of the two reduction kernels ------------------------------------------------------------------------
-def _valid(n_ticks: int, nlog: np.ndarray) -> np.ndarray:
-    """[ticks, replicas]: replica r recorded tick k."""
-    return np.arange(n_ticks)[:, None] < np.asarray(nlog)[None, :]
-
-
-def moments_rows(rows: np.ndarray, nlog: np.ndarray) -> np.ndarray:
-    """rows [ticks, FIELDS, n_dc, R], nlog [R] (ticks each replica recorded) -> [4, ticks * FIELDS * n_dc]
-    {n, sum, min, max}; an empty column is 0, 0, +inf, -inf."""
-    T, F, D, R = rows.shape
-    ok = np.broadcast_to(_valid(T, nlog)[:, None, None, :], rows.shape)
-    return moments_cols(rows.reshape(-1, R), ok.reshape(-1, R))
-
-
 def moments_cols(x: np.ndarray, m: np.ndarray) -> np.ndarray:
-    """x [columns, R] values, m [columns, R] which of them count -> [4, columns] {n, sum, min, max}."""
+    """x [columns, R] values, m [columns, R] which of them count -> [4, columns] {n, sum, min, max}; an empty column is
+    0, 0, +inf, -inf."""
     out = np.empty((4, x.shape[0]))
     out[0] = m.sum(axis=1)
     out[1] = np.where(m, x, 0.0).sum(axis=1)
@@ -81,15 +71,9 @@ def moments_cols(x: np.ndarray, m: np.ndarray) -> np.ndarray:
     return out
 
 
-def bin_widths(lo: np.ndarray, hi: np.ndarray, n_dc: int) -> np.ndarray:
-    """Per column of the cluster-log ensemble: the histogram's bin width (0: every value in bin 0)."""
-    field = (np.arange(np.asarray(lo).size) // n_dc) % len(FIELDS)
-    return bin_widths_for(lo, hi, np.isin(field, INTEGER_FIELDS))
-
-
 def bin_widths_for(lo: np.ndarray, hi: np.ndarray, integral: np.ndarray) -> np.ndarray:
-    """Per column: the histogram's bin width given which columns are integer fields — the kernel's rule, the kernel's
-    float ops."""
+    """Per column: the histogram's bin width (0: every value in bin 0) given which columns are integer fields — the
+    kernel's rule, the kernel's float ops."""
     lo, hi = np.asarray(lo, dtype=np.float64), np.asarray(hi, dtype=np.float64)
     with np.errstate(invalid="ignore", over="ignore"):
         span = hi - lo + 1.0
@@ -106,16 +90,9 @@ def bin_index(x: np.ndarray, lo, width) -> np.ndarray:
     return np.where(width > 0, b, 0)
 
 
-def spread_rows(rows: np.ndarray, nlog: np.ndarray, mean: np.ndarray, lo: np.ndarray, hi: np.ndarray):
-    """-> (m2 [columns] = sum (x - mean)^2, hist [columns, BINS] uint64) over the replicas that recorded each tick."""
-    T, F, D, R = rows.shape
-    ok = np.broadcast_to(_valid(T, nlog)[:, None, None, :], rows.shape).reshape(-1, R)
-    x = rows.reshape(-1, R)
-    return spread_cols(x, ok, mean, lo, hi, bin_widths(lo, hi, D))
-
-
 def spread_cols(x: np.ndarray, ok: np.ndarray, mean, lo, hi, width):
-    """x [columns, R], ok [columns, R], per-column mean / lo / width -> (m2 [columns], hist [columns, BINS] uint64)."""
+    """x [columns, R], ok [columns, R], per-column mean / lo / width -> (m2 [columns] = sum (x - mean)^2 over the values
+    that count, hist [columns, BINS] uint64)."""
     mean = np.asarray(mean, dtype=np.float64)
     with np.errstate(invalid="ignore"):
         m2 = np.where(ok, (x - mean[:, None]) ** 2, 0.0).sum(axis=1)
@@ -150,6 +127,40 @@ def hist_quantiles(hist: np.ndarray, n: np.ndarray, lo: np.ndarray, hi: np.ndarr
 
 
 @dataclass
+class ColumnStats:
+    """Per-column statistics of the all-reduced passes; arrays are [columns], quantiles [Q, columns]."""
+    n: np.ndarray
+    mean: np.ndarray
+    var: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    std: np.ndarray
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray
+
+    def result_fields(self, shape) -> dict:
+        """n, mean, std, min, max, q and quantiles with the columns laid out as ``shape``: the fields the result
+        classes share."""
+        return dict(n=self.n.reshape(shape), mean=self.mean.reshape(shape), std=self.std.reshape(shape),
+                    min=self.min.reshape(shape), max=self.max.reshape(shape), q=self.q,
+                    quantiles=self.quantiles.reshape(self.quantiles.shape[:1] + tuple(shape)))
+
+
+def column_stats(mom: np.ndarray, m2: np.ndarray, hist: np.ndarray, integral: np.ndarray,
+                 quantiles: Sequence[float]) -> ColumnStats:
+    """All-reduced moments [4, columns], m2 [columns] and histograms [columns, BINS], and which columns are integer
+    fields -> statistics; an empty column has NaN mean, std, min, max and quantiles."""
+    n, s, lo, hi = (np.asarray(a, dtype=np.float64) for a in mom)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        mean = np.where(n > 0, s / n, np.nan)
+        var = np.where(n > 1, np.asarray(m2, dtype=np.float64) / (n - 1), np.where(n == 1, 0.0, np.nan))
+    empty = n == 0
+    qv = hist_quantiles(np.asarray(hist), n, lo, hi, bin_widths_for(lo, hi, integral), integral, quantiles)
+    return ColumnStats(n=n.astype(np.int64), mean=mean, var=var, std=np.sqrt(var), min=np.where(empty, np.nan, lo),
+                       max=np.where(empty, np.nan, hi), q=tuple(float(q) for q in quantiles), quantiles=qv)
+
+
+@dataclass
 class EnsembleResult:
     """Per (tick, field, dc) statistics over every replica of the batch; arrays are [ticks, len(fields), n_dc]."""
     time_s: np.ndarray
@@ -181,30 +192,29 @@ class EnsembleResult:
                                    + [repr(float(self.max[k, i, d]))])
 
 
+def _cluster_columns(rows: np.ndarray, nlog: np.ndarray):
+    """rows [ticks, FIELDS, n_dc, R], nlog [R] (ticks each replica recorded) -> (x, ok) [columns, R], columns
+    (tick, field, dc) as the kernels'; replica r counts in the ticks it recorded."""
+    R = rows.shape[-1]
+    ok = np.arange(rows.shape[0])[:, None, None, None] < np.asarray(nlog)[None, None, None, :]
+    return rows.reshape(-1, R), np.broadcast_to(ok, rows.shape).reshape(-1, R)
+
+
+def _cluster_integral(n_cols: int, n_dc: int) -> np.ndarray:
+    return np.isin((np.arange(n_cols) // n_dc) % len(FIELDS), INTEGER_FIELDS)
+
+
 def finalize(mom: np.ndarray, m2: np.ndarray, hist: np.ndarray, n_dc: int, log_interval: float,
              quantiles: Sequence[float] = DEFAULT_QUANTILES) -> EnsembleResult:
     """All-reduced moments [4, columns], m2 [columns] and histograms [columns, BINS] -> statistics.  Trailing ticks no
     replica recorded are dropped."""
     F = len(FIELDS)
-    n_all, s, lo, hi = (np.asarray(a, dtype=np.float64) for a in mom)
-    cols_per_tick = F * n_dc
-    per_tick = n_all.reshape(-1, cols_per_tick).max(axis=1)
+    mom = np.asarray(mom, dtype=np.float64)
+    per_tick = mom[0].reshape(-1, F * n_dc).max(axis=1)
     T = int(np.nonzero(per_tick > 0)[0].max()) + 1 if np.any(per_tick > 0) else 0
-    c = T * cols_per_tick
-    n_all, s, lo, hi, m2 = n_all[:c], s[:c], lo[:c], hi[:c], np.asarray(m2, dtype=np.float64)[:c]
-    hist = np.asarray(hist)[:c]
-    with np.errstate(invalid="ignore", divide="ignore"):
-        mean = np.where(n_all > 0, s / n_all, np.nan)
-        std = np.where(n_all > 1, np.sqrt(m2 / (n_all - 1)), np.where(n_all == 1, 0.0, np.nan))
-    empty = n_all == 0
-    width = bin_widths(lo, hi, n_dc)
-    integral = np.isin((np.arange(c) // n_dc) % F, INTEGER_FIELDS)
-    qv = hist_quantiles(hist, n_all, lo, hi, width, integral, quantiles)
-    shape = (T, F, n_dc)
-    return EnsembleResult(time_s=tick_times(log_interval, T), fields=FIELDS, n=n_all.astype(np.int64).reshape(shape),
-                          mean=mean.reshape(shape), std=std.reshape(shape),
-                          min=np.where(empty, np.nan, lo).reshape(shape), max=np.where(empty, np.nan, hi).reshape(shape),
-                          q=tuple(float(q) for q in quantiles), quantiles=qv.reshape((len(quantiles),) + shape))
+    c = T * F * n_dc
+    st = column_stats(mom[:, :c], np.asarray(m2)[:c], np.asarray(hist)[:c], _cluster_integral(c, n_dc), quantiles)
+    return EnsembleResult(time_s=tick_times(log_interval, T), fields=FIELDS, **st.result_fields((T, F, n_dc)))
 
 
 # ---- the two passes with the all-reduces in between ------------------------------------------------------------------
@@ -221,16 +231,15 @@ def _allreduce(t, op):
     return t
 
 
-def reduce_passes(moments_fn, spread_fn, n_dc: int, log_interval: float,
-                  quantiles: Sequence[float] = DEFAULT_QUANTILES) -> EnsembleResult:
-    """moments_fn() -> torch [4, columns] float64; spread_fn(mean, lo, hi) -> (m2 [columns] float64, hist [columns, BINS]
-    int64), torch tensors on one device.  Runs pass 1, all-reduces it, pass 2 on the global mean / min / max, all-reduces
-    that, and finalizes on the host."""
-    return finalize(*two_passes(moments_fn, spread_fn), n_dc, log_interval, quantiles)
+def _allreduce_sum(t) -> np.ndarray:
+    import torch.distributed as dist
+    return _allreduce(t, dist.ReduceOp.SUM).cpu().numpy()
 
 
 def two_passes(moments_fn, spread_fn):
-    """The two passes with the all-reduces in between (see reduce_passes) -> host (moments, m2, hist)."""
+    """moments_fn() -> torch [4, columns] float64; spread_fn(mean, lo, hi) -> (m2 [columns] float64, hist [columns, BINS]
+    int64), torch tensors on one device.  Runs pass 1, all-reduces it, pass 2 on the global mean / min / max, all-reduces
+    that -> host (moments, m2, hist)."""
     import torch
     import torch.distributed as dist
     mom = moments_fn()
@@ -246,6 +255,48 @@ def two_passes(moments_fn, spread_fn):
     return mom.cpu().numpy(), m2.cpu().numpy(), hist.cpu().numpy()
 
 
+def device_passes(dev, cols: int, moments_into, spread_into, stat_cols: int = None):
+    """two_passes over a device recorder of ``cols`` columns: ``moments_into(out_ptr)`` and ``spread_into(mean_ptr,
+    lo_ptr, hi_ptr, m2_ptr, hist_ptr)`` (a BatchedEngine's ``*_into`` methods), the spread over the first ``stat_cols``
+    columns (None: all of them)."""
+    import torch
+    stat_cols = cols if stat_cols is None else stat_cols
+
+    def moments():
+        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
+        if cols:
+            torch.cuda.synchronize(dev)                # the library runs on the handle's stream, torch on its own
+            moments_into(out.data_ptr())
+            torch.cuda.synchronize(dev)
+        return out
+
+    def spread(mean, lo, hi):
+        m2 = torch.zeros(stat_cols, dtype=torch.float64, device=dev)
+        hist = torch.zeros((stat_cols, BINS), dtype=torch.int64, device=dev)
+        if cols:
+            torch.cuda.synchronize(dev)
+            spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
+            torch.cuda.synchronize(dev)
+        return m2, hist
+
+    return two_passes(moments, spread)
+
+
+def host_passes(x: np.ndarray, ok: np.ndarray, integral: np.ndarray, stat_cols: int = None):
+    """two_passes through the numpy mirror of the kernels over the columns x [columns, R] (ok [columns, R]: the values
+    that count), the spread over the first ``stat_cols`` columns (None: all of them), ``integral`` [stat_cols] the
+    integer fields among them."""
+    import torch
+    c = slice(stat_cols)
+
+    def spread(mean, lo, hi):
+        lo, hi = lo.numpy()[c], hi.numpy()[c]
+        m2, hist = spread_cols(x[c], ok[c], mean.numpy()[c], lo, hi, bin_widths_for(lo, hi, integral))
+        return torch.from_numpy(m2.astype(np.float64)), torch.from_numpy(hist.astype(np.int64))
+
+    return two_passes(lambda: torch.from_numpy(moments_cols(x, ok)), spread)
+
+
 def cluster_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> EnsembleResult:
     """Statistics of the cluster-log ensemble of ``engine`` (a finished BatchedEngine with enable_cluster_ensemble()),
     over all ranks when torch.distributed runs with world > 1 (every rank calls this).  Raises RecorderOverflow if a
@@ -253,38 +304,17 @@ def cluster_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> 
     import torch
     dev = torch.device("cuda", engine.device)
     cols = engine.cluster_ensemble_capacity * len(FIELDS) * engine.spec.n_dc
-
-    def moments():
-        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
-        if cols:
-            torch.cuda.synchronize(dev)                # the library runs on the handle's stream, torch on its own
-            engine.ensemble_moments_into(out.data_ptr())
-            torch.cuda.synchronize(dev)
-        return out
-
-    def spread(mean, lo, hi):
-        m2 = torch.zeros(cols, dtype=torch.float64, device=dev)
-        hist = torch.zeros((cols, BINS), dtype=torch.int64, device=dev)
-        if cols:
-            torch.cuda.synchronize(dev)
-            engine.ensemble_spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
-            torch.cuda.synchronize(dev)
-        return m2, hist
-
-    return reduce_passes(moments, spread, engine.spec.n_dc, engine.spec.log_interval, quantiles)
+    passes = device_passes(dev, cols, engine.ensemble_moments_into, engine.ensemble_spread_into)
+    return finalize(*passes, engine.spec.n_dc, engine.spec.log_interval, quantiles)
 
 
 def cluster_ensemble_from_rows(rows: np.ndarray, nlog: np.ndarray, log_interval: float,
                                quantiles: Sequence[float] = DEFAULT_QUANTILES) -> EnsembleResult:
     """The same statistics from host rows [ticks, FIELDS, n_dc, R] through the numpy mirror (all-reduced over the ranks
     like cluster_ensemble)."""
-    import torch
     n_dc = rows.shape[2]
-    return reduce_passes(lambda: torch.from_numpy(moments_rows(rows, nlog)),
-                         lambda mean, lo, hi: tuple(torch.from_numpy(np.ascontiguousarray(a).astype(dt)) for a, dt in
-                                                    zip(spread_rows(rows, nlog, mean.numpy(), lo.numpy(), hi.numpy()),
-                                                        (np.float64, np.int64))),
-                         n_dc, log_interval, quantiles)
+    x, ok = _cluster_columns(rows, nlog)
+    return finalize(*host_passes(x, ok, _cluster_integral(x.shape[0], n_dc)), n_dc, log_interval, quantiles)
 
 
 # ---- job-log ensemble ------------------------------------------------------------------------------------------------
@@ -400,37 +430,18 @@ def job_finalize(mom, m2, hist, lat_hist, n_dc: int, bin_s: float, end_time: flo
                  quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobEnsembleResult:
     """All-reduced moments [4, columns], m2, histograms [columns, BINS] and per-DC latency histograms -> statistics."""
     F, J = len(JOB_FIELDS), 2
-    n_all, s, lo, hi = (np.asarray(a, dtype=np.float64) for a in mom)
-    m2 = np.asarray(m2, dtype=np.float64)
-    c = n_all.size
-    rows = c // (F * n_dc * J)
-    with np.errstate(invalid="ignore", divide="ignore"):
-        mean = np.where(n_all > 0, s / n_all, np.nan)
-        std = np.where(n_all > 1, np.sqrt(m2 / (n_all - 1)), np.where(n_all == 1, 0.0, np.nan))
-    empty = n_all == 0
-    integral = _job_integral(c, n_dc)
-    qv = hist_quantiles(np.asarray(hist), n_all, lo, hi, bin_widths_for(lo, hi, integral), integral, quantiles)
+    mom = np.asarray(mom, dtype=np.float64)
+    rows = mom.shape[1] // (F * n_dc * J)
     shape = (rows, F, n_dc, J)
-    s4 = s.reshape(shape)
+    st = column_stats(mom, m2, hist, _job_integral(mom.shape[1], n_dc), quantiles)
+    s4 = mom[1].reshape(shape)
     with np.errstate(invalid="ignore", divide="ignore"):
         pooled = np.where(s4[:, 0] > 0, s4[:, 1] / s4[:, 0], np.nan)
-    W = rows - 1
-    k = np.arange(W, dtype=np.float64)
+    k = np.arange(rows - 1, dtype=np.float64)
     return JobEnsembleResult(t0_s=np.append(k * bin_s, 0.0), t1_s=np.append((k + 1.0) * bin_s, float(end_time)),
-                             bin_s=float(bin_s), end_time=float(end_time), fields=JOB_FIELDS,
-                             n=n_all.astype(np.int64).reshape(shape), mean=mean.reshape(shape), std=std.reshape(shape),
-                             min=np.where(empty, np.nan, lo).reshape(shape), max=np.where(empty, np.nan, hi).reshape(shape),
-                             q=tuple(float(q) for q in quantiles), quantiles=qv.reshape((len(quantiles),) + shape),
+                             bin_s=float(bin_s), end_time=float(end_time), fields=JOB_FIELDS, **st.result_fields(shape),
                              pooled_mean_latency_s=pooled,
                              latency_histogram=np.asarray(lat_hist).astype(np.uint64).reshape(n_dc, J, LAT_BINS))
-
-
-def _job_passes(moments_fn, spread_fn, lat_hist, n_dc, bin_s, end_time, quantiles):
-    """The two passes, then the per-DC latency histograms (torch int64, on the device of the passes) all-reduced."""
-    import torch.distributed as dist
-    mom, m2, hist = two_passes(moments_fn, spread_fn)
-    lh = _allreduce(lat_hist, dist.ReduceOp.SUM).cpu().numpy()
-    return job_finalize(mom, m2, hist, lh, n_dc, bin_s, end_time, quantiles)
 
 
 def job_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobEnsembleResult:
@@ -440,25 +451,9 @@ def job_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobE
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
     cols = (engine.job_ensemble_windows + 1) * len(JOB_FIELDS) * n_dc * 2
-
-    def moments():
-        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
-        torch.cuda.synchronize(dev)                    # the library runs on the handle's stream, torch on its own
-        engine.job_ensemble_moments_into(out.data_ptr())
-        torch.cuda.synchronize(dev)
-        return out
-
-    def spread(mean, lo, hi):
-        m2 = torch.zeros(cols, dtype=torch.float64, device=dev)
-        hist = torch.zeros((cols, BINS), dtype=torch.int64, device=dev)
-        torch.cuda.synchronize(dev)
-        engine.job_ensemble_spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
-        torch.cuda.synchronize(dev)
-        return m2, hist
-
-    lat_hist = torch.from_numpy(engine.dc_latency_histogram().astype(np.int64)).to(dev)
-    return _job_passes(moments, spread, lat_hist, n_dc, engine.job_ensemble_bin,
-                       engine.spec.end_time, quantiles)
+    passes = device_passes(dev, cols, engine.job_ensemble_moments_into, engine.job_ensemble_spread_into)
+    lat_hist = _allreduce_sum(torch.from_numpy(engine.dc_latency_histogram().astype(np.int64)).to(dev))
+    return job_finalize(*passes, lat_hist, n_dc, engine.job_ensemble_bin, engine.spec.end_time, quantiles)
 
 
 def job_ensemble_from_rows(rows: np.ndarray, hist: np.ndarray, status: np.ndarray, bin_s: float, end_time: float,
@@ -469,15 +464,10 @@ def job_ensemble_from_rows(rows: np.ndarray, hist: np.ndarray, status: np.ndarra
     import torch
     n_dc = rows.shape[2]
     x, ok = _job_columns(rows, status)
-    width_of = lambda lo, hi: bin_widths_for(lo, hi, _job_integral(x.shape[0], n_dc))  # noqa: E731
+    passes = host_passes(x, ok, _job_integral(x.shape[0], n_dc))
     good = np.asarray(status) == 0
-    lat_hist = torch.from_numpy(np.asarray(hist)[..., good].astype(np.int64).sum(axis=-1))
-    return _job_passes(lambda: torch.from_numpy(moments_cols(x, ok)),
-                       lambda mean, lo, hi: tuple(torch.from_numpy(np.ascontiguousarray(a).astype(dt)) for a, dt in
-                                                  zip(spread_cols(x, ok, mean.numpy(), lo.numpy(), hi.numpy(),
-                                                                  width_of(lo.numpy(), hi.numpy())),
-                                                      (np.float64, np.int64))),
-                       lat_hist, n_dc, bin_s, end_time, quantiles)
+    lat_hist = _allreduce_sum(torch.from_numpy(np.asarray(hist)[..., good].astype(np.int64).sum(axis=-1)))
+    return job_finalize(*passes, lat_hist, n_dc, bin_s, end_time, quantiles)
 
 
 # ---- power profile ---------------------------------------------------------------------------------------------------
@@ -590,36 +580,21 @@ def pp_finalize(mom, m2, hist, n_dc: int, hi: float, threshold: float, energy: f
                 quantiles: Sequence[float] = PP_CSV_QUANTILES) -> PowerProfileResult:
     """All-reduced moments [4, PP_FIELDS + n_dc + PP_BINS], m2 and histograms over the first PP_FIELDS + n_dc columns,
     and the pooled energy -> statistics."""
-    n_all, s, lo, mx = (np.asarray(a, dtype=np.float64) for a in mom)
+    mom = np.asarray(mom, dtype=np.float64)
     c = len(PP_FIELDS) + n_dc
-    n, s_c, lo_c, mx_c, m2 = n_all[:c], s[:c], lo[:c], mx[:c], np.asarray(m2, dtype=np.float64)[:c]
-    with np.errstate(invalid="ignore", divide="ignore"):
-        mean = np.where(n > 0, s_c / n, np.nan)
-        std = np.where(n > 1, np.sqrt(m2 / (n - 1)), np.where(n == 1, 0.0, np.nan))
-    empty = n == 0
-    integral = _pp_integral(c)
-    qv = hist_quantiles(np.asarray(hist)[:c], n, lo_c, mx_c, bin_widths_for(lo_c, mx_c, integral), integral, quantiles)
+    st = column_stats(mom[:, :c], np.asarray(m2)[:c], np.asarray(hist)[:c], _pp_integral(c), quantiles)
     columns = tuple((f, -1) for f in PP_FIELDS) + tuple(("dc_peak_w", d) for d in range(n_dc))
-    return PowerProfileResult(columns=columns, n=n.astype(np.int64), mean=mean, std=std,
-                              min=np.where(empty, np.nan, lo_c), max=np.where(empty, np.nan, mx_c),
-                              q=tuple(float(q) for q in quantiles), quantiles=qv, hi=float(hi), threshold=float(threshold),
-                              duration_curve=(pp_bin_edges(hi), s[c:c + PP_BINS].copy()), pooled_energy_j=float(energy))
+    return PowerProfileResult(columns=columns, **st.result_fields((c,)), hi=float(hi), threshold=float(threshold),
+                              duration_curve=(pp_bin_edges(hi), mom[1, c:c + PP_BINS].copy()), pooled_energy_j=float(energy))
 
 
-def _pp_passes(moments_fn, spread_fn, energy, n_dc, hi, threshold, quantiles):
-    """The two passes, then the pooled energy (a float64 torch scalar tensor) all-reduced."""
-    import torch.distributed as dist
-    mom, m2, hist = two_passes(moments_fn, spread_fn)
-    e = float(_allreduce(energy, dist.ReduceOp.SUM).cpu().numpy().reshape(-1)[0])
-    return pp_finalize(mom, m2, hist, n_dc, hi, threshold, e, quantiles)
-
-
-def _good_energy(summary: np.ndarray):
+def _pooled_energy(summary: np.ndarray, dev=None) -> float:
+    """Total energy of the replicas with status 0, summed over the ranks (the tensor all-reduced lives on ``dev``)."""
     import torch
     from . import spec as S
     s = np.asarray(summary)
     good = s[:, S.S_STATUS] == 0
-    return torch.tensor([float(s[good, S.S_TOTAL_ENERGY_J].sum())], dtype=torch.float64)
+    return float(_allreduce_sum(torch.tensor([float(s[good, S.S_TOTAL_ENERGY_J].sum())], dtype=torch.float64, device=dev))[0])
 
 
 def power_profile(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES, summary=None) -> PowerProfileResult:
@@ -631,27 +606,11 @@ def power_profile(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES, summary
         raise RuntimeError("power profile not enabled (enable_power_profile)")
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
-    cols, stat_cols = len(PP_FIELDS) + n_dc + PP_BINS, len(PP_FIELDS) + n_dc
-
-    def moments():
-        out = torch.zeros((4, cols), dtype=torch.float64, device=dev)
-        torch.cuda.synchronize(dev)                    # the library runs on the handle's stream, torch on its own
-        engine.power_profile_moments_into(out.data_ptr())
-        torch.cuda.synchronize(dev)
-        return out
-
-    def spread(mean, lo, hi):
-        m2 = torch.zeros(stat_cols, dtype=torch.float64, device=dev)
-        hist = torch.zeros((stat_cols, BINS), dtype=torch.int64, device=dev)
-        torch.cuda.synchronize(dev)
-        engine.power_profile_spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
-        torch.cuda.synchronize(dev)
-        return m2, hist
-
-    energy = _good_energy(engine.summary() if summary is None else summary).to(dev)
+    passes = device_passes(dev, len(PP_FIELDS) + n_dc + PP_BINS, engine.power_profile_moments_into,
+                           engine.power_profile_spread_into, stat_cols=len(PP_FIELDS) + n_dc)
+    energy = _pooled_energy(engine.summary() if summary is None else summary, dev)
     thr = engine.power_threshold
-    return _pp_passes(moments, spread, energy, n_dc, engine.power_profile_range(),
-                      float("inf") if thr is None else thr, quantiles)
+    return pp_finalize(*passes, n_dc, engine.power_profile_range(), float("inf") if thr is None else thr, energy, quantiles)
 
 
 def power_profile_from_rows(rows: np.ndarray, summary: np.ndarray, hi: float, threshold=None,
@@ -659,20 +618,11 @@ def power_profile_from_rows(rows: np.ndarray, summary: np.ndarray, hi: float, th
     """The same statistics from host rows [PP_FIELDS + n_dc + PP_BINS, R] (BatchedEngine.power_profile_rows) and the
     summary rows [R, SUMMARY_K] through the numpy mirror of both passes; replicas with status != 0 are left out.
     All-reduced over the ranks like power_profile."""
-    import torch
     from . import spec as S
     rows = np.asarray(rows, dtype=np.float64)
     n_dc = rows.shape[0] - len(PP_FIELDS) - PP_BINS
     stat_cols = len(PP_FIELDS) + n_dc
     good = np.asarray(summary)[:, S.S_STATUS] == 0
-    ok = np.broadcast_to(good[None, :], rows.shape)
-    integral = _pp_integral(stat_cols)
-    return _pp_passes(lambda: torch.from_numpy(moments_cols(rows, ok)),
-                      lambda mean, lo, hi_: tuple(torch.from_numpy(np.ascontiguousarray(a).astype(dt)) for a, dt in
-                                                  zip(spread_cols(rows[:stat_cols], ok[:stat_cols], mean.numpy()[:stat_cols],
-                                                                  lo.numpy()[:stat_cols],
-                                                                  hi_.numpy()[:stat_cols],
-                                                                  bin_widths_for(lo.numpy()[:stat_cols], hi_.numpy()[:stat_cols],
-                                                                                 integral)),
-                                                      (np.float64, np.int64))),
-                      _good_energy(summary), n_dc, hi, float("inf") if threshold is None else float(threshold), quantiles)
+    passes = host_passes(rows, np.broadcast_to(good[None, :], rows.shape), _pp_integral(stat_cols), stat_cols)
+    return pp_finalize(*passes, n_dc, hi, float("inf") if threshold is None else float(threshold), _pooled_energy(summary),
+                       quantiles)
