@@ -53,7 +53,8 @@ DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsig
   if (r0 - (uint64_t)(grp % DCSIM_REPLICAS_PER_WARP) >= P.n_replicas) return;
   const bool ghost = r0 >= P.n_replicas;
 #endif
-  const uint64_t r = ghost ? P.n_replicas - 1u : r0; /* (a ghost only ever READS through these pointers) */
+  const uint64_t r = ghost ? P.n_replicas - 1u : r0; /* (a ghost only ever READS replica n-1's state: in place, where blk
+                                                        is that replica's live block, see dcsim_ctx_t::quiet) */
   const int bytes = MODE == DCSIM_MODE_HEAD ? P.L.rec_off : P.L.total_bytes; /* what is staged */
   char* home = P.state + r * (uint64_t)P.L.total_bytes;
   char* blk = MODE != DCSIM_MODE_INPLACE ? dcsim_smem + (size_t)grp * (size_t)bytes : home;
@@ -65,7 +66,7 @@ DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsig
     for (int i = lane; i < bytes / 16; i += DCSIM_LANES) dst[i] = src[i];
   }
   dcsim_warp_sync();
-  const uint32_t n = dcsim_replica_step<CAP, MODE != DCSIM_MODE_STAGED, PP>(&P, r, blk, rec, fresh, ghost);
+  const uint32_t n = dcsim_replica_step<CAP, MODE != DCSIM_MODE_STAGED, PP, MODE == DCSIM_MODE_INPLACE>(&P, r, blk, rec, fresh, ghost);
   dcsim_warp_sync();
   if (MODE != DCSIM_MODE_INPLACE && !ghost) {
     const uint4* src = reinterpret_cast<const uint4*>(blk);

@@ -503,6 +503,9 @@ struct dcsim_ctx_t {
   bool is_traced, is_logged;
   bool pp;               /* the power-profile recorder runs: a compile-time false in the instantiations without it
                             (dcsim_replica_step<..., PP>), so their code does not change */
+  bool quiet;            /* a ghost lane group of an in-place launch, whose blk is replica n-1's live block in HBM: it must
+                            not even publish the pop-min cache there.  A compile-time false in the staged and head-staged
+                            instantiations (a ghost's blk is its own shared-memory slot there) */
   /* Hot scalars kept in registers and written back to the header when the launch ends.  seq: lane 0's copy is
    * authoritative (only lane 0 runs handlers); the others are warp-uniform. */
   uint32_t seq;          /* successful pushes (SIM:163) */
@@ -1317,7 +1320,7 @@ DCSIM_DEV uint32_t* dcsim_list_seq_slot(dcsim_ctx_t& c, uint32_t m) {
 struct dcsim_omin_t { uint32_t hi, lo, seq; int slot; bool fresh; }; /* (1); fresh: just reduced, not yet in the header */
 /* Lane 0, after the event's first sync (every lane has read the header's copy by then): publishes a fresh (1). */
 DCSIM_DEV void dcsim_omin_publish(dcsim_ctx_t& c, const dcsim_omin_t& o) {
-  if (o.fresh && c.lane == 0) {
+  if (o.fresh && c.lane == 0 && !c.quiet) {
     c.H->omin_t = dcsim_hilo_f64(o.hi, o.lo); c.H->omin_seq = o.seq; c.H->omin_slot = (uint32_t)o.slot; c.H->cand_dirty = 0u;
   }
 }
@@ -2517,8 +2520,9 @@ DCSIM_DEV void dcsim_write_summary(dcsim_ctx_t& c, double* out) {
  * block (shared memory on the GPU), already loaded unless `fresh`; `rec` is the base the running-job record offsets
  * apply to (== blk when the records were staged with it, the block's home in HBM when only the head was: RECG).
  * PP: the power-profile recorder is compiled in (it runs when P->pp is set); a separate instantiation, so that the
- * kernels without it keep their registers and code. */
-template <bool CAP, bool RECG, bool PP = false>
+ * kernels without it keep their registers and code.  INPLACE: `blk` is the block's home itself (nothing staged), so a
+ * ghost's blk is replica n-1's live block (see dcsim_ctx_t::quiet). */
+template <bool CAP, bool RECG, bool PP = false, bool INPLACE = false>
 DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char* blk, char* rec, bool fresh, bool ghost = false) {
   dcsim_ctx_t c;
   c.P = P; c.blk = blk; c.rec = rec; c.H = reinterpret_cast<dcsim_hdr_t*>(blk); c.lane = dcsim_lane();
@@ -2526,7 +2530,9 @@ DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char
   c.is_traced = !ghost && ((int64_t)r == P->rec.trace_replica);
   c.is_logged = !ghost && ((int64_t)r == P->rec.log_replica);
   c.pp = PP && !ghost && P->pp != nullptr;
-  if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing */
+  c.quiet = INPLACE && ghost;
+  if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing to a
+                  replica's state (staged modes: its own shared-memory slot takes the pop-min cache; in place: quiet) */
     c.seq = 0u; c.now = 0.0; c.cursor = 0u;
     return dcsim_replica_run<CAP, RECG>(c, false);
   }

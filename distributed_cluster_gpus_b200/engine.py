@@ -435,8 +435,9 @@ def _pp_key(power_profile, power_threshold):
 
 
 def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None):
+    # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            bool(cluster_ensemble), job_bin, pp)
+            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp)
 
 
 def _drop_parked_batch_engine():
