@@ -28,6 +28,8 @@ EXPORTS = (
     "dcsim_arrivals_compatible", "dcsim_create_shared", "dcsim_paired_moments", "dcsim_paired_spread",
     "dcsim_enable_power_profile", "dcsim_power_profile_range", "dcsim_fetch_power_profile", "dcsim_power_profile_moments",
     "dcsim_power_profile_spread",
+    "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_job_waits_moments", "dcsim_job_waits_spread",
+    "dcsim_fetch_dc_wait_histogram",
 )
 
 _lib = None
@@ -130,6 +132,17 @@ def load():
         L.dcsim_paired_moments.argtypes = [vp, vp, u64, vp]
         L.dcsim_paired_spread.restype = i32
         L.dcsim_paired_spread.argtypes = [vp, vp, u64, vp, vp, vp, vp, vp]
+    if hasattr(L, "dcsim_enable_job_waits"):
+        L.dcsim_enable_job_waits.restype = i32
+        L.dcsim_enable_job_waits.argtypes = [vp]
+        L.dcsim_fetch_job_waits.restype = i32
+        L.dcsim_fetch_job_waits.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
+        L.dcsim_job_waits_moments.restype = i32
+        L.dcsim_job_waits_moments.argtypes = [vp, vp]
+        L.dcsim_job_waits_spread.restype = i32
+        L.dcsim_job_waits_spread.argtypes = [vp, vp, vp, vp, vp, vp]
+        L.dcsim_fetch_dc_wait_histogram.restype = i32
+        L.dcsim_fetch_dc_wait_histogram.argtypes = [vp, vp, C.c_size_t]
     if hasattr(L, "dcsim_enable_power_profile"):
         L.dcsim_enable_power_profile.restype = i32
         L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]

@@ -202,6 +202,42 @@ struct dcsim_ens_job_src {
   __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JENS_FIELDS == DCSIM_JENS_JOBS; }
 };
 
+/* Waiting and response times: column (row, field, dc, jtype) as the job-log ensemble's, `cells` = n_dc * 2 per field.
+ * WAITED, WAIT_SUM and RESP_SUM are stored ([row][DCSIM_JWAIT_STORED][cell][replica]) and count for every valid replica;
+ * MEAN_WAIT = WAIT_SUM / JOBS and MEAN_RESPONSE = RESP_SUM / JOBS for those with a job in the cell (JOBS: the job-log
+ * ensemble's count of the same cell).  Only replicas with status 0 count. */
+struct dcsim_ens_wait_src {
+  const double* jwait;
+  const double* jens;
+  const uint32_t* status;
+  uint64_t n;
+  uint32_t cells;
+  struct view {
+    const double* x;
+    const double* jobs;
+    const uint32_t* status;
+    bool mean;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (status[r] != 0u) return false;
+      if (!mean) { v = x[r]; return true; }
+      const double k = jobs[r];
+      if (!(k > 0.0)) return false;
+      v = x[r] / k;
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const {
+    const uint64_t row = col / ((uint64_t)DCSIM_JWAIT_FIELDS * cells), cell = col % cells;
+    const int field = (int)((col / cells) % DCSIM_JWAIT_FIELDS);
+    const bool mean = field >= DCSIM_JWAIT_STORED;
+    const uint64_t stored = mean ? (uint64_t)(field - DCSIM_JWAIT_STORED + DCSIM_JWAIT_WAIT_SUM) : (uint64_t)field;
+    const double* x = jwait + ((row * DCSIM_JWAIT_STORED + stored) * cells + cell) * n;
+    const double* jobs = jens + ((row * DCSIM_JENS_STORED + DCSIM_JENS_JOBS) * cells + cell) * n;
+    return view{x, jobs, status, mean};
+  }
+  __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JWAIT_FIELDS == DCSIM_JWAIT_WAITED; }
+};
+
 /* Paired comparison: column (metric, field) over replica r's summary rows of a base and a variant batch (the same keys).
  * Counted when both rows have status 0 and the metric is defined in both; fields base, variant, variant - base,
  * variant < base, variant > base (include/dcsim_b200.h DCSIM_PAIR_*). */
@@ -449,6 +485,9 @@ struct dcsim {
   double* d_pp;            /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile (opt-in) */
   double* d_pp_work;       /* [n_replicas][DCSIM_PPW_N] its working state */
   double pp_threshold;
+  double* d_jwait;         /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waiting / response times (opt-in) */
+  uint32_t* d_jwait_hist;  /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] their per-DC histograms */
+  unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_wait_histogram */
   uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the job ensemble and power profile
                          reductions, refreshed on the stream ahead of every one of them (status_words) */
   unsigned long long events_seen;
@@ -467,6 +506,11 @@ static size_t jens_row_bytes(const dcsim_t* h) { /* one row (window) of the job-
 static size_t jens_hist_bytes(const dcsim_t* h) {
   return (size_t)h->n_replicas * (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(uint32_t);
 }
+
+static size_t jwait_row_bytes(const dcsim_t* h) {
+  return (size_t)DCSIM_JWAIT_STORED * (size_t)h->spec.n_dc * 2 * (size_t)h->n_replicas * sizeof(double);
+}
+static size_t jwait_hist_bytes(const dcsim_t* h) { return 2 * jens_hist_bytes(h); }
 
 static uint64_t pp_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc + DCSIM_PP_BINS); }
 static size_t pp_bytes(const dcsim_t* h) { return (size_t)pp_cols(h) * (size_t)h->n_replicas * sizeof(double); }
@@ -687,10 +731,11 @@ static cudaError_t size_launch(dcsim_t* h) {
   return cudaSuccess;
 }
 
-/* job_log.csv needs size / f / jid in the running records; switching it on or off re-lays the state block out. */
+/* job_log.csv needs size / f / jid in the running records, the waiting-time recorder the jid; switching them on or off
+ * re-lays the state block out. */
 static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
-  dcsim_make_layout(&h->spec, &L, job_log);
+  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL);
   if (L.lean == h->L.lean) return DCSIM_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
@@ -882,6 +927,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
   }
+  if (h->d_jwait) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, (h->jens_windows + 1) * jwait_row_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
+  }
   if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
     h->g->seed0 = base_seed + first_replica_id;
     h->g->arrivals_ready = 0;
@@ -964,6 +1013,7 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->finish_rec = (P->lat_hist || P->jens) ? 1u : 0u;
   P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
   P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
+  P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
 }
 
 /* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */
@@ -1258,6 +1308,8 @@ int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
   CUDA_TRY(h, cudaSetDevice(h->device));
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist);
   h->d_jens = NULL; h->d_jens_hist = NULL; h->jens_windows = 0; h->jens_bin = 0.0;
+  cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); /* sized by the windows: re-enabled after the job ensemble */
+  h->d_jwait = NULL; h->d_jwait_hist = NULL;
   const uint64_t windows = dcsim_jens_windows(h->spec.end_time, bin);
   const double need = ((double)windows + 1.0) * (double)jens_row_bytes(h) + (double)jens_hist_bytes(h);
   const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
@@ -1321,6 +1373,69 @@ int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes
   const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
   if (rc != DCSIM_OK) return rc;
   CUDA_TRY(h, hist_reduce(h, h->d_jens_hist, row_len, h->d_status, h->d_jens_hist_out, out));
+  return DCSIM_OK;
+}
+
+int dcsim_enable_job_waits(dcsim_t* h) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "enable_job_waits needs the job ensemble (dcsim_enable_job_ensemble first)%s%lld");
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_job_waits on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_waits must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const size_t rows_bytes = (h->jens_windows + 1) * jwait_row_bytes(h);
+  if (!h->d_jwait) {
+    if (!h->d_jwait_hist_out) CUDA_TRY(h, cudaMalloc(&h->d_jwait_hist_out, (size_t)h->spec.n_dc * 4 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
+    const int rc = recorder_alloc(h, (void**)&h->d_jwait, rows_bytes, (void**)&h->d_jwait_hist, jwait_hist_bytes(h),
+                                  "enable_job_waits: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)",
+                                  (long long)(rows_bytes + jwait_hist_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, rows_bytes, h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes) {
+  if (!h) return DCSIM_E_INVALID;
+  const int rc = recorder_ready(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
+  if (rc != DCSIM_OK) return rc;
+  const size_t need_rows = (h->jens_windows + 1) * jwait_row_bytes(h), need_hist = jwait_hist_bytes(h);
+  if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
+    return set_err(h, DCSIM_E_INVALID, "fetch_job_waits: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
+  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jwait, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
+  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jwait_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_job_waits_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
+  const dcsim_ens_wait_src src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells};
+  return ens_moments(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JWAIT_FIELDS * cells, dev_out);
+}
+
+int dcsim_job_waits_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                           double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
+  const dcsim_ens_wait_src src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells};
+  return ens_spread(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JWAIT_FIELDS * cells, dev_mean, dev_lo, dev_hi,
+                    dev_m2_out, dev_hist_out);
+}
+
+int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  const uint32_t row_len = 4u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
+  const size_t need = (size_t)row_len * sizeof(uint64_t);
+  if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_wait_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
+  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
+  if (rc != DCSIM_OK) return rc;
+  CUDA_TRY(h, hist_reduce(h, h->d_jwait_hist, row_len, h->d_status, h->d_jwait_hist_out, out));
   return DCSIM_OK;
 }
 
@@ -1448,6 +1563,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
   cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
+  cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }

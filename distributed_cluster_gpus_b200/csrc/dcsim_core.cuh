@@ -486,6 +486,8 @@ struct dcsim_kparams_t {
   double* pp_work;      /* [n_replicas][DCSIM_PPW_N] its working state (with pp) */
   double pp_threshold;  /* [W], +inf: none */
   double pp_hi;         /* upper end of the histogram range (dcsim_pp_range) */
+  double* jwait;        /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waits (needs jens and L.lean == 0), or NULL */
+  uint32_t* jwait_hist; /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] per-DC wait / response histograms (with jwait) */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -1840,6 +1842,39 @@ DCSIM_COLD void dcsim_jens_add(const dcsim_kparams_t* P, uint32_t r, int d, int 
 #endif
 }
 
+/* Waiting and response times (opt-in: P->jwait, on top of P->jens): the job of running record i (at `rec`, the base of
+ * the L.rn_* offsets) of DC d and type jt finished at `now`; its start and jid are read here, off the hot path.  Its arrival and xfer_done instants are the pre-pass's and the merge's (arr_t / arr_tx of arrival
+ * jid - 1: written once before the event loop, read-only since), bit for bit the instants the event loop ran the
+ * arrival and the xfer_done at.  Same cells, window and write discipline as dcsim_jens_add. */
+DCSIM_COLD void dcsim_jwait_add(const dcsim_kparams_t* P, uint32_t r, int d, int jt, double now, char* rec, int i) {
+  const double start = dcsim_at<double>(rec, P->L.rn_start)[i];
+  const uint32_t jid = dcsim_at<uint32_t>(rec, P->L.rn_jid)[i];
+  const uint64_t a = (uint64_t)r * (uint64_t)P->cap_arr + (uint64_t)(jid - 1u);
+  const double wait = start - P->arr_tx[a];
+  const double resp = now - P->arr_t[a];
+  const uint64_t n = P->n_replicas, W = P->jens_windows;
+  const uint64_t fs = 2ull * (uint64_t)P->spec.n_dc * n; /* field stride */
+  const double f = floor(now / P->jens_bin);
+  const uint64_t k = f >= (double)(W - 1u) ? W - 1u : (uint64_t)f;
+  double* win = P->jwait + k * (DCSIM_JWAIT_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  double* all = P->jwait + W * (DCSIM_JWAIT_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  uint32_t* cell = P->jwait_hist + ((uint64_t)r * (uint64_t)P->spec.n_dc + (uint64_t)d) * (4 * DCSIM_LAT_BINS) +
+                   (uint32_t)(jt * DCSIM_LAT_BINS);
+#ifdef DCSIM_HOST_EMU
+  if (wait > 0.0) { win[DCSIM_JWAIT_WAITED * fs] += 1.0; all[DCSIM_JWAIT_WAITED * fs] += 1.0; }
+  win[DCSIM_JWAIT_WAIT_SUM * fs] += wait; win[DCSIM_JWAIT_RESP_SUM * fs] += resp;
+  all[DCSIM_JWAIT_WAIT_SUM * fs] += wait; all[DCSIM_JWAIT_RESP_SUM * fs] += resp;
+  cell[dcsim_lat_bin(wait)] += 1u;
+  cell[2 * DCSIM_LAT_BINS + dcsim_lat_bin(resp)] += 1u;
+#else
+  if (wait > 0.0) { atomicAdd(win + DCSIM_JWAIT_WAITED * fs, 1.0); atomicAdd(all + DCSIM_JWAIT_WAITED * fs, 1.0); }
+  atomicAdd(win + DCSIM_JWAIT_WAIT_SUM * fs, wait); atomicAdd(win + DCSIM_JWAIT_RESP_SUM * fs, resp);
+  atomicAdd(all + DCSIM_JWAIT_WAIT_SUM * fs, wait); atomicAdd(all + DCSIM_JWAIT_RESP_SUM * fs, resp);
+  atomicAdd(cell + dcsim_lat_bin(wait), 1u);
+  atomicAdd(cell + 2 * DCSIM_LAT_BINS + dcsim_lat_bin(resp), 1u);
+#endif
+}
+
 /* SIM:701-927 minus RL/elastic branches (lane 0 part, after the record was read and before it is erased). */
 DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const dcsim_spec_t& sp = c.P->spec;
@@ -1862,6 +1897,7 @@ DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
 #endif
     if (c.P->lat_hist) dcsim_hist_add(c.P->lat_hist, (uint64_t)c.r, jt, lat);
     if (c.P->jens) dcsim_jens_add(c.P, c.r, d, jt, now, lat);
+    if (c.P->jwait) dcsim_jwait_add(c.P, c.r, d, jt, now, c.rec, i); /* (only with jens, in the layout keeping the jid) */
   }
   if (L.lean == 0) { /* the readers of a finished job's size / f / jid: job_log.csv and the bandit's reward */
     const double f_used = dcsim_at<double>(c.rec, L.rn_f)[i];

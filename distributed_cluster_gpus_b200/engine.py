@@ -22,6 +22,7 @@ LAT_BINS = 128
 ENS_FIELDS = 11     # DCSIM_ENS_FIELDS (names: ensemble.FIELDS)
 ENS_BINS = 1024     # DCSIM_ENS_BINS
 JENS_STORED = 2     # DCSIM_JENS_STORED: jobs, lat_sum per (window, dc, jtype) and replica
+JWAIT_STORED = 3    # DCSIM_JWAIT_STORED: waited, wait_sum, resp_sum per (window, dc, jtype) and replica
 
 
 def latency_bin_edges() -> np.ndarray:
@@ -230,6 +231,8 @@ class BatchedEngine:
         """Opt-in, before the first advance of a batch (stays on across reset): every replica sums its finished jobs and
         their latencies per finish window of ``bin_s`` seconds (None / 0: log_interval), DC and job type, plus a per-DC
         job-latency histogram."""
+        if self._jens_bin != (float(bin_s) if bin_s else float(self.spec.log_interval)):
+            self._jwait_on = False     # the library drops the waits recorder with the old windows, even when this fails
         N.check(self._lib.dcsim_enable_job_ensemble(self._h, float(bin_s or 0.0)), self._h)
         w = C.c_uint32(0)
         N.check(self._lib.dcsim_job_ensemble_windows(self._h, C.byref(w)), self._h)
@@ -270,6 +273,44 @@ class BatchedEngine:
         """[n_dc, 2, LAT_BINS] uint64: job-latency counts per DC and job type over the replicas with status 0."""
         out = np.zeros((self.spec.n_dc, 2, LAT_BINS), dtype=np.uint64)
         N.check(self._lib.dcsim_fetch_dc_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
+        return out
+
+    # -- waiting and response times (ensemble.job_waits), in the job ensemble's cells ---------------------------------
+    def enable_job_waits(self):
+        """Opt-in, after enable_job_ensemble and before the first advance of a batch (stays on across reset, zeroed by
+        it): every finished job adds its wait (start - xfer_done) and response time (finish - arrival) to its cells of the
+        job ensemble, and to per-DC wait and response histograms.  The running records then carry the job id."""
+        N.check(self._lib.dcsim_enable_job_waits(self._h), self._h)
+        self._jwait_on = True
+
+    @property
+    def job_waits_enabled(self) -> bool:
+        return getattr(self, "_jwait_on", False) and bool(self._jens_windows)
+
+    def job_waits_rows(self):
+        """(rows [W + 1, JWAIT_STORED, n_dc, 2, n_replicas] float64 {waited, wait_sum, resp_sum}, hist [n_dc, 2 kinds,
+        2, LAT_BINS, n_replicas] uint32): every replica's raw recorder.  For tests and small batches."""
+        if not self.job_waits_enabled:
+            raise RuntimeError("job waits not enabled (enable_job_waits)")
+        rows = np.empty((self._jens_windows + 1, JWAIT_STORED, self.spec.n_dc, 2, self.n_replicas), dtype=np.float64)
+        hist = np.empty((self.n_replicas, self.spec.n_dc, 2, 2, LAT_BINS), dtype=np.uint32)
+        N.check(self._lib.dcsim_fetch_job_waits(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
+                                                C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
+
+    def job_waits_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][(W + 1) * 3 * n_dc * 2] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_job_waits_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def job_waits_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_job_waits_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                 C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
+    def dc_wait_histogram(self) -> np.ndarray:
+        """[n_dc, 2 kinds (wait, response), 2, LAT_BINS] uint64 over the replicas with status 0."""
+        out = np.zeros((self.spec.n_dc, 2, 2, LAT_BINS), dtype=np.uint64)
+        N.check(self._lib.dcsim_fetch_dc_wait_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
 
     # -- power profile (ensemble.power_profile turns it into batch statistics) ----------------------------------------
@@ -434,10 +475,10 @@ def _pp_key(power_profile, power_threshold):
     return (float("inf") if power_threshold is None else float(power_threshold)) if power_profile else None
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None):
+def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False):
     # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp)
+            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None))
 
 
 def _drop_parked_batch_engine():
@@ -447,13 +488,15 @@ def _drop_parked_batch_engine():
 
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
-                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None):
+                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
     ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
-    power-profile recorder on, threshold ``power_threshold`` watts (None: none).  A parked engine is only reused by a
-    caller that asks for the same recorders."""
-    job_bin = _job_bin(sp, job_ensemble, job_ensemble_bin)
-    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold))
+    power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
+    response-time recorder on (it implies the job ensemble).  A parked engine is only reused by a caller that asks for
+    the same recorders."""
+    job_bin = _job_bin(sp, job_ensemble or job_waits, job_ensemble_bin)
+    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
+                     job_waits)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -468,6 +511,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_cluster_ensemble()
         if job_bin is not None:
             eng.enable_job_ensemble(job_bin)
+        if job_waits:
+            eng.enable_job_waits()
         if power_profile:
             eng.enable_power_profile(power_threshold)
     except BaseException:
@@ -483,7 +528,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     _drop_parked_batch_engine()
     _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
                                                         eng.job_ensemble_bin,
-                                                        _pp_key(eng.power_profile_enabled, eng.power_threshold))
+                                                        _pp_key(eng.power_profile_enabled, eng.power_threshold),
+                                                        eng.job_waits_enabled)
 
 
 def free_cached_engine():
@@ -532,19 +578,19 @@ class LoggedReplica:
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
-                      job_ensemble_bin=None, power_profile=False, power_threshold=None):
+                      job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
     kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
     ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
     window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
-    None = no threshold)."""
+    None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble)."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
-                             job_ensemble, job_ensemble_bin, power_profile, power_threshold)
+                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

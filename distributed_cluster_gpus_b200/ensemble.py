@@ -17,6 +17,8 @@ sums into per-column statistics with ``column_stats``.
 
 The job-log ensemble (``BatchedEngine.enable_job_ensemble``, ``job_ensemble``) runs the same two passes over columns
 (row, field, DC, job type): rows are finish windows of ``bin_s`` seconds plus the whole run, fields ``JOB_FIELDS``.
+Waiting and response times (``BatchedEngine.enable_job_waits``, ``job_waits``) use the same rows and cells, fields
+``WAIT_FIELDS``.
 """
 import csv
 import math
@@ -468,6 +470,171 @@ def job_ensemble_from_rows(rows: np.ndarray, hist: np.ndarray, status: np.ndarra
     good = np.asarray(status) == 0
     lat_hist = _allreduce_sum(torch.from_numpy(np.asarray(hist)[..., good].astype(np.int64).sum(axis=-1)))
     return job_finalize(*passes, lat_hist, n_dc, bin_s, end_time, quantiles)
+
+
+# ---- waiting and response times ---------------------------------------------------------------------------------------
+WAIT_FIELDS = ("waited", "wait_sum", "resp_sum", "mean_wait_s", "mean_response_s")   # DCSIM_JWAIT_* order
+WAIT_CSV_FIELDS = ("waited", "mean_wait_s", "mean_response_s")
+
+
+def _wait_columns(rows: np.ndarray, jobs: np.ndarray, status: np.ndarray):
+    """rows [W + 1, 3, n_dc, 2, R] {waited, wait_sum, resp_sum}, jobs [W + 1, n_dc, 2, R] (the job ensemble's counts) ->
+    (x, ok) [columns, R], columns (row, WAIT_FIELDS, dc, jtype) as the kernels'."""
+    R = rows.shape[-1]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        x = np.concatenate([rows, rows[:, 1:3] / jobs[:, None]], axis=1)
+    good = np.broadcast_to((np.asarray(status) == 0)[None, None, None, :], jobs.shape)
+    has = good & (jobs > 0)
+    ok = np.stack([good, good, good, has, has], axis=1)
+    return x.reshape(-1, R), ok.reshape(-1, R)
+
+
+def _wait_integral(n_cols: int, n_dc: int) -> np.ndarray:
+    return (np.arange(n_cols) // (2 * n_dc)) % len(WAIT_FIELDS) == 0
+
+
+def zero_share_quantiles(hist_row, zero_share: float, qs) -> list:
+    """latency_quantiles of one wait histogram row, except that a quantile whose share lies at or below ``zero_share``
+    (the jobs that did not wait: their bin 0 also holds waits below 2^-20 s) is exactly 0."""
+    from .engine import latency_quantiles
+    vals = latency_quantiles(hist_row, qs)
+    return [0.0 if float(q) <= zero_share and np.asarray(hist_row).sum() else v for q, v in zip(qs, vals)]
+
+
+@dataclass
+class JobWaitsResult:
+    """Per (row, field, dc, jtype) statistics over every replica of the batch; arrays are [W + 1, len(fields), n_dc, 2],
+    rows as JobEnsembleResult's.  wait = start - xfer_done (the time in the DC's FIFO), response = finish - arrival."""
+    t0_s: np.ndarray
+    t1_s: np.ndarray
+    bin_s: float
+    end_time: float
+    fields: Tuple[str, ...]
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray                              # [Q, W + 1, fields, n_dc, 2]
+    jobs: np.ndarray                                   # [n_dc, 2]: finished jobs of the valid replicas, whole run
+    waited: np.ndarray                                 # [n_dc, 2]: of them, jobs whose wait was > 0
+    wait_sum: np.ndarray                               # [n_dc, 2]: their waits' sum (pooled over replicas)
+    resp_sum: np.ndarray                               # [n_dc, 2]: their response times' sum
+    wait_histogram: np.ndarray                         # [n_dc, 2 kinds (wait, response), 2, LAT_BINS] uint64
+
+    def quantile_names(self):
+        return [f"p{int(round(q * 100)):02d}" for q in self.q]
+
+    def zero_wait_share(self, d: int, jt: int) -> float:
+        """1 - waited / jobs of DC d and type jt (whole run, pooled): the share of jobs that did not wait."""
+        return 1.0 - float(self.waited[d, jt]) / float(self.jobs[d, jt]) if self.jobs[d, jt] else float("nan")
+
+    def wait_quantiles(self, d: int, jt: int, qs=None) -> list:
+        """Quantiles [s] of the wait of DC d's jobs of type jt, pooled over the replicas (log-binned; exactly 0 at or below
+        the zero-wait share)."""
+        return zero_share_quantiles(self.wait_histogram[d, 0, jt], self.zero_wait_share(d, jt), self.q if qs is None else qs)
+
+    def response_quantiles(self, d: int, jt: int, qs=None) -> list:
+        from .engine import latency_quantiles
+        return latency_quantiles(self.wait_histogram[d, 1, jt], self.q if qs is None else qs)
+
+    def pooled(self, qs=(0.5, 0.95, 0.99)) -> dict:
+        """Per job type over all DCs: pooled mean / quantiles of wait and response, and waited_share."""
+        from .engine import latency_quantiles
+        out = {}
+        for jt, name in enumerate(JOB_TYPES):
+            jobs, waited = float(self.jobs[:, jt].sum()), float(self.waited[:, jt].sum())
+            wh, rh = self.wait_histogram[:, 0, jt].sum(axis=0), self.wait_histogram[:, 1, jt].sum(axis=0)
+            share = 1.0 - waited / jobs if jobs else float("nan")
+            e = {"jobs": int(jobs), "waited_share": waited / jobs if jobs else float("nan"),
+                 "mean_wait_s": float(self.wait_sum[:, jt].sum()) / jobs if jobs else float("nan"),
+                 "mean_response_s": float(self.resp_sum[:, jt].sum()) / jobs if jobs else float("nan")}
+            for q, v in zip(qs, zero_share_quantiles(wh, share, qs)):
+                e[f"p{int(round(q * 100)):02d}_wait_s"] = v
+            for q, v in zip(qs, latency_quantiles(rh, qs)):
+                e[f"p{int(round(q * 100)):02d}_response_s"] = v
+            out[name] = e
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """The job ensemble's long format (t0_s,t1_s,dc,type,field,n,mean,std,min,p05,...,p95,max).  Per window, then for
+        the whole run, the rows of ``waited``, ``mean_wait_s`` and ``mean_response_s`` per DC and type; then per DC and
+        type three whole-run rows: ``wait_s`` and ``response_s`` (n = jobs, mean = the pooled mean, quantiles from the
+        per-DC histograms, wait quantiles exactly 0 at or below the zero-wait share; std / min / max empty) and
+        ``waited_share`` (mean = waited / jobs)."""
+        rows, F, D, J = self.n.shape
+        keep = [self.fields.index(f) for f in WAIT_CSV_FIELDS]
+        nan = float("nan")
+        with open(path, "w", newline="") as f:
+            w = csv.writer(f)
+            w.writerow(JOB_CSV_HEADER_HEAD + self.quantile_names() + ["max"])
+            for k in range(rows):
+                for d in range(D):
+                    for jt in range(J):
+                        for i in keep:
+                            w.writerow([repr(float(self.t0_s[k])), repr(float(self.t1_s[k])), dc_names[d], JOB_TYPES[jt],
+                                        self.fields[i], int(self.n[k, i, d, jt]), repr(float(self.mean[k, i, d, jt])),
+                                        repr(float(self.std[k, i, d, jt])), repr(float(self.min[k, i, d, jt]))]
+                                       + [repr(float(self.quantiles[j, k, i, d, jt])) for j in range(len(self.q))]
+                                       + [repr(float(self.max[k, i, d, jt]))])
+            head = [repr(0.0), repr(float(self.end_time))]
+            for d in range(D):
+                for jt in range(J):
+                    jobs = float(self.jobs[d, jt])
+                    for name, s_, qv in (("wait_s", self.wait_sum, self.wait_quantiles(d, jt)),
+                                         ("response_s", self.resp_sum, self.response_quantiles(d, jt))):
+                        w.writerow(head + [dc_names[d], JOB_TYPES[jt], name, int(jobs),
+                                           repr(float(s_[d, jt]) / jobs if jobs else nan), "", ""]
+                                   + [repr(float(v)) for v in qv] + [""])
+                    w.writerow(head + [dc_names[d], JOB_TYPES[jt], "waited_share", int(jobs),
+                                       repr(float(self.waited[d, jt]) / jobs if jobs else nan), "", ""]
+                               + [""] * len(self.q) + [""])
+
+
+def waits_finalize(mom, m2, hist, wait_hist, n_dc: int, bin_s: float, end_time: float,
+                   quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobWaitsResult:
+    """All-reduced moments [4, columns], m2, histograms [columns, BINS] and per-DC wait / response histograms ->
+    statistics."""
+    F, J = len(WAIT_FIELDS), 2
+    mom = np.asarray(mom, dtype=np.float64)
+    rows = mom.shape[1] // (F * n_dc * J)
+    shape = (rows, F, n_dc, J)
+    st = column_stats(mom, m2, hist, _wait_integral(mom.shape[1], n_dc), quantiles)
+    s4 = mom[1].reshape(shape)[-1]                     # whole-run sums over the valid replicas
+    wh = np.asarray(wait_hist).astype(np.uint64).reshape(n_dc, 2, J, LAT_BINS)
+    k = np.arange(rows - 1, dtype=np.float64)
+    return JobWaitsResult(t0_s=np.append(k * bin_s, 0.0), t1_s=np.append((k + 1.0) * bin_s, float(end_time)),
+                          bin_s=float(bin_s), end_time=float(end_time), fields=WAIT_FIELDS, **st.result_fields(shape),
+                          jobs=wh[:, 0].sum(axis=-1), waited=s4[0], wait_sum=s4[1], resp_sum=s4[2], wait_histogram=wh)
+
+
+def job_waits(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobWaitsResult:
+    """Statistics of the waiting / response-time recorder of ``engine`` (a finished BatchedEngine with enable_job_waits()),
+    over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
+    import torch
+    if not engine.job_waits_enabled:
+        raise RuntimeError("job waits not enabled (enable_job_waits)")
+    dev = torch.device("cuda", engine.device)
+    n_dc = engine.spec.n_dc
+    cols = (engine.job_ensemble_windows + 1) * len(WAIT_FIELDS) * n_dc * 2
+    passes = device_passes(dev, cols, engine.job_waits_moments_into, engine.job_waits_spread_into)
+    wait_hist = _allreduce_sum(torch.from_numpy(engine.dc_wait_histogram().astype(np.int64)).to(dev))
+    return waits_finalize(*passes, wait_hist, n_dc, engine.job_ensemble_bin, engine.spec.end_time, quantiles)
+
+
+def job_waits_from_rows(rows: np.ndarray, hist: np.ndarray, jobs: np.ndarray, status: np.ndarray, bin_s: float,
+                        end_time: float, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobWaitsResult:
+    """The same statistics from host rows [W + 1, 3, n_dc, 2, R], per-DC histograms [n_dc, 2 kinds, 2, LAT_BINS, R]
+    (BatchedEngine.job_waits_rows) and the job ensemble's counts [W + 1, n_dc, 2, R] (job_ensemble_rows()[0][:, 0])
+    through the numpy mirror; replicas with status != 0 are left out.  All-reduced over the ranks like job_waits."""
+    import torch
+    n_dc = rows.shape[2]
+    x, ok = _wait_columns(rows, jobs, status)
+    passes = host_passes(x, ok, _wait_integral(x.shape[0], n_dc))
+    good = np.asarray(status) == 0
+    wait_hist = _allreduce_sum(torch.from_numpy(np.asarray(hist)[..., good].astype(np.int64).sum(axis=-1)))
+    return waits_finalize(*passes, wait_hist, n_dc, bin_s, end_time, quantiles)
 
 
 # ---- power profile ---------------------------------------------------------------------------------------------------

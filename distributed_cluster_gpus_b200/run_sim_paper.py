@@ -65,7 +65,11 @@ def parse_args(argv=None):
                    help="write, per finish window and for the whole run, statistics of every DC's job counts and mean "
                         "latencies per job type over all replicas (long format), and per-DC latency quantiles, to this file")
     p.add_argument("--job-ensemble-bin", type=float, default=None, metavar="SECONDS",
-                   help="finish-window width of --job-ensemble-csv (default: --log-interval)")
+                   help="finish-window width of --job-ensemble-csv and --job-waits-csv (default: --log-interval)")
+    p.add_argument("--job-waits-csv", type=str, default=None, metavar="PATH",
+                   help="write, per finish window and for the whole run, statistics of every DC's jobs that waited, mean "
+                        "wait (start - xfer_done) and mean response time (finish - arrival) per job type over all "
+                        "replicas (the --job-ensemble-csv format), and per-DC wait and response quantiles, to this file")
     p.add_argument("--power-profile-csv", type=str, default=None, metavar="PATH",
                    help="write batch statistics of every replica's cluster power over time — peak, time and energy over "
                         "--power-threshold, longest excursion, per-DC peaks — and the pooled power-duration curve's "
@@ -114,7 +118,7 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
         cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
         job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
-        power_threshold=power_threshold(args))
+        power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None)
     return sim
 
 
@@ -152,6 +156,7 @@ def main(argv=None):
     stats = batch_statistics(sim.summary)
     _add_latency_quantiles(stats, sim.latency_histogram)
     _add_power_profile(stats, sim.power_profile)
+    _add_job_waits(stats, sim.job_waits)
     _report(args, stats)
     return sim
 
@@ -163,6 +168,8 @@ def _write_ensemble(args, sim):
         sim.job_ensemble.to_csv(args.job_ensemble_csv, [dc.name for dc in sim.dcs.values()])
     if args.power_profile_csv:
         sim.power_profile.to_csv(args.power_profile_csv, [dc.name for dc in sim.dcs.values()])
+    if args.job_waits_csv:
+        sim.job_waits.to_csv(args.job_waits_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -179,6 +186,13 @@ def _add_power_profile(stats, res):
                     "excursions_mean": float(res.mean[col("excursions")]),
                     "longest_over_s_max": float(res.max[col("longest_over_s")]), "over_share": res.over_share})
     stats["power_profile"] = out
+
+
+def _add_job_waits(stats, res):
+    """Per job type, pooled over DCs and replicas, for --summary-json: mean / p50 / p95 / p99 of wait and response
+    time, and the share of jobs that waited."""
+    if res is not None:
+        stats["job_waits"] = res.pooled()
 
 
 def _add_latency_quantiles(stats, hist):
@@ -221,6 +235,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--job-ensemble-csv needs at least one replica per rank")
     if args.power_profile_csv and count == 0:
         raise SystemExit("--power-profile-csv needs at least one replica per rank")
+    if args.job_waits_csv and count == 0:
+        raise SystemExit("--job-waits-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -255,6 +271,7 @@ def _main_sharded(args, world, rank):
                  "mean_latency_s_p05_p50_p95": [float(q) for q in np.percentile(cols[1][keep], [5, 50, 95])]}
         _add_latency_quantiles(stats, hist.cpu().numpy().astype(np.uint64))
         _add_power_profile(stats, sim.power_profile)
+        _add_job_waits(stats, sim.job_waits)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -275,9 +292,9 @@ def _main_compare(args, world, rank):
     if args.power_profile_csv or args.power_threshold is not None:
         raise SystemExit("--power-profile-csv / --power-threshold are not available with --compare-algos (run each algo "
                          "on its own)")
-    if args.ensemble_csv or args.job_ensemble_csv:
-        raise SystemExit("--ensemble-csv / --job-ensemble-csv are not available with --compare-algos (run each algo "
-                         "on its own for its cluster-log and job-log ensembles)")
+    if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
+        raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
+                         "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")
     dist = None
     first, count, device = 0, args.replicas, args.device
     if world > 1:

@@ -401,6 +401,45 @@ int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* 
 /* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
+/* Waiting and response times (beside the job-log ensemble, in its cells): a finished job's arrival instant `arr`
+ * (simulator_paper_multi.py:539-540), its xfer_done instant `tx` (SIM:580-588) and its start and finish give
+ *   wait = start - tx        (the time in its DC's FIFO, SIM:678 -> SIM:840-927; exactly 0.0 when it started at tx)
+ *   resp = finish - arr      (time in system: WAN transfer + wait + service)
+ * each one f64 subtraction.  Per replica and cell (the job ensemble's window k and row W, DC, job type), added in finish
+ * order: WAITED (jobs with wait > 0), WAIT_SUM, RESP_SUM.  Device layout [W + 1][DCSIM_JWAIT_STORED][n_dc][2 jtypes]
+ * [n_replicas] doubles, replica fastest, and per-DC histograms [n_replicas][n_dc][2 kinds: wait, resp][2 jtypes]
+ * [DCSIM_LAT_BINS] u32 (the bin rule of the latency histograms; a zero wait falls in bin 0).  The reductions' columns
+ * are (row, field, dc, jtype): the three stored fields over every valid replica (WAITED the integer one), then
+ * MEAN_WAIT = WAIT_SUM / JOBS and MEAN_RESPONSE = RESP_SUM / JOBS over the replicas with JOBS > 0 in the cell (JOBS from
+ * the job ensemble). */
+enum {
+  DCSIM_JWAIT_WAITED = 0,        /* finished jobs of the cell whose wait was > 0 */
+  DCSIM_JWAIT_WAIT_SUM = 1,      /* sum of their waits [s] (all finished jobs of the cell) */
+  DCSIM_JWAIT_RESP_SUM = 2,      /* sum of their response times [s] */
+  DCSIM_JWAIT_STORED = 3,        /* fields the recorder stores per replica */
+  DCSIM_JWAIT_MEAN_WAIT = 3,     /* WAIT_SUM / JOBS (reductions only) */
+  DCSIM_JWAIT_MEAN_RESPONSE = 4, /* RESP_SUM / JOBS (reductions only) */
+  DCSIM_JWAIT_FIELDS = 5         /* fields of the reductions' columns */
+};
+/* Opt-in, after dcsim_enable_job_ensemble and before the first advance of a batch (stays on across dcsim_reset, zeroed
+ * by it; a later dcsim_enable_job_ensemble with another bin_s switches it off).  The running-job records then carry the
+ * job id (the layout job_log.csv uses).  DCSIM_E_STATE without the job
+ * ensemble, after the first advance or on a member of a shared group; DCSIM_E_NOMEM (with the byte count in
+ * dcsim_last_error) when the buffers do not fit. */
+int dcsim_enable_job_waits(dcsim_t* h);
+/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][DCSIM_JWAIT_STORED][n_dc][2]
+ * [n_replicas] doubles, `hist` [n_replicas][n_dc][2][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than
+ * its array is DCSIM_E_INVALID. */
+int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
+/* The two passes over the columns (row, field, dc, jtype), [4][(W + 1) * DCSIM_JWAIT_FIELDS * n_dc * 2]: the contract
+ * of dcsim_job_ensemble_moments / _spread; WAITED is the integer field. */
+int dcsim_job_waits_moments(dcsim_t* h, double* dev_out);
+int dcsim_job_waits_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                           double* dev_m2_out, uint64_t* dev_hist_out);
+/* The per-DC wait and response histograms summed over the valid replicas: `out` [n_dc][2 kinds][2][DCSIM_LAT_BINS] u64
+ * (synchronises). */
+int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
+
 /* Power profile: for EVERY replica, the cluster power P(t) its total energy integrates, as a step function, and what a
  * site is sized by — peak, time and energy over a threshold, a time-weighted power histogram.
  *   - Each inter-event interval (t_{k-1}, t_k] of positive length has power sum_d P_d, summed in DC order from 0.0,

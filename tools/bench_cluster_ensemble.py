@@ -1,9 +1,10 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job / power, the job-log ensemble / the power profile) at bench size: the event loop with
+"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits, the job-log ensemble / the power profile / the
+waiting-time recorder on top of the job ensemble) at bench size: the event loop with
 the recorder off and on, the two reduction kernels, the recorder's bytes per replica.  One JSON line on stdout; writes
 nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
@@ -28,7 +29,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -45,7 +46,11 @@ def main():
 
     def make(arm):
         e = BatchedEngine(sp, n, base_seed=seed, cuda_stream=stream.cuda_stream)
-        if arm == "on" and args.recorder == "job":
+        if args.recorder == "waits":            # the waits' own cost: both arms run the job ensemble they need
+            e.enable_job_ensemble()
+            if arm == "on":
+                e.enable_job_waits()
+        elif arm == "on" and args.recorder == "job":
             e.enable_job_ensemble()
         elif arm == "on" and args.recorder == "power":
             e.enable_power_profile(sp.power_cap if sp.power_cap > 0 else None)
@@ -63,6 +68,7 @@ def main():
                 e.close()
 
     on = make("on")
+    stats = None
     try:
         on.advance(0)
         events = float(on.summary()[:, S.S_EVENTS].sum())
@@ -70,6 +76,17 @@ def main():
             cols = S.PP_FIELDS + sp.n_dc + S.PP_BINS
             moments_into, spread_into = on.power_profile_moments_into, on.power_profile_spread_into
             rows, recorder_bytes = cols, cols * 8 + 20 * 8      # columns + the working row (DCSIM_PPW_N doubles)
+        elif args.recorder == "waits":
+            cols = (on.job_ensemble_windows + 1) * len(EN.WAIT_FIELDS) * sp.n_dc * 2
+            moments_into, spread_into = on.job_waits_moments_into, on.job_waits_spread_into
+            rows, recorder_bytes = on.job_ensemble_windows + 1, ((on.job_ensemble_windows + 1) * 3 * sp.n_dc * 2 * 8
+                                                                 + sp.n_dc * 2 * 2 * EN.LAT_BINS * 4)
+            summ = on.summary()
+            stats = EN.job_waits(on).pooled()
+            for jt, name in enumerate(EN.JOB_TYPES):   # the service latency the summaries report, beside the waits
+                fin = summ[:, S.S_FIN_INF if jt == 0 else S.S_FIN_TRN].sum()
+                lat = summ[:, S.S_LAT_SUM_INF if jt == 0 else S.S_LAT_SUM_TRN].sum()
+                stats[name]["mean_service_s"] = float(lat / fin) if fin else float("nan")
         elif args.recorder == "job":
             cols = (on.job_ensemble_windows + 1) * len(EN.JOB_FIELDS) * sp.n_dc * 2
             moments_into, spread_into = on.job_ensemble_moments_into, on.job_ensemble_spread_into
@@ -112,7 +129,8 @@ def main():
                       "events_per_s_on": events / (med(loop_ms["on"]) / 1e3),
                       "slowdown_on_vs_off": med(loop_ms["on"]) / med(loop_ms["off"]) - 1.0,
                       "rows": rows, "bytes_per_replica": recorder_bytes, "bytes_total": recorder_bytes * n,
-                      "moments_ms": moments_ms, "spread_ms": spread_ms}), flush=True)
+                      "moments_ms": moments_ms, "spread_ms": spread_ms,
+                      **({"waits": stats} if args.recorder == "waits" else {})}), flush=True)
 
 
 if __name__ == "__main__":
