@@ -30,6 +30,8 @@ EXPORTS = (
     "dcsim_power_profile_spread",
     "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_job_waits_moments", "dcsim_job_waits_spread",
     "dcsim_fetch_dc_wait_histogram",
+    "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy", "dcsim_occupancy_moments",
+    "dcsim_occupancy_spread",
 )
 
 _lib = None
@@ -143,6 +145,17 @@ def load():
         L.dcsim_job_waits_spread.argtypes = [vp, vp, vp, vp, vp, vp]
         L.dcsim_fetch_dc_wait_histogram.restype = i32
         L.dcsim_fetch_dc_wait_histogram.argtypes = [vp, vp, C.c_size_t]
+    if hasattr(L, "dcsim_enable_occupancy"):
+        L.dcsim_enable_occupancy.restype = i32
+        L.dcsim_enable_occupancy.argtypes = [vp]
+        L.dcsim_occupancy_bin_widths.restype = i32
+        L.dcsim_occupancy_bin_widths.argtypes = [vp, vp]
+        L.dcsim_fetch_occupancy.restype = i32
+        L.dcsim_fetch_occupancy.argtypes = [vp, vp, C.c_size_t]
+        L.dcsim_occupancy_moments.restype = i32
+        L.dcsim_occupancy_moments.argtypes = [vp, vp]
+        L.dcsim_occupancy_spread.restype = i32
+        L.dcsim_occupancy_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_power_profile"):
         L.dcsim_enable_power_profile.restype = i32
         L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]

@@ -36,8 +36,8 @@ extern __shared__ __align__(16) char dcsim_smem[];
  *                      leave the SM below its 32 warps (8 DC x 256: 17 kB -> 12 warps/SM; head ~4 kB -> 32);
  *   DCSIM_MODE_INPLACE nothing is staged (even the head exceeds a CTA's shared memory): same core on the HBM copy. */
 enum { DCSIM_MODE_INPLACE = 0, DCSIM_MODE_STAGED = 1, DCSIM_MODE_HEAD = 2 };
-/* PP = the power-profile recorder is compiled in (launched when it is enabled): the kernels without it keep their
- * registers, spills and code. */
+/* PP = the profile recorders (power profile, occupancy) are compiled in (launched when either is enabled): the kernels
+ * without them keep their registers, spills and code. */
 template <bool CAP, int MODE, bool PP>
 __global__ void __launch_bounds__(DCSIM_MAX_WARPS_PER_CTA * 32, DCSIM_MIN_CTAS_PER_SM)
 DCSIM_ADV(dcsim_advance_kernel)(const __grid_constant__ dcsim_kparams_t P, unsigned long long* __restrict__ events_total) {
@@ -91,15 +91,15 @@ static DCSIM_ADV(dcsim_advance_fn) DCSIM_ADV(dcsim_pick_kernel)(bool cap, int mo
 int DCSIM_ADV(dcsim_adv_min_ctas)(void) { return DCSIM_MIN_CTAS_PER_SM; }
 
 /* Launch on `stream`: `ctas` CTAs of `threads` threads (threads / DCSIM_LANES replicas each), `smem` dynamic bytes.  The
- * instantiation with the power-profile recorder when P->pp is set. */
+ * instantiation with the profile recorders when P->pp or P->occ is set. */
 cudaError_t DCSIM_ADV(dcsim_adv_launch)(const dcsim_kparams_t* P, unsigned long long* events, int cap, int mode, int ctas, int threads,
                                         int smem, cudaStream_t stream) {
-  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
+  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr || P->occ != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
   return cudaGetLastError();
 }
 
 /* Registers per thread and resident CTAs per SM of the instantiation for (cap, mode) at that CTA shape (the one without
- * the power-profile recorder); also raises the dynamic shared-memory limit of both to `smem_optin`. */
+ * the profile recorders); also raises the dynamic shared-memory limit of both to `smem_optin`. */
 cudaError_t DCSIM_ADV(dcsim_adv_attrs)(int cap, int mode, int threads, int smem, int smem_optin, int* regs, int* blocks_per_sm,
                                        int* min_ctas_per_sm) {
   const DCSIM_ADV(dcsim_advance_fn) kern = DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, false);

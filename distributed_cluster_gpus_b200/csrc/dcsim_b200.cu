@@ -320,6 +320,36 @@ struct dcsim_ens_pp_src {
   }
 };
 
+/* Occupancy: the first DCSIM_OCC_FIELDS * n_dc columns are the statistics (field, dc) — the stored per-DC field over
+ * PROFILE_S, the two maxima as stored — then the 2 * DCSIM_OCC_BINS * n_dc bins as stored
+ * ([1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n], column c of the source at stored column 1 + c).  A
+ * replica counts when its status is 0 and PROFILE_S > 0. */
+struct dcsim_ens_occ_src {
+  const double* occ;
+  const uint32_t* status;
+  uint64_t n;
+  uint32_t stat_cols; /* DCSIM_OCC_FIELDS * n_dc */
+  uint32_t n_dc;
+  struct view {
+    const double* x;
+    const double* profile;
+    const uint32_t* status;
+    bool share;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      const double p = profile[r];
+      if (status[r] != 0u || !(p > 0.0)) return false;
+      v = share ? x[r] / p : x[r];
+      return true;
+    }
+  };
+  __device__ __forceinline__ static bool is_max(int field) { return field == DCSIM_OCC_Q_INF_MAX || field == DCSIM_OCC_Q_TRN_MAX; }
+  __device__ __forceinline__ view at(uint64_t col) const {
+    const bool share = col < stat_cols && !is_max((int)(col / n_dc));
+    return view{occ + (col + 1) * n, occ, status, share};
+  }
+  __device__ __forceinline__ bool integral(uint64_t col) const { return col < stat_cols && is_max((int)(col / n_dc)); }
+};
+
 __device__ __forceinline__ double dcsim_ens_min(double a, double b) { return b < a ? b : a; }
 __device__ __forceinline__ double dcsim_ens_max(double a, double b) { return b > a ? b : a; }
 
@@ -485,6 +515,8 @@ struct dcsim {
   double* d_pp;            /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile (opt-in) */
   double* d_pp_work;       /* [n_replicas][DCSIM_PPW_N] its working state */
   double pp_threshold;
+  double* d_occ;           /* [1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n_replicas] occupancy (opt-in) */
+  double* d_occ_work;      /* [n_replicas][n_dc][DCSIM_OCCW_N] its working state */
   double* d_jwait;         /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waiting / response times (opt-in) */
   uint32_t* d_jwait_hist;  /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] their per-DC histograms */
   unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_wait_histogram */
@@ -515,6 +547,13 @@ static size_t jwait_hist_bytes(const dcsim_t* h) { return 2 * jens_hist_bytes(h)
 static uint64_t pp_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc + DCSIM_PP_BINS); }
 static size_t pp_bytes(const dcsim_t* h) { return (size_t)pp_cols(h) * (size_t)h->n_replicas * sizeof(double); }
 static size_t pp_work_bytes(const dcsim_t* h) { return (size_t)h->n_replicas * DCSIM_PPW_N * sizeof(double); }
+
+static uint64_t occ_stat_cols(const dcsim_t* h) { return (uint64_t)DCSIM_OCC_FIELDS * (uint64_t)h->spec.n_dc; }
+static uint64_t occ_cols(const dcsim_t* h) { return occ_stat_cols(h) + 2ull * DCSIM_OCC_BINS * (uint64_t)h->spec.n_dc; }
+static size_t occ_bytes(const dcsim_t* h) { return (size_t)(1 + occ_cols(h)) * (size_t)h->n_replicas * sizeof(double); }
+static size_t occ_work_bytes(const dcsim_t* h) {
+  return (size_t)h->n_replicas * (size_t)h->spec.n_dc * DCSIM_OCCW_N * sizeof(double);
+}
 
 static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", long long b = 0) {
   char* dst = h ? h->err : g_create_err;
@@ -927,6 +966,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
   }
+  if (h->d_occ) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_occ, 0, occ_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_occ_work, 0, occ_work_bytes(h), h->g->stream));
+  }
   if (h->d_jwait) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, (h->jens_windows + 1) * jwait_row_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
@@ -1014,6 +1057,7 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
   P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
   P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
+  P->occ = h->d_occ; P->occ_work = h->d_occ_work;
 }
 
 /* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */
@@ -1493,6 +1537,57 @@ int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double*
   return ens_spread(h, src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
+int dcsim_enable_occupancy(dcsim_t* h) {
+  if (!h) return DCSIM_E_INVALID;
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_occupancy on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_occupancy must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  if (!h->d_occ) {
+    const int rc = recorder_alloc(h, (void**)&h->d_occ, occ_bytes(h), (void**)&h->d_occ_work, occ_work_bytes(h),
+                                  "enable_occupancy: %s%lld bytes of device memory do not fit (run fewer replicas)",
+                                  (long long)(occ_bytes(h) + occ_work_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->d_occ, 0, occ_bytes(h), h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_occ_work, 0, occ_work_bytes(h), h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_occupancy_bin_widths(dcsim_t* h, int32_t* w_out) {
+  if (!h || !w_out) return DCSIM_E_INVALID;
+  for (int d = 0; d < h->spec.n_dc; ++d) w_out[d] = DCSIM_OCC_BUSY_WIDTH(h->spec.dc[d].total_gpus);
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  const int rc = recorder_ready(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
+  if (rc != DCSIM_OK) return rc;
+  if (out_bytes < occ_bytes(h))
+    return set_err(h, DCSIM_E_INVALID, "fetch_occupancy: buffer too small (need %s%lld bytes)", "", (long long)occ_bytes(h));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_occ, occ_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_occupancy_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_occ_src src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)h->spec.n_dc};
+  return ens_moments(h, src, h->n_replicas, occ_cols(h), dev_out);
+}
+
+int dcsim_occupancy_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                           double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_occ_src src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)h->spec.n_dc};
+  return ens_spread(h, src, h->n_replicas, occ_stat_cols(h), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out); /* the bins need no spread */
+}
+
 int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {
   if (!h || !out3) return DCSIM_E_INVALID;
   CUDA_TRY(h, cudaSetDevice(h->device));
@@ -1563,6 +1658,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
   cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
+  cudaFree(h->d_occ); cudaFree(h->d_occ_work);
   cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;

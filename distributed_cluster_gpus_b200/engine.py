@@ -355,6 +355,44 @@ class BatchedEngine:
         N.check(self._lib.dcsim_power_profile_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
                                                      C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
+    # -- occupancy (ensemble.occupancy turns it into batch statistics) ------------------------------------------------
+    def enable_occupancy(self):
+        """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records, per
+        DC, the time-weighted queue lengths, running jobs and busy GPUs between every two events — areas, maxima, time
+        queued / saturated / idle, and queue-length and busy-GPU histograms (include/dcsim_b200.h DCSIM_OCC_*).  Runs the
+        event-loop instantiation with the profile recorders compiled in."""
+        N.check(self._lib.dcsim_enable_occupancy(self._h), self._h)
+        self._occ_on = True
+
+    @property
+    def occupancy_enabled(self) -> bool:
+        return getattr(self, "_occ_on", False)
+
+    def occupancy_bin_widths(self) -> np.ndarray:
+        """[n_dc] int32: GPUs per busy-GPU bin of each DC (1 for DCs of up to 127 GPUs)."""
+        w = np.zeros(self.spec.n_dc, dtype=np.int32)
+        N.check(self._lib.dcsim_occupancy_bin_widths(self._h, C.c_void_p(w.ctypes.data)), self._h)
+        return w
+
+    def occupancy_rows(self) -> np.ndarray:
+        """[1 + OCC_FIELDS * n_dc + 2 * OCC_BINS * n_dc, n_replicas] float64: every replica's raw columns.  For tests
+        and small batches."""
+        n_dc = self.spec.n_dc
+        rows = np.empty((1 + S.OCC_FIELDS * n_dc + 2 * S.OCC_BINS * n_dc, self.n_replicas), dtype=np.float64)
+        N.check(self._lib.dcsim_fetch_occupancy(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
+        return rows
+
+    def occupancy_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][OCC_FIELDS * n_dc + 2 * OCC_BINS * n_dc] float64 {n, sum, min, max} at
+        ``device_ptr``."""
+        N.check(self._lib.dcsim_occupancy_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def occupancy_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream over the first OCC_FIELDS * n_dc columns: sum (x - mean)^2 and an ENS_BINS
+        histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_occupancy_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                 C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
     # -- paired reductions (compare.py) ------------------------------------------------------------------------------
     def paired_moments_into(self, variant_summary_ptr: int, device_ptr: int):
         """Pass 1 on this (base) handle's stream against a variant's [n_replicas, SUMMARY_K] summaries on the device:
@@ -475,10 +513,12 @@ def _pp_key(power_profile, power_threshold):
     return (float("inf") if power_threshold is None else float(power_threshold)) if power_profile else None
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False):
+def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False,
+               occupancy=False):
     # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None))
+            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None),
+            bool(occupancy))
 
 
 def _drop_parked_batch_engine():
@@ -488,15 +528,16 @@ def _drop_parked_batch_engine():
 
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
-                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False):
+                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
+                   occupancy=False):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
     ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
     power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
-    response-time recorder on (it implies the job ensemble).  A parked engine is only reused by a caller that asks for
-    the same recorders."""
+    response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on.  A parked
+    engine is only reused by a caller that asks for the same recorders."""
     job_bin = _job_bin(sp, job_ensemble or job_waits, job_ensemble_bin)
     key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
-                     job_waits)
+                     job_waits, occupancy)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -515,6 +556,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_job_waits()
         if power_profile:
             eng.enable_power_profile(power_threshold)
+        if occupancy:
+            eng.enable_occupancy()
     except BaseException:
         eng.close()
         raise
@@ -529,7 +572,7 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
                                                         eng.job_ensemble_bin,
                                                         _pp_key(eng.power_profile_enabled, eng.power_threshold),
-                                                        eng.job_waits_enabled)
+                                                        eng.job_waits_enabled, eng.occupancy_enabled)
 
 
 def free_cached_engine():
@@ -578,19 +621,21 @@ class LoggedReplica:
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
-                      job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False):
+                      job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
+                      occupancy=False):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
     kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
     ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
     window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
-    None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble)."""
+    None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble);
+    ``occupancy``: with the occupancy recorder on."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
-                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits)
+                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

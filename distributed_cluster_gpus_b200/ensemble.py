@@ -793,3 +793,157 @@ def power_profile_from_rows(rows: np.ndarray, summary: np.ndarray, hi: float, th
     passes = host_passes(rows, np.broadcast_to(good[None, :], rows.shape), _pp_integral(stat_cols), stat_cols)
     return pp_finalize(*passes, n_dc, hi, float("inf") if threshold is None else float(threshold), _pooled_energy(summary),
                        quantiles)
+
+
+# ---- occupancy -------------------------------------------------------------------------------------------------------
+# per-replica statistics of each DC's step functions (DCSIM_OCC_* order): the time averages of Qi, Qt and N, the longest
+# queues, and the shares of the profile with a queue, with every GPU busy and with none busy
+OCC_STATS = ("mean_q_inf", "mean_q_trn", "mean_running", "max_q_inf", "max_q_trn", "queued_share", "saturated_share",
+             "idle_share")
+OCC_MAX_STATS = (3, 4)                                 # the stored maxima: integer columns, not divided by profile_s
+OCC_BINS = 128                                         # DCSIM_OCC_BINS
+OCC_TIME_KINDS = ("queue", "busy")
+
+
+def _occ_integral(n_dc: int) -> np.ndarray:
+    return np.isin(np.arange(len(OCC_STATS) * n_dc) // n_dc, OCC_MAX_STATS)
+
+
+def _occ_columns(rows: np.ndarray, status: np.ndarray):
+    """rows [1 + 8 * n_dc + 2 * OCC_BINS * n_dc, R], status [R] -> (x, ok) [8 * n_dc + 2 * OCC_BINS * n_dc, R] as the
+    kernels' column source: the stored per-DC fields over profile_s (the maxima as stored), then the bins; replica r
+    counts when its status is 0 and profile_s > 0."""
+    rows = np.asarray(rows, dtype=np.float64)
+    profile = rows[0]
+    n_dc = (rows.shape[0] - 1) // (len(OCC_STATS) + 2 * OCC_BINS)
+    n_stat = len(OCC_STATS) * n_dc
+    x = rows[1:].copy()
+    share = ~np.isin(np.arange(n_stat) // n_dc, OCC_MAX_STATS)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        x[:n_stat][share] = x[:n_stat][share] / profile[None, :]
+    ok = (np.asarray(status) == 0) & (profile > 0)
+    return x, np.broadcast_to(ok[None, :], x.shape)
+
+
+@dataclass
+class OccupancyResult:
+    """Batch statistics of the occupancy recorder over the replicas with status 0 and a non-empty profile.  ``n`` ...
+    ``max`` and ``quantiles`` ([Q, columns]) cover ``columns`` = (stat, dc) for every OCC_STATS entry and DC.
+    ``queue_bins`` / ``busy_bins`` [n_dc, OCC_BINS]: pooled seconds at each queue length (the last bin: that length or
+    more) and each busy-GPU bin of ``bin_widths`` GPUs, summed over the replicas."""
+    columns: Tuple[Tuple[str, int], ...]
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray
+    queue_bins: np.ndarray
+    busy_bins: np.ndarray
+    bin_widths: np.ndarray
+
+    def column(self, stat: str, dc: int) -> int:
+        return self.columns.index((stat, dc))
+
+    @property
+    def replicas(self) -> int:
+        return int(self.n[0]) if len(self.n) else 0
+
+    def queue_curve(self, dc: int):
+        """(queue lengths [OCC_BINS], pooled seconds at each); the last bin holds OCC_BINS - 1 jobs or more."""
+        return np.arange(OCC_BINS, dtype=np.float64), self.queue_bins[dc].copy()
+
+    def busy_curve(self, dc: int):
+        """(busy GPUs at each bin's lower edge [OCC_BINS], pooled seconds in each bin); exact values when the DC's bin
+        width is 1."""
+        return np.arange(OCC_BINS, dtype=np.float64) * float(self.bin_widths[dc]), self.busy_bins[dc].copy()
+
+    def time_quantiles(self, kind: str, dc: int, shares: Sequence[float]) -> np.ndarray:
+        """For ``kind`` "queue" or "busy": the value the DC was at or above for each share of the pooled time (0.01: the
+        queue length reached or exceeded 1 % of the time), a bin's lower edge; NaN without pooled time."""
+        vals, sec = self.queue_curve(dc) if kind == "queue" else self.busy_curve(dc)
+        total = sec.sum()
+        out = np.full(len(shares), np.nan)
+        if total <= 0:
+            return out
+        above = np.cumsum(sec[::-1])[::-1]             # time at or above each bin
+        for i, s in enumerate(shares):
+            k = np.nonzero(above >= float(s) * total)[0]
+            out[i] = vals[int(k.max()) if len(k) else 0]
+        return out
+
+    def pooled(self) -> dict:
+        """Per DC (index): the batch means of mean_q_inf, mean_q_trn, saturated_share and idle_share, and the queue
+        length exceeded for 10 % and 1 % of the pooled time."""
+        out = {}
+        for d in range(self.queue_bins.shape[0]):
+            row = {s: float(self.mean[self.column(s, d)]) for s in ("mean_q_inf", "mean_q_trn", "saturated_share", "idle_share")}
+            p10, p1 = self.time_quantiles("queue", d, (0.1, 0.01))
+            row.update(queue_len_top10pct=float(p10), queue_len_top1pct=float(p1))
+            out[d] = row
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """Long format: dc,field,n,mean,std,min,p05,p25,p50,p75,p95,p99,max — one row per DC and statistic, then per DC
+        a ``queue_len_time`` and a ``busy_gpus_time`` row for the pooled time distributions: n = replicas, mean = the
+        time-weighted mean of the bins' values, std empty, min / max the lowest / highest occupied bin, the quantiles the
+        values reached or exceeded for 95 / 75 / 50 / 25 / 5 / 1 % of the pooled time."""
+        fmt = lambda x: repr(float(x))  # noqa: E731
+        D = self.queue_bins.shape[0]
+        with open(path, "w", newline="") as f:
+            w = csv.writer(f)
+            w.writerow(PP_CSV_HEADER)
+            for d in range(D):
+                for s in OCC_STATS:
+                    c = self.column(s, d)
+                    w.writerow([dc_names[d], s, int(self.n[c]), fmt(self.mean[c]), fmt(self.std[c]), fmt(self.min[c])]
+                               + [fmt(self.quantiles[j, c]) for j in range(len(self.q))] + [fmt(self.max[c])])
+            for d in range(D):
+                for kind, field in zip(OCC_TIME_KINDS, ("queue_len_time", "busy_gpus_time")):
+                    vals, sec = self.queue_curve(d) if kind == "queue" else self.busy_curve(d)
+                    total = sec.sum()
+                    occ = np.nonzero(sec > 0)[0]
+                    mean = float((vals * sec).sum() / total) if total > 0 else float("nan")
+                    lo = vals[occ.min()] if len(occ) else float("nan")
+                    hi = vals[occ.max()] if len(occ) else float("nan")
+                    tq = self.time_quantiles(kind, d, [1.0 - q for q in PP_CSV_QUANTILES])
+                    w.writerow([dc_names[d], field, self.replicas, fmt(mean), "", fmt(lo)] + [fmt(v) for v in tq] + [fmt(hi)])
+
+
+def occ_finalize(mom, m2, hist, n_dc: int, widths, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> OccupancyResult:
+    """All-reduced moments [4, 8 * n_dc + 2 * OCC_BINS * n_dc], m2 and histograms over the first 8 * n_dc columns, and
+    the busy-bin widths -> statistics."""
+    mom = np.asarray(mom, dtype=np.float64)
+    c = len(OCC_STATS) * n_dc
+    st = column_stats(mom[:, :c], np.asarray(m2)[:c], np.asarray(hist)[:c], _occ_integral(n_dc), quantiles)
+    columns = tuple((s, d) for s in OCC_STATS for d in range(n_dc))
+    bins = mom[1, c:c + 2 * OCC_BINS * n_dc].reshape(2, n_dc, OCC_BINS)
+    return OccupancyResult(columns=columns, **st.result_fields((c,)), queue_bins=bins[0].copy(), busy_bins=bins[1].copy(),
+                           bin_widths=np.asarray(widths, dtype=np.int64))
+
+
+def occupancy(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> OccupancyResult:
+    """Statistics of the occupancy recorder of ``engine`` (a finished BatchedEngine with enable_occupancy()), over all
+    ranks when torch.distributed runs with world > 1 (every rank calls this)."""
+    import torch
+    if not engine.occupancy_enabled:
+        raise RuntimeError("occupancy not enabled (enable_occupancy)")
+    dev = torch.device("cuda", engine.device)
+    n_dc = engine.spec.n_dc
+    stat = len(OCC_STATS) * n_dc
+    passes = device_passes(dev, stat + 2 * OCC_BINS * n_dc, engine.occupancy_moments_into, engine.occupancy_spread_into,
+                           stat_cols=stat)
+    return occ_finalize(*passes, n_dc, engine.occupancy_bin_widths(), quantiles)
+
+
+def occupancy_from_rows(rows: np.ndarray, summary: np.ndarray, widths, quantiles: Sequence[float] = PP_CSV_QUANTILES
+                        ) -> OccupancyResult:
+    """The same statistics from host rows [1 + 8 * n_dc + 2 * OCC_BINS * n_dc, R] (BatchedEngine.occupancy_rows), the
+    summary rows [R, SUMMARY_K] and the busy-bin widths [n_dc] (BatchedEngine.occupancy_bin_widths) through the numpy
+    mirror of both passes.  All-reduced over the ranks like occupancy."""
+    from . import spec as S
+    x, ok = _occ_columns(rows, np.asarray(summary)[:, S.S_STATUS])
+    n_dc = len(widths)
+    passes = host_passes(x, ok, _occ_integral(n_dc), len(OCC_STATS) * n_dc)
+    return occ_finalize(*passes, n_dc, widths, quantiles)

@@ -70,6 +70,10 @@ def parse_args(argv=None):
                    help="write, per finish window and for the whole run, statistics of every DC's jobs that waited, mean "
                         "wait (start - xfer_done) and mean response time (finish - arrival) per job type over all "
                         "replicas (the --job-ensemble-csv format), and per-DC wait and response quantiles, to this file")
+    p.add_argument("--occupancy-csv", type=str, default=None, metavar="PATH",
+                   help="write batch statistics of every DC's time-averaged queue lengths and running jobs, longest "
+                        "queues and shares of time queued / saturated / idle, measured between every two events, and "
+                        "the pooled queue-length and busy-GPU time distributions, to this file")
     p.add_argument("--power-profile-csv", type=str, default=None, metavar="PATH",
                    help="write batch statistics of every replica's cluster power over time — peak, time and energy over "
                         "--power-threshold, longest excursion, per-DC peaks — and the pooled power-duration curve's "
@@ -118,7 +122,8 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
         cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
         job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
-        power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None)
+        power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None,
+        occupancy=args.occupancy_csv is not None)
     return sim
 
 
@@ -157,6 +162,7 @@ def main(argv=None):
     _add_latency_quantiles(stats, sim.latency_histogram)
     _add_power_profile(stats, sim.power_profile)
     _add_job_waits(stats, sim.job_waits)
+    _add_occupancy(stats, sim.occupancy, sim)
     _report(args, stats)
     return sim
 
@@ -170,6 +176,8 @@ def _write_ensemble(args, sim):
         sim.power_profile.to_csv(args.power_profile_csv, [dc.name for dc in sim.dcs.values()])
     if args.job_waits_csv:
         sim.job_waits.to_csv(args.job_waits_csv, [dc.name for dc in sim.dcs.values()])
+    if args.occupancy_csv:
+        sim.occupancy.to_csv(args.occupancy_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -193,6 +201,14 @@ def _add_job_waits(stats, res):
     time, and the share of jobs that waited."""
     if res is not None:
         stats["job_waits"] = res.pooled()
+
+
+def _add_occupancy(stats, res, sim):
+    """Per DC, for --summary-json: the batch means of mean_q_inf, mean_q_trn, saturated_share and idle_share, and the
+    pooled queue length reached for 10 % and 1 % of the time."""
+    if res is not None:
+        names = [dc.name for dc in sim.dcs.values()]
+        stats["occupancy"] = {names[d]: v for d, v in res.pooled().items()}
 
 
 def _add_latency_quantiles(stats, hist):
@@ -237,6 +253,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--power-profile-csv needs at least one replica per rank")
     if args.job_waits_csv and count == 0:
         raise SystemExit("--job-waits-csv needs at least one replica per rank")
+    if args.occupancy_csv and count == 0:
+        raise SystemExit("--occupancy-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -272,6 +290,7 @@ def _main_sharded(args, world, rank):
         _add_latency_quantiles(stats, hist.cpu().numpy().astype(np.uint64))
         _add_power_profile(stats, sim.power_profile)
         _add_job_waits(stats, sim.job_waits)
+        _add_occupancy(stats, sim.occupancy, sim)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -292,6 +311,9 @@ def _main_compare(args, world, rank):
     if args.power_profile_csv or args.power_threshold is not None:
         raise SystemExit("--power-profile-csv / --power-threshold are not available with --compare-algos (run each algo "
                          "on its own)")
+    if args.occupancy_csv:
+        raise SystemExit("--occupancy-csv is not available with --compare-algos (run each algo on its own for its "
+                         "occupancy)")
     if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
         raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
                          "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")

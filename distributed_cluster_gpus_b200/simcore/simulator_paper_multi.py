@@ -61,7 +61,7 @@ class MultiIngressPaperSimulator:
                  replicas: int = 1, device: int = 0, first_replica_id: int = 0, write_logs: bool = True,
                  cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
                  job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None, power_profile: bool = False,
-                 power_threshold: Optional[float] = None, job_waits: bool = False):
+                 power_threshold: Optional[float] = None, job_waits: bool = False, occupancy: bool = False):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -114,6 +114,10 @@ class MultiIngressPaperSimulator:
         # above), ensemble.JobWaitsResult.  It runs the job ensemble's recorder too (its windows and job counts)
         self._want_job_waits = bool(job_waits)
         self.job_waits = None
+        # occupancy=True: after run(), statistics of every DC's time-weighted queue lengths, running jobs and busy GPUs
+        # between events over all replicas (all ranks, as above), ensemble.OccupancyResult
+        self._want_occupancy = bool(occupancy)
+        self.occupancy = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -166,7 +170,8 @@ class MultiIngressPaperSimulator:
                                           self.cuda_stream, configure=configure, while_running=while_running,
                                           cluster_ensemble=self._want_ensemble, job_ensemble=self._want_job_ensemble,
                                           job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
-                                          power_threshold=self._power_threshold, job_waits=self._want_job_waits)
+                                          power_threshold=self._power_threshold, job_waits=self._want_job_waits,
+                                          occupancy=self._want_occupancy)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -187,6 +192,9 @@ class MultiIngressPaperSimulator:
             if self._want_job_waits:
                 from ..ensemble import job_waits
                 self.job_waits = job_waits(eng)
+            if self._want_occupancy:
+                from ..ensemble import occupancy
+                self.occupancy = occupancy(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

@@ -43,6 +43,10 @@ AGG_K = 16
 # power-profile columns (DCSIM_PP_*): the fields, then DC_PEAK_W per DC, then PP_BINS histogram bins
 PP_PROFILE_S, PP_PEAK_W, PP_T_PEAK_S, PP_OVER_S, PP_OVER_J, PP_EXCURSIONS, PP_LONGEST_OVER_S, PP_OUT_OF_RANGE = range(8)
 PP_FIELDS, PP_BINS = 8, 1024
+# occupancy columns (DCSIM_OCC_*): PROFILE_S, then per DC the fields (column 1 + field * n_dc + dc), then per DC
+# OCC_BINS queue-length bins, then per DC OCC_BINS busy-GPU bins
+OCC_Q_INF_AREA, OCC_Q_TRN_AREA, OCC_RUN_AREA, OCC_Q_INF_MAX, OCC_Q_TRN_MAX, OCC_QUEUED_S, OCC_SATURATED_S, OCC_IDLE_S = range(8)
+OCC_FIELDS, OCC_BINS = 8, 128
 
 
 class Coeffs(C.Structure):

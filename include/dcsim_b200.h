@@ -485,6 +485,49 @@ int dcsim_power_profile_moments(dcsim_t* h, double* dev_out);
 int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                                double* dev_m2_out, uint64_t* dev_hist_out);
 
+/* Occupancy: for EVERY replica and DC d, how long the queues were and how full the DC was over time.  Step functions over
+ * [t0, end_time]: Qi(t) = len(q_inf), Qt(t) = len(q_train), Q = Qi + Qt, N(t) = running jobs, B(t) = busy GPUs.
+ *   - t0 is the first processed event (DCSIM_S_UTIL_BEGIN); a replica without one has an empty profile (every field 0).
+ *   - Over each inter-event interval (t_{k-1}, t_k] the value is the state before event k (the state the energy and
+ *     utilisation accrual integrates, SIM:429-437); over the tail (t_last, end_time] the final state.
+ *   - A LEVEL of one function is a maximal run of positive-length intervals with the same value.  Every field is a sum
+ *     over that function's levels in time order, a level adding value * (end - start) or its length end - start.
+ * Per replica PROFILE_S = end_time - t0, then per DC (column 1 + field * n_dc + d):
+ *   Q_INF_AREA, Q_TRN_AREA, RUN_AREA   sum of value * length over the levels of Qi, Qt, N
+ *   Q_INF_MAX, Q_TRN_MAX               largest level value, 0 if none (<= the instantaneous DCSIM_S_MAX_Q)
+ *   QUEUED_S                           total length of the levels of Q with Q > 0
+ *   SATURATED_S / IDLE_S               total length of the levels of B with B == total_gpus / B == 0
+ * then DCSIM_OCC_BINS queue-length bins per DC (seconds at each Q: bin min(Q, DCSIM_OCC_BINS - 1)) and DCSIM_OCC_BINS
+ * busy-GPU bins per DC (seconds at each B: bin B / DCSIM_OCC_BUSY_WIDTH(total_gpus)).
+ * Device layout [1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n_replicas] doubles, replica fastest: the
+ * queue bins of DC d at column 1 + FIELDS * n_dc + d * BINS, its busy bins at 1 + FIELDS * n_dc + (n_dc + d) * BINS. */
+enum {
+  DCSIM_OCC_Q_INF_AREA = 0, DCSIM_OCC_Q_TRN_AREA = 1, DCSIM_OCC_RUN_AREA = 2, DCSIM_OCC_Q_INF_MAX = 3,
+  DCSIM_OCC_Q_TRN_MAX = 4, DCSIM_OCC_QUEUED_S = 5, DCSIM_OCC_SATURATED_S = 6, DCSIM_OCC_IDLE_S = 7,
+  DCSIM_OCC_FIELDS = 8 /* per DC, after the PROFILE_S column */
+};
+#define DCSIM_OCC_BINS 128
+/* Busy-GPU bin width of a DC with `total` GPUs: ceil((total + 1) / DCSIM_OCC_BINS), 1 for up to 127 GPUs. */
+#define DCSIM_OCC_BUSY_WIDTH(total) (((total) + DCSIM_OCC_BINS) / DCSIM_OCC_BINS)
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  DCSIM_E_STATE after the
+ * first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the rows
+ * and their working state do not fit. */
+int dcsim_enable_occupancy(dcsim_t* h);
+/* w_out[n_dc]: each DC's busy-GPU bin width (DCSIM_OCC_BUSY_WIDTH). */
+int dcsim_occupancy_bin_widths(dcsim_t* h, int32_t* w_out);
+/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
+int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes);
+/* Columns: first DCSIM_OCC_FIELDS * n_dc statistics (field, dc), field-major, per replica Q_INF_AREA / PROFILE_S,
+ * Q_TRN_AREA / PROFILE_S, RUN_AREA / PROFILE_S, Q_INF_MAX, Q_TRN_MAX, QUEUED_S / PROFILE_S, SATURATED_S / PROFILE_S,
+ * IDLE_S / PROFILE_S; then the 2 * DCSIM_OCC_BINS * n_dc bins as stored.  A replica counts when its status is 0 and
+ * PROFILE_S > 0.  Pass 1 over every column: dev_out = [4][columns] {n, sum, min, max}; the bins' sums are the pooled
+ * time-weighted distributions of queue length and busy GPUs.  Pass 2 over the statistics columns only: m2 and
+ * histograms, the contract of dcsim_ensemble_spread; Q_INF_MAX and Q_TRN_MAX are the integer columns.  Both on the
+ * handle's stream, with device pointers. */
+int dcsim_occupancy_moments(dcsim_t* h, double* dev_out);
+int dcsim_occupancy_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                           double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant
  * batch with the same keys (a member's dcsim_summary_device_ptr or a copy of it: [n][DCSIM_SUMMARY_K] doubles on the
  * base's device).  Replica r counts in a column when both rows have status 0 and the metric is defined in both (a

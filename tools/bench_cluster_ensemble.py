@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits, the job-log ensemble / the power profile / the
-waiting-time recorder on top of the job ensemble) at bench size: the event loop with
+"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy, the job-log ensemble / the power
+profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder) at bench size: the event loop with
 the recorder off and on, the two reduction kernels, the recorder's bytes per replica.  One JSON line on stdout; writes
 nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
@@ -29,7 +29,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -54,6 +54,8 @@ def main():
             e.enable_job_ensemble()
         elif arm == "on" and args.recorder == "power":
             e.enable_power_profile(sp.power_cap if sp.power_cap > 0 else None)
+        elif arm == "on" and args.recorder == "occupancy":
+            e.enable_occupancy()
         elif arm == "on":
             e.enable_cluster_ensemble()
         return e
@@ -76,6 +78,10 @@ def main():
             cols = S.PP_FIELDS + sp.n_dc + S.PP_BINS
             moments_into, spread_into = on.power_profile_moments_into, on.power_profile_spread_into
             rows, recorder_bytes = cols, cols * 8 + 20 * 8      # columns + the working row (DCSIM_PPW_N doubles)
+        elif args.recorder == "occupancy":
+            cols = (S.OCC_FIELDS + 2 * S.OCC_BINS) * sp.n_dc
+            moments_into, spread_into = on.occupancy_moments_into, on.occupancy_spread_into
+            rows, recorder_bytes = cols + 1, (cols + 1) * 8 + sp.n_dc * 11 * 8   # columns + working rows (DCSIM_OCCW_N)
         elif args.recorder == "waits":
             cols = (on.job_ensemble_windows + 1) * len(EN.WAIT_FIELDS) * sp.n_dc * 2
             moments_into, spread_into = on.job_waits_moments_into, on.job_waits_spread_into
