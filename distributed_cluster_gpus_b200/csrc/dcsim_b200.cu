@@ -1101,6 +1101,57 @@ int dcsim_prepare(dcsim_t* h) {
   return DCSIM_OK;
 }
 
+#ifdef DCSIM_TEST_HOOKS
+/* TEST-ONLY (hook build only, like dcsim_test_set_time_quantum): fills the group's arrival, merge-scratch, list and
+ * header buffers with 0xee bytes, so that an entry the pre-pass or the merge fails to write cannot pass by holding the
+ * value an earlier batch left.  Only before the batch's prepare: the lists are read by every later advance. */
+int dcsim_test_poison_prepass(dcsim_t* h) {
+  if (!h) return DCSIM_E_INVALID;
+  if (h->g->arrivals_ready) return set_err(h, DCSIM_E_STATE, "test_poison_prepass: the batch's lists are already drawn%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const size_t ne = (size_t)h->g->n_replicas * (size_t)h->g->cap_arr;
+  cudaStream_t s = h->g->stream;
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_t, 0xee, ne * sizeof(double), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_raw, 0xee, ne * sizeof(double), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_meta, 0xee, ne * sizeof(uint32_t), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_pred, 0xee, ne * sizeof(uint32_t), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_tx, 0xee, ne * sizeof(double), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_fin, 0xee, ne * sizeof(uint32_t), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_ml_t, 0xee, 2 * ne * sizeof(double), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_ml_aux, 0xee, 2 * ne * sizeof(double), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_ml_meta, 0xee, 2 * ne * sizeof(uint32_t), s));
+  CUDA_TRY(h, cudaMemsetAsync(h->g->d_arr_hdr, 0xee, (size_t)h->g->n_replicas * sizeof(dcsim_arrhdr_t), s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DCSIM_OK;
+}
+
+/* TEST-ONLY: copies what the pre-pass and the merge left for local replicas [first, first + count) to host arrays in
+ * the device layout: arr_t / arr_raw (after the merge: the job sizes) / arr_meta / arr_pred / arr_tx [count][cap_arr],
+ * ml_t / ml_aux / ml_meta [count][2 * cap_arr] and the headers [count] (dcsim_arrhdr_t).  A range, because a large
+ * batch's lists take tens of GB. */
+int dcsim_test_fetch_prepass(dcsim_t* h, uint64_t first, uint64_t count, double* arr_t, double* arr_raw, uint32_t* arr_meta,
+                             uint32_t* arr_pred, double* arr_tx, double* ml_t, double* ml_aux, uint32_t* ml_meta, void* hdr) {
+  if (!h || !arr_t || !arr_raw || !arr_meta || !arr_pred || !arr_tx || !ml_t || !ml_aux || !ml_meta || !hdr) return DCSIM_E_INVALID;
+  if (first > h->g->n_replicas || count > h->g->n_replicas - first)
+    return set_err(h, DCSIM_E_INVALID, "test_fetch_prepass: replicas [first, first + count) out of range%s%lld");
+  if (!h->g->arrivals_ready) return set_err(h, DCSIM_E_STATE, "test_fetch_prepass: no lists drawn yet (prepare first)%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const size_t c = h->g->cap_arr, o = (size_t)first * c, ne = (size_t)count * c;
+  cudaStream_t s = h->g->stream;
+  CUDA_TRY(h, cudaMemcpyAsync(arr_t, h->g->d_arr_t + o, ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(arr_raw, h->g->d_arr_raw + o, ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(arr_meta, h->g->d_arr_meta + o, ne * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(arr_pred, h->g->d_arr_pred + o, ne * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(arr_tx, h->g->d_arr_tx + o, ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(ml_t, h->g->d_ml_t + 2 * o, 2 * ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(ml_aux, h->g->d_ml_aux + 2 * o, 2 * ne * sizeof(double), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(ml_meta, h->g->d_ml_meta + 2 * o, 2 * ne * sizeof(uint32_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaMemcpyAsync(hdr, h->g->d_arr_hdr + first, (size_t)count * sizeof(dcsim_arrhdr_t), cudaMemcpyDeviceToHost, s));
+  CUDA_TRY(h, cudaStreamSynchronize(s));
+  return DCSIM_OK;
+}
+#endif
+
 int dcsim_advance(dcsim_t* h, uint64_t max_events_per_replica, uint64_t* total_events_out) {
   if (!h) return DCSIM_E_INVALID;
   if (check_generation(h) != DCSIM_OK) return DCSIM_E_STATE;

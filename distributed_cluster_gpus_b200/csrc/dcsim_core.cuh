@@ -465,7 +465,7 @@ struct dcsim_kparams_t {
   uint32_t* arr_pred;   /* index of the stream's previous arrival (whose processing pushed this one), 0xffffffff = the constructor */
   /* merge scratch, same indexing */
   double* arr_tx;       /* xfer_done instant of arrival k (+inf: not schedulable / unreachable) */
-  uint32_t* arr_fin;    /* number of arrivals j < k whose xfer_done instant is finite */
+  uint32_t* arr_fin;    /* number of arrivals j < k whose xfer_done instant lies at or before end_time (can be listed) */
   /* merged event list, replica-major SoA: entry p of replica r at [r * 2 * cap_arr + p] (see ML_*) */
   double* ml_t;
   double* ml_aux;
@@ -1108,11 +1108,13 @@ struct dcsim_merge_ring_t {
 /* List positions of arrival k (pos_a) and of its xfer_done (pos_x, when `xin`): the number of list events before each.
  * CHECKED = false: every index the scans touch is known to be in the ring (the common case, decided once per chunk);
  * CHECKED = true: indices below `lo` are read from HBM.  `thr_gap` = max_transfer plus a margin far above any rounding:
- * an arrival earlier than (t - thr_gap) has its xfer_done — if it has one — before t, and so have all before it. */
+ * an arrival earlier than (t - thr_gap) has its xfer_done — if it has one in the list — before t, and so have all before
+ * it.  Only transfers at or before `end` count: a longer one (a finite transfer_s of 1e300 or more, which max_transfer
+ * leaves out) is never in the list and never precedes a listed event. */
 template <bool CHECKED>
 DCSIM_DEV void dcsim_merge_positions(const dcsim_merge_ring_t* ring, const double* at, const double* tx, const uint32_t* fin,
                                      const uint32_t* pred, uint32_t lo, uint32_t n, uint32_t k, double tk, double txk, uint32_t pk,
-                                     double thr_gap, bool xin, uint32_t* pos_a, uint32_t* pos_x) {
+                                     double thr_gap, double end, bool xin, uint32_t* pos_a, uint32_t* pos_x) {
   const uint32_t RM = DCSIM_MERGE_RING - 1u;
 #define MR_AT(j) ((!CHECKED || (j) >= lo) ? ring->at[(j) & RM] : at[(j)])
 #define MR_TX(j) ((!CHECKED || (j) >= lo) ? ring->tx[(j) & RM] : tx[(j)])
@@ -1128,10 +1130,10 @@ DCSIM_DEV void dcsim_merge_positions(const dcsim_merge_ring_t* ring, const doubl
     --j;
     const double tj = MR_AT(j), txj = MR_TX(j);
     if (x_open) {
-      if (tj < far_x) { cx += MR_FIN(j) + (dcsim_finite(txj) ? 1u : 0u); x_open = false; }
+      if (tj < far_x) { cx += MR_FIN(j) + (txj > end ? 0u : 1u); x_open = false; }
       else if (txj <= txk) ++cx; /* tie: pushed earlier */
     }
-    if (tj < far_a) { cnt += MR_FIN(j) + (dcsim_finite(txj) ? 1u : 0u); break; } /* every finite one up to j is earlier */
+    if (tj < far_a) { cnt += MR_FIN(j) + (txj > end ? 0u : 1u); break; } /* every listed one up to j is earlier */
     if (txj < tk || (txj == tk && pk != DCSIM_NO_PRED && j <= pk)) ++cnt;
   }
   *pos_a = k + cnt;
@@ -1195,7 +1197,7 @@ DCSIM_DEV void dcsim_merge_arrivals(const dcsim_kparams_t* P, uint64_t r, int la
         if (!(meta & 0x100u)) size = dcsim_size_from_raw(sp, size, jt);
         tk = at[k];
         v = dcsim_test_quantize(tk + sp.transfer_s[ing][dc][jt]); /* SIM:580: now + transfer_s, now == the arrival instant */
-        f = dcsim_finite(v);
+        f = !(v > end); /* listable: counted in fin (+inf and anything past end_time are not) */
       }
       const uint32_t votes = dcsim_warp_ballot(f);
       if (k < n) {
@@ -1222,8 +1224,8 @@ DCSIM_DEV void dcsim_merge_arrivals(const dcsim_kparams_t* P, uint64_t r, int la
       const bool xs = dcsim_finite(txk) && !(txk > end_eps); /* SIM:160-163 */
       const bool xin = xs && !(txk > end);                    /* SIM:427: later events are never processed */
       uint32_t pos_a, pos_x;
-      if (covered) dcsim_merge_positions<false>(ring, at, tx, fin, pred, lo, n, k, tk, txk, pk, thr_gap, xin, &pos_a, &pos_x);
-      else dcsim_merge_positions<true>(ring, at, tx, fin, pred, lo, n, k, tk, txk, pk, thr_gap, xin, &pos_a, &pos_x);
+      if (covered) dcsim_merge_positions<false>(ring, at, tx, fin, pred, lo, n, k, tk, txk, pk, thr_gap, end, xin, &pos_a, &pos_x);
+      else dcsim_merge_positions<true>(ring, at, tx, fin, pred, lo, n, k, tk, txk, pk, thr_gap, end, xin, &pos_a, &pos_x);
       if (xin) { ++n_x; ahead = pos_x - pos_a > ahead ? pos_x - pos_a : ahead; }
       const uint32_t stream = meta & 15u;
       mt[pos_a] = tk;

@@ -8,3 +8,6 @@ g++ -O2 -fPIC -shared -std=gnu++17 -ffp-contract=off -fno-fast-math -Wall -Wno-u
 # the event-loop skeleton of the lane-group GPU builds (warp-uniform: replicas switched off, not broken out of the loop)
 g++ -O2 -fPIC -shared -std=gnu++17 -ffp-contract=off -fno-fast-math -Wall -Wno-unused-function -Wno-unknown-pragmas \
     -DDCSIM_HOST_UNIFORM_LOOP -o _build/libdcsim_hostemu_pair_uniform.so hostemu_pair.cpp -lm
+# the list merge with a ring of one chunk only: every scan that reaches back or ahead takes the HBM fall-back path
+g++ -O2 -fPIC -shared -std=gnu++17 -ffp-contract=off -fno-fast-math -Wall -Wno-unused-function -Wno-unknown-pragmas \
+    -DDCSIM_MERGE_RING=32u -o _build/libdcsim_hostemu_pair_smallring.so hostemu_pair.cpp -lm

@@ -2,8 +2,9 @@
  * TEST-ONLY.  Single-lane host build of distributed_cluster_gpus_b200/csrc/dcsim_core.cuh for the rule that lets
  * handles share one arrival pre-pass (dcsim_create_shared): dump the merged {arrival, xfer_done} lists a spec gives,
  * and run the event loop of one spec on the lists drawn under another.  It is not part of, linked into, or reachable
- * from the product library.  Built twice by build.sh: plain, and with DCSIM_HOST_UNIFORM_LOOP (the warp-uniform
- * event-loop skeleton of the lane-group GPU builds).
+ * from the product library.  Built three times by build.sh: plain, with DCSIM_HOST_UNIFORM_LOOP (the warp-uniform
+ * event-loop skeleton of the lane-group GPU builds), and with a merge ring of one chunk (DCSIM_MERGE_RING=32u: every
+ * scan that reaches back or ahead takes the HBM fall-back path).
  */
 #define DCSIM_HOST_EMU 1
 #include "../../distributed_cluster_gpus_b200/csrc/dcsim_core.cuh"
@@ -36,6 +37,7 @@ dcsim_kparams_t* make_params(const void* spec_blob, uint64_t n_replicas, uint64_
         const double v = P->spec.transfer_s[i][d][jt];
         if (v == v && v < 1e300 && v > P->max_transfer) P->max_transfer = v;
       }
+  P->max_transfer += dcsim_test_time_quantum; /* test hook: a rounded-up xfer_done instant may exceed t + transfer_s */
   const size_t ne = n_replicas * (size_t)P->cap_arr;
   P->arr_t = (double*)calloc(ne, sizeof(double));
   P->arr_raw = (double*)calloc(ne, sizeof(double));
@@ -48,6 +50,12 @@ dcsim_kparams_t* make_params(const void* spec_blob, uint64_t n_replicas, uint64_
   P->ml_meta = (uint32_t*)calloc(2 * ne, sizeof(uint32_t));
   P->arr_hdr = (dcsim_arrhdr_t*)calloc(n_replicas, sizeof(dcsim_arrhdr_t));
   if (rng_kind == 1) P->mt_state = (uint32_t*)calloc(n_replicas * (size_t)DCSIM_MT_N, sizeof(uint32_t));
+  /* an entry the pre-pass or the merge never wrote would show */
+  memset(P->arr_t, 0xee, ne * sizeof(double)); memset(P->arr_raw, 0xee, ne * sizeof(double));
+  memset(P->arr_meta, 0xee, ne * sizeof(uint32_t)); memset(P->arr_pred, 0xee, ne * sizeof(uint32_t));
+  memset(P->arr_tx, 0xee, ne * sizeof(double));
+  memset(P->ml_t, 0xee, 2 * ne * sizeof(double)); memset(P->ml_aux, 0xee, 2 * ne * sizeof(double));
+  memset(P->ml_meta, 0xee, 2 * ne * sizeof(uint32_t));
   return P;
 }
 
@@ -74,6 +82,8 @@ extern "C" {
 
 size_t hostemu_pair_sizeof_spec(void) { return sizeof(dcsim_spec_t); }
 size_t hostemu_pair_sizeof_arrhdr(void) { return sizeof(dcsim_arrhdr_t); }
+uint32_t hostemu_pair_merge_ring(void) { return DCSIM_MERGE_RING; }
+void hostemu_pair_set_test_time_quantum(double q) { dcsim_test_time_quantum = q; } /* see dcsim_core.cuh dcsim_test_quantize */
 
 /* dcsim_arrival_inputs_equal: 1 equal, 0 not (the first differing field's name into `field`, `field_bytes` long), -1 on
  * a malformed blob. */
@@ -96,6 +106,30 @@ int hostemu_pair_lists(const void* spec_blob, size_t spec_bytes, uint64_t n_repl
   memcpy(ml_t, P->ml_t, ne2 * sizeof(double));
   memcpy(ml_aux, P->ml_aux, ne2 * sizeof(double));
   memcpy(ml_meta, P->ml_meta, ne2 * sizeof(uint32_t));
+  memcpy(hdr, P->arr_hdr, n_replicas * sizeof(dcsim_arrhdr_t));
+  free_params(P);
+  return 0;
+}
+
+/* Everything the pre-pass and the merge leave for n replicas from keys seed0, seed0 + 1, ...: per replica cap_arr
+ * arrivals (arr_t, arr_raw as the merge leaves it: the job sizes, arr_meta, arr_pred, arr_tx: the xfer_done instants),
+ * 2 * cap_arr list entries (ml_t, ml_aux, ml_meta) and the header.  Rows past hdr[r].count / ml_count hold 0xee bytes.
+ * -1 on a bad blob. */
+int hostemu_pair_prepass(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, uint64_t seed0, int rng_kind,
+                         double* arr_t, double* arr_raw, uint32_t* arr_meta, uint32_t* arr_pred, double* arr_tx,
+                         double* ml_t, double* ml_aux, uint32_t* ml_meta, void* hdr) {
+  if (!spec_ok(spec_blob, spec_bytes)) return -1;
+  dcsim_kparams_t* P = make_params(spec_blob, n_replicas, seed0, 0, rng_kind);
+  draw_lists(P, rng_kind);
+  const size_t ne = n_replicas * (size_t)P->cap_arr;
+  memcpy(arr_t, P->arr_t, ne * sizeof(double));
+  memcpy(arr_raw, P->arr_raw, ne * sizeof(double));
+  memcpy(arr_meta, P->arr_meta, ne * sizeof(uint32_t));
+  memcpy(arr_pred, P->arr_pred, ne * sizeof(uint32_t));
+  memcpy(arr_tx, P->arr_tx, ne * sizeof(double));
+  memcpy(ml_t, P->ml_t, 2 * ne * sizeof(double));
+  memcpy(ml_aux, P->ml_aux, 2 * ne * sizeof(double));
+  memcpy(ml_meta, P->ml_meta, 2 * ne * sizeof(uint32_t));
   memcpy(hdr, P->arr_hdr, n_replicas * sizeof(dcsim_arrhdr_t));
   free_params(P);
   return 0;
