@@ -32,6 +32,8 @@ EXPORTS = (
     "dcsim_fetch_dc_wait_histogram",
     "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy", "dcsim_occupancy_moments",
     "dcsim_occupancy_spread",
+    "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs", "dcsim_tail_latency_moments",
+    "dcsim_tail_latency_spread",
 )
 
 _lib = None
@@ -156,6 +158,17 @@ def load():
         L.dcsim_occupancy_moments.argtypes = [vp, vp]
         L.dcsim_occupancy_spread.restype = i32
         L.dcsim_occupancy_spread.argtypes = [vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "dcsim_enable_tail_latency"):
+        L.dcsim_enable_tail_latency.restype = i32
+        L.dcsim_enable_tail_latency.argtypes = [vp, C.c_double]
+        L.dcsim_fetch_tail_latency.restype = i32
+        L.dcsim_fetch_tail_latency.argtypes = [vp, vp, C.c_size_t]
+        L.dcsim_fetch_tail_jobs.restype = i32
+        L.dcsim_fetch_tail_jobs.argtypes = [vp, u64, u64, vp, C.c_size_t]
+        L.dcsim_tail_latency_moments.restype = i32
+        L.dcsim_tail_latency_moments.argtypes = [vp, vp]
+        L.dcsim_tail_latency_spread.restype = i32
+        L.dcsim_tail_latency_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_power_profile"):
         L.dcsim_enable_power_profile.restype = i32
         L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]

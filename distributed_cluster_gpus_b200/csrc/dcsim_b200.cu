@@ -13,6 +13,8 @@
  *                             per-DC [n_dc][2][128] histograms of the job-log ensemble.
  *   dcsim_ens_*_kernel        the cluster-log and job-log ensembles (opt-in) and the paired comparison of two batches
  *                             with the same keys -> per-column moments, then spread + histograms.
+ *   dcsim_tail_select_kernel  one CTA per replica: the per-run tail-latency columns (opt-in) from the slot buffer, an
+ *                             exact multi-target radix select (dcsim_tail_select, dcsim_core.cuh).
  *
  * Handles of one group (dcsim_create_shared) share the pre-pass's buffers and the merged lists it leaves: the arrival
  * lists do not depend on the policy (dcsim_arrival_inputs_equal, dcsim_core.cuh).
@@ -81,6 +83,13 @@ __global__ void __launch_bounds__(DCSIM_MERGE_THREADS) dcsim_merge_kernel(const 
   const uint64_t r = (uint64_t)blockIdx.x * (DCSIM_MERGE_THREADS / 32) + (threadIdx.x >> 5);
   if (r >= P.n_replicas) return;
   dcsim_merge_arrivals(&P, r, (int)(threadIdx.x & 31u), &rings[threadIdx.x >> 5]);
+}
+
+/* Per-run tail latency: one CTA per replica (grid-stride), its scratch a constant 18 KB of shared memory. */
+#define DCSIM_TAIL_THREADS 256
+__global__ void __launch_bounds__(DCSIM_TAIL_THREADS) dcsim_tail_select_kernel(const __grid_constant__ dcsim_kparams_t P) {
+  __shared__ dcsim_tail_smem_t S;
+  for (uint64_t r = blockIdx.x; r < P.n_replicas; r += gridDim.x) dcsim_tail_select(&P, r, (int)threadIdx.x, (int)blockDim.x, &S);
 }
 
 /* Sums per-replica histogram rows of `row_len` counts: thread t of every block owns bins t, t + blockDim.x, ...
@@ -236,6 +245,29 @@ struct dcsim_ens_wait_src {
     return view{x, jobs, status, mean};
   }
   __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JWAIT_FIELDS == DCSIM_JWAIT_WAITED; }
+};
+
+/* Per-run tail latency: column c of the [DCSIM_TAIL_COLS(n_dc)][n] columns as stored.  A replica counts when its status
+ * is 0 and the value is not NaN (an empty group's statistics, SLA_MET without a job or an SLA).  JOBS, UNFINISHED and
+ * SLA_MET are the integer columns. */
+struct dcsim_ens_tail_src {
+  const double* cols;
+  const uint32_t* status;
+  uint64_t n;
+  uint32_t group_cols; /* 2 * (n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS: the SLA_MET columns follow */
+  struct view {
+    const double* x;
+    const uint32_t* status;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (status[r] != 0u) return false;
+      v = x[r];
+      return v == v;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const { return view{cols + col * n, status}; }
+  __device__ __forceinline__ bool integral(uint64_t col) const {
+    return col >= group_cols || col % DCSIM_TAIL_GROUP_FIELDS <= DCSIM_TAIL_UNFINISHED;
+  }
 };
 
 /* Paired comparison: column (metric, field) over replica r's summary rows of a base and a variant batch (the same keys).
@@ -517,6 +549,10 @@ struct dcsim {
   double pp_threshold;
   double* d_occ;           /* [1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n_replicas] occupancy (opt-in) */
   double* d_occ_work;      /* [n_replicas][n_dc][DCSIM_OCCW_N] its working state */
+  double* d_tail;          /* [n_replicas][cap_arr][2] per-run tail latency: (start, finish) per arrival slot (opt-in) */
+  double* d_tail_cols;     /* [DCSIM_TAIL_COLS(n_dc)][n_replicas] its columns */
+  double tail_sla;
+  int tail_fresh;          /* 1: the columns were selected from this batch's finished slots */
   double* d_jwait;         /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waiting / response times (opt-in) */
   uint32_t* d_jwait_hist;  /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] their per-DC histograms */
   unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_wait_histogram */
@@ -553,6 +589,11 @@ static uint64_t occ_cols(const dcsim_t* h) { return occ_stat_cols(h) + 2ull * DC
 static size_t occ_bytes(const dcsim_t* h) { return (size_t)(1 + occ_cols(h)) * (size_t)h->n_replicas * sizeof(double); }
 static size_t occ_work_bytes(const dcsim_t* h) {
   return (size_t)h->n_replicas * (size_t)h->spec.n_dc * DCSIM_OCCW_N * sizeof(double);
+}
+
+static size_t tail_slot_bytes(const dcsim_t* h) { return (size_t)h->n_replicas * (size_t)h->g->cap_arr * 2 * sizeof(double); }
+static size_t tail_cols_bytes(const dcsim_t* h) {
+  return (size_t)DCSIM_TAIL_COLS(h->spec.n_dc) * (size_t)h->n_replicas * sizeof(double);
 }
 
 static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", long long b = 0) {
@@ -770,11 +811,11 @@ static cudaError_t size_launch(dcsim_t* h) {
   return cudaSuccess;
 }
 
-/* job_log.csv needs size / f / jid in the running records, the waiting-time recorder the jid; switching them on or off
- * re-lays the state block out. */
+/* job_log.csv needs size / f / jid in the running records, the waiting-time and tail-latency recorders the jid;
+ * switching them on or off re-lays the state block out. */
 static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
-  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL);
+  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL || h->d_tail != NULL);
   if (L.lean == h->L.lean) return DCSIM_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
@@ -974,6 +1015,8 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, (h->jens_windows + 1) * jwait_row_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
   }
+  if (h->d_tail) CUDA_TRY(h, cudaMemsetAsync(h->d_tail, 0xff, tail_slot_bytes(h), h->g->stream)); /* NaN: not finished */
+  h->tail_fresh = 0;
   if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
     h->g->seed0 = base_seed + first_replica_id;
     h->g->arrivals_ready = 0;
@@ -1053,7 +1096,8 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->mt_state = h->g->d_mt;
   P->ens = h->d_ens; P->ens_cap = h->ens_cap;
   P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
-  P->finish_rec = (P->lat_hist || P->jens) ? 1u : 0u;
+  P->tail = h->d_tail; P->tail_cols = h->d_tail_cols; P->tail_sla = h->tail_sla;
+  P->finish_rec = (P->lat_hist || P->jens || P->tail) ? 1u : 0u;
   P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
   P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
   P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
@@ -1163,6 +1207,7 @@ int dcsim_advance(dcsim_t* h, uint64_t max_events_per_replica, uint64_t* total_e
   fill_kparams(h, &P, max_events_per_replica);
   CUDA_TRY(h, adv_launch_for(h->lanes)(&P, h->d_events, h->L.cap_stale != 0, h->mode, h->ctas, h->warps_per_cta * 32, h->smem_bytes, h->g->stream));
   h->launches++;
+  h->tail_fresh = 0;
   if (total_events_out) {
     unsigned long long total = 0;
     CUDA_TRY(h, cudaMemcpyAsync(&total, h->d_events, sizeof(total), cudaMemcpyDeviceToHost, h->g->stream));
@@ -1588,6 +1633,88 @@ int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double*
   return ens_spread(h, src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
+int dcsim_enable_tail_latency(dcsim_t* h, double sla_s) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!(sla_s >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_tail_latency: sla_s must be >= 0 (+inf: none)%s%lld");
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_tail_latency on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_tail_latency must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  if (!h->d_tail) {
+    const int rc = recorder_alloc(h, (void**)&h->d_tail, tail_slot_bytes(h), (void**)&h->d_tail_cols, tail_cols_bytes(h),
+                                  "enable_tail_latency: %s%lld bytes of device memory do not fit (run fewer replicas)",
+                                  (long long)(tail_slot_bytes(h) + tail_cols_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->d_tail, 0xff, tail_slot_bytes(h), h->g->stream)); /* NaN: not finished */
+  h->tail_sla = sla_s;
+  h->tail_fresh = 0;
+  return DCSIM_OK;
+}
+
+/* The tail columns of the finished batch, selected once per batch on the stream (see dcsim_fetch_tail_latency). */
+static int tail_ready(dcsim_t* h) {
+  int rc = recorder_ready(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
+  if (rc != DCSIM_OK || h->tail_fresh) return rc;
+  int done = 0;
+  if ((rc = dcsim_all_done(h, &done)) != DCSIM_OK) return rc;
+  if (!done) return set_err(h, DCSIM_E_STATE, "tail latency read while replicas are still running (advance to the end first)%s%lld");
+  dcsim_kparams_t P;
+  fill_kparams(h, &P, 0);
+  const uint64_t per_sm = 8; /* 256 threads and 18 KB each: 8 CTAs fit an SM */
+  const uint64_t grid = h->n_replicas < per_sm * (uint64_t)h->sm_count ? h->n_replicas : per_sm * (uint64_t)h->sm_count;
+  dcsim_tail_select_kernel<<<(int)grid, DCSIM_TAIL_THREADS, 0, h->g->stream>>>(P);
+  CUDA_TRY(h, cudaGetLastError());
+  h->tail_fresh = 1;
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_tail_latency(dcsim_t* h, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  if (out_bytes < tail_cols_bytes(h))
+    return set_err(h, DCSIM_E_INVALID, "fetch_tail_latency: buffer too small (need %s%lld bytes)", "", (long long)tail_cols_bytes(h));
+  const int rc = tail_ready(h);
+  if (rc != DCSIM_OK) return rc;
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_tail_cols, tail_cols_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  if (first > h->n_replicas || count > h->n_replicas - first)
+    return set_err(h, DCSIM_E_INVALID, "fetch_tail_jobs: replicas [first, first + count) out of range%s%lld");
+  const int rc = recorder_ready(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
+  if (rc != DCSIM_OK) return rc;
+  const size_t per = (size_t)h->g->cap_arr * 2, need = (size_t)count * per * sizeof(double);
+  if (out_bytes < need)
+    return set_err(h, DCSIM_E_INVALID, "fetch_tail_jobs: buffer too small (need %s%lld bytes)", "", (long long)need);
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_tail + (size_t)first * per, need, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_tail_latency_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  int rc = tail_ready(h);
+  if (rc == DCSIM_OK) rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t group_cols = 2u * (uint32_t)(h->spec.n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
+  const dcsim_ens_tail_src src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols};
+  return ens_moments(h, src, h->n_replicas, DCSIM_TAIL_COLS(h->spec.n_dc), dev_out);
+}
+
+int dcsim_tail_latency_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                              double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  int rc = tail_ready(h);
+  if (rc == DCSIM_OK) rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
+  if (rc != DCSIM_OK) return rc;
+  const uint32_t group_cols = 2u * (uint32_t)(h->spec.n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
+  const dcsim_ens_tail_src src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols};
+  return ens_spread(h, src, h->n_replicas, DCSIM_TAIL_COLS(h->spec.n_dc), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
+}
+
 int dcsim_enable_occupancy(dcsim_t* h) {
   if (!h) return DCSIM_E_INVALID;
   if (h->member) return set_err(h, DCSIM_E_STATE, "enable_occupancy on a member of a shared group%s%lld");
@@ -1710,6 +1837,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
   cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
   cudaFree(h->d_occ); cudaFree(h->d_occ_work);
+  cudaFree(h->d_tail); cudaFree(h->d_tail_cols);
   cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;

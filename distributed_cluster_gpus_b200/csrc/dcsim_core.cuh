@@ -490,6 +490,10 @@ struct dcsim_kparams_t {
   uint32_t* jwait_hist; /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] per-DC wait / response histograms (with jwait) */
   double* occ;          /* [1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n_replicas] occupancy, or NULL */
   double* occ_work;     /* [n_replicas][n_dc][DCSIM_OCCW_N] its working state (with occ) */
+  double* tail;         /* [n_replicas][cap_arr][2] (start, finish) of each arrival slot's job, NaN until it finishes
+                           (needs L.lean == 0), or NULL */
+  double* tail_cols;    /* [DCSIM_TAIL_COLS(n_dc)][n_replicas] the per-run tail columns (dcsim_tail_select writes them) */
+  double tail_sla;      /* [s], +inf: none */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -508,6 +512,7 @@ struct dcsim_ctx_t {
   bool pp;               /* the power-profile recorder runs: a compile-time false in the instantiations without the
                             profile recorders (dcsim_replica_step<..., PP>), so their code does not change */
   bool occ;              /* the occupancy recorder runs: likewise */
+  bool tail;             /* the tail-latency recorder runs: likewise */
   bool quiet;            /* a ghost lane group of an in-place launch, whose blk is replica n-1's live block in HBM: it must
                             not even publish the pop-min cache there.  A compile-time false in the staged and head-staged
                             instantiations (a ghost's blk is its own shared-memory slot there) */
@@ -1983,6 +1988,17 @@ DCSIM_COLD void dcsim_jwait_add(const dcsim_kparams_t* P, uint32_t r, int d, int
 #endif
 }
 
+/* Per-run tail latency (opt-in: P->tail): the job of running record i (at `rec`, the base of the L.rn_* offsets) finished
+ * at `now`; its start and finish go to the slot of its arrival (jid - 1), which nothing else writes.  The job's DC, type,
+ * arrival and xfer_done instants are read by the selection pass from the pre-pass's and the merge's buffers (arr_meta,
+ * arr_t, arr_tx: written once before the event loop, read-only since). */
+DCSIM_COLD void dcsim_tail_add(const dcsim_kparams_t* P, uint32_t r, double now, char* rec, int i) {
+  const uint32_t jid = dcsim_at<uint32_t>(rec, P->L.rn_jid)[i];
+  double* slot = P->tail + 2ull * ((uint64_t)r * (uint64_t)P->cap_arr + (uint64_t)(jid - 1u));
+  slot[0] = dcsim_at<double>(rec, P->L.rn_start)[i];
+  slot[1] = now;
+}
+
 /* SIM:701-927 minus RL/elastic branches (lane 0 part, after the record was read and before it is erased). */
 DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const dcsim_spec_t& sp = c.P->spec;
@@ -1999,13 +2015,14 @@ DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   H->lat_sum += lat;
   if (jt == DCSIM_JT_INFERENCE) { H->lat_sum_inf += lat; H->n_fin_inf++; } else { H->lat_sum_trn += lat; H->n_fin_trn++; }
 #ifdef DCSIM_HOST_EMU
-  if (c.P->lat_hist || c.P->jens) { /* (the host builds set the pointers only) */
+  if (c.P->lat_hist || c.P->jens || c.P->tail) { /* (the host builds set the pointers only) */
 #else
   if (__builtin_expect(c.P->finish_rec != 0u, 0)) { /* opt-in recorders: off, they cost this one test */
 #endif
     if (c.P->lat_hist) dcsim_hist_add(c.P->lat_hist, (uint64_t)c.r, jt, lat);
     if (c.P->jens) dcsim_jens_add(c.P, c.r, d, jt, now, lat);
     if (c.P->jwait) dcsim_jwait_add(c.P, c.r, d, jt, now, c.rec, i); /* (only with jens, in the layout keeping the jid) */
+    if (c.tail) dcsim_tail_add(c.P, c.r, now, c.rec, i);               /* (in the layout keeping the jid) */
   }
   if (L.lean == 0) { /* the readers of a finished job's size / f / jid: job_log.csv and the bandit's reward */
     const double f_used = dcsim_at<double>(c.rec, L.rn_f)[i];
@@ -2696,6 +2713,7 @@ DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char
   c.is_logged = !ghost && ((int64_t)r == P->rec.log_replica);
   c.pp = PP && !ghost && P->pp != nullptr;
   c.occ = PP && !ghost && P->occ != nullptr;
+  c.tail = PP && !ghost && P->tail != nullptr;
   c.quiet = INPLACE && ghost;
   if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing to a
                   replica's state (staged modes: its own shared-memory slot takes the pop-min cache; in place: quiet) */
@@ -2722,4 +2740,178 @@ DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char
   dcsim_write_summary(c, P->summary + r * DCSIM_SUMMARY_K);
   dcsim_warp_sync();
   return n;
+}
+
+/* ---- per-run tail latency: the selection pass ---------------------------------------------------------------------
+ * One CTA per replica (dcsim_tail_select_kernel, grid-stride; the host builds: one thread) turns the replica's slot
+ * buffer (P->tail) into its DCSIM_TAIL_* columns, exactly: every order statistic is one job's value, bit for bit.
+ *
+ * A multi-target radix select over order-preserving 64-bit keys of the values (dcsim_tail_key).  A target is one (group,
+ * kind, quantile) with its rank k; per group a job enters 3 kinds x 4 quantiles, and a job is in two groups (its type over
+ * all DCs, its type in its DC).  The first read over the replica's created slots counts JOBS and UNFINISHED and takes
+ * every (group, kind)'s smallest and largest key; the bits above their highest differing bit are shared by every value of
+ * the (group, kind) and give its targets' first key bits.  Each further read settles one 4-bit digit of every target
+ * whose next undetermined digit it is: per-target digit histograms in shared memory, counted over the values that agree
+ * with the target's settled bits, then the digit where the running count reaches k.  At most 16 digit reads; the
+ * scratch is a constant (dcsim_tail_smem_t, 18 KB at DCSIM_MAX_DC = 8) whatever cap_arr, and no value is copied.
+ * Counts are integer atomics, so the result does not depend on thread scheduling. */
+#define DCSIM_TAIL_GROUPS_MAX (2 * (DCSIM_MAX_DC + 1))
+#define DCSIM_TAIL_TARGETS_MAX (DCSIM_TAIL_GROUPS_MAX * DCSIM_TAIL_KINDS * DCSIM_TAIL_QUANTILES)
+#define DCSIM_TAIL_RADIX 16
+struct dcsim_tail_smem_t {
+  uint32_t hist[DCSIM_TAIL_TARGETS_MAX][DCSIM_TAIL_RADIX]; /* digit counts of the pass */
+  unsigned long long key[DCSIM_TAIL_TARGETS_MAX];          /* the settled high bits (the rest 0) */
+  unsigned long long lo[DCSIM_TAIL_GROUPS_MAX * DCSIM_TAIL_KINDS], hi[DCSIM_TAIL_GROUPS_MAX * DCSIM_TAIL_KINDS];
+  uint32_t rank[DCSIM_TAIL_TARGETS_MAX];                   /* k among the values that agree with `key` */
+  uint32_t low[DCSIM_TAIL_TARGETS_MAX];                    /* low bits not settled yet (a multiple of 4; 0: done) */
+  uint32_t jobs[DCSIM_TAIL_GROUPS_MAX], unfinished[DCSIM_TAIL_GROUPS_MAX];
+};
+
+#ifdef DCSIM_HOST_EMU
+static inline void dcsim_tail_sync() {}
+static inline void dcsim_tail_add_u32(uint32_t* a, uint32_t v) { *a += v; }
+static inline void dcsim_tail_min_u64(unsigned long long* a, unsigned long long v) { if (v < *a) *a = v; }
+static inline void dcsim_tail_max_u64(unsigned long long* a, unsigned long long v) { if (v > *a) *a = v; }
+static inline unsigned long long dcsim_tail_bits(double x) { unsigned long long u; memcpy(&u, &x, 8); return u; }
+static inline double dcsim_tail_double(unsigned long long u) { double x; memcpy(&x, &u, 8); return x; }
+static inline int dcsim_tail_clz64(unsigned long long x) { return __builtin_clzll(x); }
+#else
+__device__ __forceinline__ void dcsim_tail_sync() { __syncthreads(); }
+__device__ __forceinline__ void dcsim_tail_add_u32(uint32_t* a, uint32_t v) { atomicAdd(a, v); }
+__device__ __forceinline__ void dcsim_tail_min_u64(unsigned long long* a, unsigned long long v) { atomicMin(a, v); }
+__device__ __forceinline__ void dcsim_tail_max_u64(unsigned long long* a, unsigned long long v) { atomicMax(a, v); }
+__device__ __forceinline__ unsigned long long dcsim_tail_bits(double x) { return (unsigned long long)__double_as_longlong(x); }
+__device__ __forceinline__ double dcsim_tail_double(unsigned long long u) { return __longlong_as_double((long long)u); }
+__device__ __forceinline__ int dcsim_tail_clz64(unsigned long long x) { return __clzll((long long)x); }
+#endif
+
+/* Keys that order like the values (IEEE patterns with the sign folded in), and back. */
+DCSIM_DEV unsigned long long dcsim_tail_key(double v) {
+  const unsigned long long b = dcsim_tail_bits(v);
+  return (b >> 63) ? ~b : (b | 0x8000000000000000ull);
+}
+DCSIM_DEV double dcsim_tail_value(unsigned long long k) {
+  return dcsim_tail_double((k >> 63) ? (k & 0x7fffffffffffffffull) : ~k);
+}
+/* a and b agree above bit `sh` (everything agrees above bit 63) */
+DCSIM_DEV bool dcsim_tail_same_above(unsigned long long a, unsigned long long b, uint32_t sh) {
+  return sh >= 64u || (a >> sh) == (b >> sh);
+}
+
+/* Job k of replica r's created slots: false while unfinished; else its (all-DC, own-DC) groups and the keys of its
+ * latency, wait and response (the f64 subtractions of include/dcsim_b200.h). */
+DCSIM_DEV bool dcsim_tail_job(const dcsim_kparams_t* P, uint64_t base, uint32_t k, int* g0, int* g1,
+                              unsigned long long v[DCSIM_TAIL_KINDS]) {
+  const uint32_t meta = P->arr_meta[base + k];
+  const int jt = (int)(meta & 1u), dc = (int)((meta >> 4) & 7u);
+  *g0 = jt * (P->spec.n_dc + 1);
+  *g1 = *g0 + 1 + dc;
+  const double start = P->tail[2 * (base + k)], finish = P->tail[2 * (base + k) + 1];
+  if (finish != finish) return false;
+  v[DCSIM_TAIL_LATENCY] = dcsim_tail_key(finish - start);
+  v[DCSIM_TAIL_WAIT] = dcsim_tail_key(start - P->arr_tx[base + k]);
+  v[DCSIM_TAIL_RESPONSE] = dcsim_tail_key(finish - P->arr_t[base + k]);
+  return true;
+}
+
+/* Replica r's columns (thread `tid` of `nt`; every thread of the CTA calls it with the same r). */
+DCSIM_DEV void dcsim_tail_select(const dcsim_kparams_t* P, uint64_t r, int tid, int nt, dcsim_tail_smem_t* S) {
+  const int D = P->spec.n_dc, G = 2 * (D + 1), T = G * DCSIM_TAIL_KINDS * DCSIM_TAIL_QUANTILES;
+  const uint64_t n = P->n_replicas;
+  double* out = P->tail_cols + r;
+  const double* summ = P->summary + r * DCSIM_SUMMARY_K;
+  const double nan = dcsim_tail_double(0x7ff8000000000000ull);
+  dcsim_tail_sync(); /* the previous replica's readers of S are done */
+  if (summ[DCSIM_S_STATUS] != 0.0) {
+    for (int c = tid; c < DCSIM_TAIL_COLS(D); c += nt) out[(uint64_t)c * n] = nan;
+    return;
+  }
+  const uint32_t created = (uint32_t)summ[DCSIM_S_JOBS_CREATED];
+  const uint64_t base = r * (uint64_t)P->cap_arr;
+  for (int i = tid; i < G; i += nt) { S->jobs[i] = 0u; S->unfinished[i] = 0u; }
+  for (int i = tid; i < G * DCSIM_TAIL_KINDS; i += nt) { S->lo[i] = ~0ull; S->hi[i] = 0ull; }
+  for (int i = tid; i < T * DCSIM_TAIL_RADIX; i += nt) (&S->hist[0][0])[i] = 0u;
+  dcsim_tail_sync();
+  for (uint32_t k = (uint32_t)tid; k < created; k += (uint32_t)nt) { /* read 0: counts and key ranges */
+    int g[2];
+    unsigned long long v[DCSIM_TAIL_KINDS];
+    if (!dcsim_tail_job(P, base, k, &g[0], &g[1], v)) {
+      dcsim_tail_add_u32(&S->unfinished[g[0]], 1u); dcsim_tail_add_u32(&S->unfinished[g[1]], 1u);
+      continue;
+    }
+    for (int j = 0; j < 2; ++j) {
+      dcsim_tail_add_u32(&S->jobs[g[j]], 1u);
+      for (int c = 0; c < DCSIM_TAIL_KINDS; ++c) {
+        dcsim_tail_min_u64(&S->lo[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
+        dcsim_tail_max_u64(&S->hi[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
+      }
+    }
+  }
+  dcsim_tail_sync();
+  for (int t = tid; t < T; t += nt) { /* targets: rank and the bits every value of the (group, kind) shares */
+    const int g = t / (DCSIM_TAIL_KINDS * DCSIM_TAIL_QUANTILES), gk = t / DCSIM_TAIL_QUANTILES;
+    const uint32_t m = S->jobs[g];
+    S->low[t] = 0u; S->key[t] = 0ull; S->rank[t] = 0u;
+    if (!m) continue;
+    const int q = t % DCSIM_TAIL_QUANTILES;
+    const double qv = q == DCSIM_TAIL_P50 ? 0.5 : q == DCSIM_TAIL_P95 ? 0.95 : q == DCSIM_TAIL_P99 ? 0.99 : 0.999;
+    const double kf = ceil((double)m * qv);
+    S->rank[t] = kf < 1.0 ? 1u : (uint32_t)kf;
+    const unsigned long long a = S->lo[gk], x = a ^ S->hi[gk];
+    const uint32_t nb = x ? ((uint32_t)(64 - dcsim_tail_clz64(x)) + 3u) & ~3u : 0u;
+    S->low[t] = nb;
+    S->key[t] = nb >= 64u ? 0ull : (a >> nb) << nb;
+  }
+  dcsim_tail_sync();
+  uint32_t top = 0u;
+  for (int t = 0; t < T; ++t) top = S->low[t] > top ? S->low[t] : top;
+  for (int s = (int)top - 4; s >= 0; s -= 4) { /* one read per digit */
+    const uint32_t above = (uint32_t)s + 4u;
+    for (uint32_t k = (uint32_t)tid; k < created; k += (uint32_t)nt) {
+      int g[2];
+      unsigned long long v[DCSIM_TAIL_KINDS];
+      if (!dcsim_tail_job(P, base, k, &g[0], &g[1], v)) continue;
+      for (int j = 0; j < 2; ++j)
+        for (int c = 0; c < DCSIM_TAIL_KINDS; ++c) {
+          const int t0 = (g[j] * DCSIM_TAIL_KINDS + c) * DCSIM_TAIL_QUANTILES;
+          const uint32_t digit = (uint32_t)(v[c] >> s) & (DCSIM_TAIL_RADIX - 1u);
+          for (int q = 0; q < DCSIM_TAIL_QUANTILES; ++q)
+            if (S->low[t0 + q] == above && dcsim_tail_same_above(v[c], S->key[t0 + q], above))
+              dcsim_tail_add_u32(&S->hist[t0 + q][digit], 1u);
+        }
+    }
+    dcsim_tail_sync();
+    for (int t = tid; t < T; t += nt) {
+      if (S->low[t] != above) continue;
+      uint32_t below = 0u;
+      for (uint32_t d = 0; d < DCSIM_TAIL_RADIX; ++d) {
+        const uint32_t c = S->hist[t][d];
+        if (below + c >= S->rank[t]) { S->key[t] |= (unsigned long long)d << s; S->rank[t] -= below; break; }
+        below += c;
+      }
+      for (uint32_t d = 0; d < DCSIM_TAIL_RADIX; ++d) S->hist[t][d] = 0u;
+      S->low[t] = (uint32_t)s;
+    }
+    dcsim_tail_sync();
+  }
+  for (int t = tid; t < T; t += nt) {
+    const int g = t / (DCSIM_TAIL_KINDS * DCSIM_TAIL_QUANTILES), c = (t / DCSIM_TAIL_QUANTILES) % DCSIM_TAIL_KINDS;
+    const int col = g * DCSIM_TAIL_GROUP_FIELDS + DCSIM_TAIL_STAT(c, t % DCSIM_TAIL_QUANTILES);
+    out[(uint64_t)col * n] = S->jobs[g] ? dcsim_tail_value(S->key[t]) : nan;
+  }
+  for (int i = tid; i < G * DCSIM_TAIL_KINDS; i += nt) {
+    const int g = i / DCSIM_TAIL_KINDS;
+    out[(uint64_t)(g * DCSIM_TAIL_GROUP_FIELDS + DCSIM_TAIL_STAT(i % DCSIM_TAIL_KINDS, DCSIM_TAIL_MAX)) * n] =
+        S->jobs[g] ? dcsim_tail_value(S->hi[i]) : nan;
+  }
+  for (int g = tid; g < G; g += nt) {
+    out[(uint64_t)(g * DCSIM_TAIL_GROUP_FIELDS + DCSIM_TAIL_JOBS) * n] = (double)S->jobs[g];
+    out[(uint64_t)(g * DCSIM_TAIL_GROUP_FIELDS + DCSIM_TAIL_UNFINISHED) * n] = (double)S->unfinished[g];
+  }
+  for (int i = tid; i < 2 * DCSIM_TAIL_KINDS; i += nt) { /* SLA_MET (kind, jt): the all-DC group's P99 */
+    const int c = i / 2, g = (i % 2) * (D + 1);
+    const int t = (g * DCSIM_TAIL_KINDS + c) * DCSIM_TAIL_QUANTILES + DCSIM_TAIL_P99;
+    const bool none = !S->jobs[g] || !(P->tail_sla < DCSIM_INF);
+    out[(uint64_t)(G * DCSIM_TAIL_GROUP_FIELDS + i) * n] = none ? nan : (dcsim_tail_value(S->key[t]) <= P->tail_sla ? 1.0 : 0.0);
+  }
 }

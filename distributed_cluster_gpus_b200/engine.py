@@ -393,6 +393,52 @@ class BatchedEngine:
         N.check(self._lib.dcsim_occupancy_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
                                                  C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
+    # -- per-run tail latency (ensemble.tail_latency turns it into batch statistics) ----------------------------------
+    def enable_tail_latency(self, sla_s=None):
+        """Opt-in, before the first advance of a batch (stays on across reset, cleared by it): every finished job's start
+        and finish instants are kept per arrival slot, and once the batch is done a selection pass turns them into each
+        replica's exact p50 / p95 / p99 / p99.9 / max of service, wait and response time per (job type, scope), and
+        whether its p99 met ``sla_s`` seconds (None: no SLA) — include/dcsim_b200.h DCSIM_TAIL_*.  The running records
+        then carry the job id."""
+        N.check(self._lib.dcsim_enable_tail_latency(self._h, float("inf") if sla_s is None else float(sla_s)), self._h)
+        self._tail_sla = None if sla_s is None else float(sla_s)
+        self._tail_on = True
+
+    @property
+    def tail_latency_enabled(self) -> bool:
+        return getattr(self, "_tail_on", False)
+
+    @property
+    def tail_latency_sla(self):
+        """The SLA [s] of the enabled recorder (None: none)."""
+        return getattr(self, "_tail_sla", None)
+
+    def tail_latency_rows(self) -> np.ndarray:
+        """[S.tail_cols(n_dc), n_replicas] float64: every replica's columns (NaN: does not count).  Runs the selection
+        pass first if the batch has not had it yet.  For tests and small batches."""
+        rows = np.empty((S.tail_cols(self.spec.n_dc), self.n_replicas), dtype=np.float64)
+        N.check(self._lib.dcsim_fetch_tail_latency(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
+        return rows
+
+    def tail_latency_jobs(self, first: int = 0, count=None) -> np.ndarray:
+        """[count, cap_arrivals, 2] float64: the raw slot buffer of local replicas [first, first + count) (None: to the
+        last) — (start, finish) of the job of every arrival slot (jid - 1), NaN while it has not finished.  For tests."""
+        cap = self.spec.cap_arrivals if self.spec.cap_arrivals > 0 else 16384
+        count = self.n_replicas - first if count is None else int(count)
+        out = np.empty((count, cap, 2), dtype=np.float64)
+        N.check(self._lib.dcsim_fetch_tail_jobs(self._h, int(first), count, C.c_void_p(out.ctypes.data), out.nbytes),
+                self._h)
+        return out
+
+    def tail_latency_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][S.tail_cols(n_dc)] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_tail_latency_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def tail_latency_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_tail_latency_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                    C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
     # -- paired reductions (compare.py) ------------------------------------------------------------------------------
     def paired_moments_into(self, variant_summary_ptr: int, device_ptr: int):
         """Pass 1 on this (base) handle's stream against a variant's [n_replicas, SUMMARY_K] summaries on the device:
@@ -514,11 +560,16 @@ def _pp_key(power_profile, power_threshold):
 
 
 def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False,
-               occupancy=False):
+               occupancy=False, tail=None):
     # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
             os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None),
-            bool(occupancy))
+            bool(occupancy), tail)
+
+
+def _tail_key(tail_latency, tail_sla_s):
+    """The tail-latency recorder's SLA as the engine cache sees it: None when the recorder is off, +inf for no SLA."""
+    return (float("inf") if tail_sla_s is None else float(tail_sla_s)) if tail_latency else None
 
 
 def _drop_parked_batch_engine():
@@ -529,15 +580,16 @@ def _drop_parked_batch_engine():
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
                    job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                   occupancy=False):
+                   occupancy=False, tail_latency=False, tail_sla_s=None):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
     ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
     power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
-    response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on.  A parked
+    response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on;
+    ``tail_latency``: with the per-run tail-latency recorder on, SLA ``tail_sla_s`` seconds (None: none).  A parked
     engine is only reused by a caller that asks for the same recorders."""
     job_bin = _job_bin(sp, job_ensemble or job_waits, job_ensemble_bin)
     key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
-                     job_waits, occupancy)
+                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s))
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -558,6 +610,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_power_profile(power_threshold)
         if occupancy:
             eng.enable_occupancy()
+        if tail_latency:
+            eng.enable_tail_latency(tail_sla_s)
     except BaseException:
         eng.close()
         raise
@@ -572,7 +626,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
                                                         eng.job_ensemble_bin,
                                                         _pp_key(eng.power_profile_enabled, eng.power_threshold),
-                                                        eng.job_waits_enabled, eng.occupancy_enabled)
+                                                        eng.job_waits_enabled, eng.occupancy_enabled,
+                                                        _tail_key(eng.tail_latency_enabled, eng.tail_latency_sla))
 
 
 def free_cached_engine():
@@ -622,7 +677,7 @@ class LoggedReplica:
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
                       job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                      occupancy=False):
+                      occupancy=False, tail_latency=False, tail_sla_s=None):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
@@ -630,12 +685,14 @@ def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, d
     ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
     window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
     None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble);
-    ``occupancy``: with the occupancy recorder on."""
+    ``occupancy``: with the occupancy recorder on; ``tail_latency``: with the per-run tail-latency recorder on
+    (``tail_sla_s``: its SLA [s], None = none), its slot buffer sized by each attempt's cap_arrivals."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
-                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy)
+                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy,
+                             tail_latency, tail_sla_s)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

@@ -947,3 +947,194 @@ def occupancy_from_rows(rows: np.ndarray, summary: np.ndarray, widths, quantiles
     n_dc = len(widths)
     passes = host_passes(x, ok, _occ_integral(n_dc), len(OCC_STATS) * n_dc)
     return occ_finalize(*passes, n_dc, widths, quantiles)
+
+
+# ---- per-run tail latency --------------------------------------------------------------------------------------------
+# per replica and group (job type, scope) the columns TAIL_FIELDS, then per (kind, job type) SLA_MET (DCSIM_TAIL_*)
+TAIL_KINDS = ("latency", "wait", "response")
+TAIL_STATS = ("p50", "p95", "p99", "p999", "max")
+TAIL_QUANTILES = (0.5, 0.95, 0.99, 0.999)              # the order statistics p50 .. p999
+TAIL_FIELDS = ("jobs", "unfinished") + tuple(f"{k}_{s}_s" for k in TAIL_KINDS for s in TAIL_STATS)
+TAIL_TYPES = ("inference", "training")                 # DCSIM_JT_* order
+TAIL_CSV_HEADER = ["type"] + PP_CSV_HEADER
+# one created job of a replica, as the tail-latency mirror takes it (finish NaN: not finished by end_time)
+TAIL_JOB_DTYPE = np.dtype([("jtype", "<i4"), ("dc", "<i4"), ("arrival", "<f8"), ("xfer_done", "<f8"), ("start", "<f8"),
+                           ("finish", "<f8")])
+
+
+def _tail_columns(n_dc: int):
+    """(type, dc, field) of every column in the kernels' order; dc = -1: all DCs."""
+    cols = [(TAIL_TYPES[jt], dc, f) for jt in range(2) for dc in range(-1, n_dc) for f in TAIL_FIELDS]
+    return tuple(cols + [(TAIL_TYPES[jt], -1, f"{k}_sla_met") for k in TAIL_KINDS for jt in range(2)])
+
+
+def _tail_integral(n_dc: int) -> np.ndarray:
+    cols = _tail_columns(n_dc)
+    return np.array([f in ("jobs", "unfinished") or f.endswith("_sla_met") for _, _, f in cols])
+
+
+def order_statistic(values: np.ndarray, q: float) -> float:
+    """The q-quantile as the per-run tail columns define it: numpy's ``inverted_cdf``, the k-th smallest value with
+    k = max(ceil(n * q), 1)."""
+    return float(np.quantile(np.asarray(values, dtype=np.float64), q, method="inverted_cdf"))
+
+
+def tail_rows_from_jobs(jobs: Sequence[np.ndarray], status, n_dc: int, sla_s=None) -> np.ndarray:
+    """numpy mirror of the selection pass: per replica its created jobs (TAIL_JOB_DTYPE) and its status word ->
+    [tail columns, R] float64 (BatchedEngine.tail_latency_rows).  Values are the f64 subtractions of the device; NaN
+    where a column does not count."""
+    from . import spec as S
+    R = len(jobs)
+    sla = math.inf if sla_s is None else float(sla_s)
+    out = np.full((S.tail_cols(n_dc), R), np.nan)
+    for r in range(R):
+        if int(status[r]) != 0:
+            continue
+        j = np.asarray(jobs[r])
+        fin = ~np.isnan(j["finish"])
+        vals = (j["finish"] - j["start"], j["start"] - j["xfer_done"], j["finish"] - j["arrival"])
+        for jt in range(2):
+            for dc in range(-1, n_dc):
+                sel = (j["jtype"] == jt) & ((j["dc"] == dc) if dc >= 0 else True)
+                c0 = S.tail_col(n_dc, jt, 0, dc)
+                out[c0 + S.TAIL_JOBS, r] = np.count_nonzero(sel & fin)
+                out[c0 + S.TAIL_UNFINISHED, r] = np.count_nonzero(sel & ~fin)
+                if not np.any(sel & fin):
+                    continue
+                for k, v in enumerate(vals):
+                    x = v[sel & fin]
+                    base = c0 + S.TAIL_STATS_BASE + k * len(TAIL_STATS)
+                    for i, q in enumerate(TAIL_QUANTILES):
+                        out[base + i, r] = order_statistic(x, q)
+                    out[base + len(TAIL_QUANTILES), r] = x.max()
+        if math.isfinite(sla):
+            for k in range(len(TAIL_KINDS)):
+                for jt in range(2):
+                    if out[S.tail_col(n_dc, jt, S.TAIL_JOBS), r] > 0:
+                        p99 = out[S.tail_col(n_dc, jt, S.TAIL_STATS_BASE + k * len(TAIL_STATS) + 2), r]
+                        out[S.tail_sla_col(n_dc, k, jt), r] = 1.0 if p99 <= sla else 0.0
+    return out
+
+
+def wilson_interval(successes: float, n: float, z: float = 1.959963984540054):
+    """The Wilson score interval of a binomial share (95 % by default); (NaN, NaN) without trials."""
+    if n <= 0:
+        return float("nan"), float("nan")
+    p = successes / n
+    d = 1.0 + z * z / n
+    c = (p + z * z / (2.0 * n)) / d
+    h = z * math.sqrt(p * (1.0 - p) / n + z * z / (4.0 * n * n)) / d
+    return max(0.0, c - h), min(1.0, c + h)
+
+
+@dataclass
+class TailLatencyResult:
+    """Batch statistics of every replica's own tail-latency columns over the replicas with status 0 (a column counts the
+    replicas where it is defined: a group with a finished job; SLA_MET with an SLA).  ``n`` ... ``max`` and
+    ``quantiles`` ([Q, columns]) cover ``columns`` = (type, dc, field), dc = -1 for all DCs."""
+    columns: Tuple[Tuple[str, int, str], ...]
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray
+    sla_s: float                                       # +inf: none
+
+    @staticmethod
+    def _type(jtype) -> str:
+        return TAIL_TYPES[jtype] if isinstance(jtype, (int, np.integer)) else str(jtype)
+
+    def column(self, kind, jtype, field: str, dc: int = -1) -> int:
+        """Column of ``field`` ("jobs", "unfinished", "p50" ... "max", "sla_met") of ``kind`` (TAIL_KINDS; None for jobs
+        and unfinished) for job type ``jtype`` (0 / 1 or TAIL_TYPES) in DC ``dc`` (-1: all DCs)."""
+        if kind is None:
+            name = field
+        elif field == "sla_met":
+            name = f"{kind}_sla_met"
+        else:
+            name = f"{kind}_{field}_s"
+        return self.columns.index((self._type(jtype), dc, name))
+
+    def sla_attainment(self, kind, jtype) -> dict:
+        """The share of runs (status 0, with a finished job of the type) whose p99 of ``kind`` met the SLA, with its 95 %
+        Wilson interval; NaN without an SLA or such runs."""
+        c = self.column(kind, jtype, "sla_met")
+        runs = int(self.n[c])
+        met = float(self.mean[c]) * runs if runs else 0.0
+        lo, hi = wilson_interval(round(met), runs) if math.isfinite(self.sla_s) else (float("nan"), float("nan"))
+        share = met / runs if runs and math.isfinite(self.sla_s) else float("nan")
+        return {"share": share, "ci95_lo": lo, "ci95_hi": hi, "runs": runs, "met": int(round(met))}
+
+    def pooled(self) -> dict:
+        """{job type: {kind: ...}}: the SLA attainment (share, 95 % interval, runs) and the mean / p05 / p50 / p95 over
+        the runs of the per-run p99 (the quantiles read off the batch histogram, within one bin width)."""
+        out = {jt: {} for jt in TAIL_TYPES}
+        qi = {q: self.q.index(q) for q in (0.05, 0.5, 0.95) if q in self.q}
+        for jt in TAIL_TYPES:
+            for kind in TAIL_KINDS:
+                c = self.column(kind, jt, "p99")
+                row = {"sla_s": self.sla_s if math.isfinite(self.sla_s) else None,
+                       "sla_attainment": self.sla_attainment(kind, jt), "runs": int(self.n[c]),
+                       "p99_mean_s": float(self.mean[c])}
+                for q, i in qi.items():
+                    row[f"p99_p{int(round(q * 100)):02d}_s"] = float(self.quantiles[i, c])
+                out[jt][kind] = row
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """Long format: type,dc,field,n,mean,std,min,p05,p25,p50,p75,p95,p99,max — one row per (type, scope, field),
+        dc empty for all DCs, then the *_sla_met rows (left empty without an SLA)."""
+        fmt = lambda x: repr(float(x))  # noqa: E731
+        with open(path, "w", newline="") as f:
+            w = csv.writer(f)
+            w.writerow(TAIL_CSV_HEADER)
+            for c, (jt, d, field) in enumerate(self.columns):
+                dc = dc_names[d] if d >= 0 else ""
+                if field.endswith("_sla_met") and not math.isfinite(self.sla_s):
+                    w.writerow([jt, dc, field] + [""] * (len(TAIL_CSV_HEADER) - 3))
+                    continue
+                w.writerow([jt, dc, field, int(self.n[c]), fmt(self.mean[c]), fmt(self.std[c]), fmt(self.min[c])]
+                           + [fmt(self.quantiles[j, c]) for j in range(len(self.q))] + [fmt(self.max[c])])
+
+
+def tail_finalize(mom, m2, hist, n_dc: int, sla_s: float, quantiles: Sequence[float] = PP_CSV_QUANTILES
+                  ) -> TailLatencyResult:
+    """All-reduced moments, m2 and histograms over the tail columns -> statistics."""
+    cols = _tail_columns(n_dc)
+    st = column_stats(np.asarray(mom, dtype=np.float64), np.asarray(m2), np.asarray(hist), _tail_integral(n_dc), quantiles)
+    return TailLatencyResult(columns=cols, **st.result_fields((len(cols),)), sla_s=float(sla_s))
+
+
+def tail_latency(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> TailLatencyResult:
+    """Statistics of the per-run tail-latency columns of ``engine`` (a finished BatchedEngine with
+    enable_tail_latency()), over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
+    import torch
+    from . import spec as S
+    if not engine.tail_latency_enabled:
+        raise RuntimeError("tail latency not enabled (enable_tail_latency)")
+    dev = torch.device("cuda", engine.device)
+    n_dc = engine.spec.n_dc
+    passes = device_passes(dev, S.tail_cols(n_dc), engine.tail_latency_moments_into, engine.tail_latency_spread_into)
+    sla = engine.tail_latency_sla
+    return tail_finalize(*passes, n_dc, math.inf if sla is None else sla, quantiles)
+
+
+def tail_latency_from_rows(rows: np.ndarray, status, sla_s=None, quantiles: Sequence[float] = PP_CSV_QUANTILES
+                           ) -> TailLatencyResult:
+    """The same statistics from host columns [tail columns, R] (BatchedEngine.tail_latency_rows) and the replicas'
+    status words through the numpy mirror of both passes.  All-reduced over the ranks like tail_latency."""
+    from . import spec as S
+    rows = np.asarray(rows, dtype=np.float64)
+    n_dc = (rows.shape[0] - 2 * len(TAIL_KINDS)) // (2 * S.TAIL_GROUP_FIELDS) - 1
+    ok = (np.asarray(status)[None, :] == 0) & ~np.isnan(rows)
+    passes = host_passes(rows, ok, _tail_integral(n_dc))
+    return tail_finalize(*passes, n_dc, math.inf if sla_s is None else float(sla_s), quantiles)
+
+
+def tail_latency_from_jobs(jobs: Sequence[np.ndarray], status, n_dc: int, sla_s=None,
+                           quantiles: Sequence[float] = PP_CSV_QUANTILES) -> TailLatencyResult:
+    """The numpy mirror end to end: per replica its created jobs (TAIL_JOB_DTYPE) and status word -> the per-run
+    columns with np.quantile(..., method="inverted_cdf") -> batch statistics through host_passes."""
+    return tail_latency_from_rows(tail_rows_from_jobs(jobs, status, n_dc, sla_s), status, sla_s, quantiles)

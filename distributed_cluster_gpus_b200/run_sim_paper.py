@@ -74,6 +74,10 @@ def parse_args(argv=None):
                    help="write batch statistics of every DC's time-averaged queue lengths and running jobs, longest "
                         "queues and shares of time queued / saturated / idle, measured between every two events, and "
                         "the pooled queue-length and busy-GPU time distributions, to this file")
+    p.add_argument("--tail-latency-csv", type=str, default=None, metavar="PATH",
+                   help="write batch statistics of every run's own exact p50 / p95 / p99 / p99.9 / max of service, "
+                        "wait and response time per job type and DC, its finished and unfinished jobs, and whether its "
+                        "p99 met --sla_p99_ms, to this file")
     p.add_argument("--power-profile-csv", type=str, default=None, metavar="PATH",
                    help="write batch statistics of every replica's cluster power over time — peak, time and energy over "
                         "--power-threshold, longest excursion, per-DC peaks — and the pooled power-duration curve's "
@@ -123,7 +127,7 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
         job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
         power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None,
-        occupancy=args.occupancy_csv is not None)
+        occupancy=args.occupancy_csv is not None, tail_latency=args.tail_latency_csv is not None)
     return sim
 
 
@@ -163,6 +167,7 @@ def main(argv=None):
     _add_power_profile(stats, sim.power_profile)
     _add_job_waits(stats, sim.job_waits)
     _add_occupancy(stats, sim.occupancy, sim)
+    _add_tail_latency(stats, sim.tail_latency)
     _report(args, stats)
     return sim
 
@@ -178,6 +183,8 @@ def _write_ensemble(args, sim):
         sim.job_waits.to_csv(args.job_waits_csv, [dc.name for dc in sim.dcs.values()])
     if args.occupancy_csv:
         sim.occupancy.to_csv(args.occupancy_csv, [dc.name for dc in sim.dcs.values()])
+    if args.tail_latency_csv:
+        sim.tail_latency.to_csv(args.tail_latency_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -209,6 +216,13 @@ def _add_occupancy(stats, res, sim):
     if res is not None:
         names = [dc.name for dc in sim.dcs.values()]
         stats["occupancy"] = {names[d]: v for d, v in res.pooled().items()}
+
+
+def _add_tail_latency(stats, res):
+    """Per job type and kind, for --summary-json: the share of runs whose p99 met the SLA (95 % Wilson interval) and
+    the mean / p05 / p50 / p95 over the runs of the per-run p99."""
+    if res is not None:
+        stats["tail_latency"] = res.pooled()
 
 
 def _add_latency_quantiles(stats, hist):
@@ -255,6 +269,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--job-waits-csv needs at least one replica per rank")
     if args.occupancy_csv and count == 0:
         raise SystemExit("--occupancy-csv needs at least one replica per rank")
+    if args.tail_latency_csv and count == 0:
+        raise SystemExit("--tail-latency-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -291,6 +307,7 @@ def _main_sharded(args, world, rank):
         _add_power_profile(stats, sim.power_profile)
         _add_job_waits(stats, sim.job_waits)
         _add_occupancy(stats, sim.occupancy, sim)
+        _add_tail_latency(stats, sim.tail_latency)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -314,6 +331,9 @@ def _main_compare(args, world, rank):
     if args.occupancy_csv:
         raise SystemExit("--occupancy-csv is not available with --compare-algos (run each algo on its own for its "
                          "occupancy)")
+    if args.tail_latency_csv:
+        raise SystemExit("--tail-latency-csv is not available with --compare-algos (run each algo on its own for its "
+                         "per-run tail latency)")
     if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
         raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
                          "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")

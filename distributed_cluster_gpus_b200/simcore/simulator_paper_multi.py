@@ -61,7 +61,8 @@ class MultiIngressPaperSimulator:
                  replicas: int = 1, device: int = 0, first_replica_id: int = 0, write_logs: bool = True,
                  cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
                  job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None, power_profile: bool = False,
-                 power_threshold: Optional[float] = None, job_waits: bool = False, occupancy: bool = False):
+                 power_threshold: Optional[float] = None, job_waits: bool = False, occupancy: bool = False,
+                 tail_latency: bool = False):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -118,6 +119,11 @@ class MultiIngressPaperSimulator:
         # between events over all replicas (all ranks, as above), ensemble.OccupancyResult
         self._want_occupancy = bool(occupancy)
         self.occupancy = None
+        # tail_latency=True: after run(), statistics over all replicas (all ranks, as above) of every run's own exact
+        # p50 / p95 / p99 / p99.9 / max of service, wait and response time per job type and DC, and the share of runs
+        # whose p99 met sla_p99_ms, ensemble.TailLatencyResult
+        self._want_tail_latency = bool(tail_latency)
+        self.tail_latency = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -171,7 +177,8 @@ class MultiIngressPaperSimulator:
                                           cluster_ensemble=self._want_ensemble, job_ensemble=self._want_job_ensemble,
                                           job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
                                           power_threshold=self._power_threshold, job_waits=self._want_job_waits,
-                                          occupancy=self._want_occupancy)
+                                          occupancy=self._want_occupancy, tail_latency=self._want_tail_latency,
+                                          tail_sla_s=float(self.sla_p99_ms) / 1000.0)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -195,6 +202,9 @@ class MultiIngressPaperSimulator:
             if self._want_occupancy:
                 from ..ensemble import occupancy
                 self.occupancy = occupancy(eng)
+            if self._want_tail_latency:
+                from ..ensemble import tail_latency
+                self.tail_latency = tail_latency(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

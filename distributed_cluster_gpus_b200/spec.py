@@ -47,6 +47,27 @@ PP_FIELDS, PP_BINS = 8, 1024
 # OCC_BINS queue-length bins, then per DC OCC_BINS busy-GPU bins
 OCC_Q_INF_AREA, OCC_Q_TRN_AREA, OCC_RUN_AREA, OCC_Q_INF_MAX, OCC_Q_TRN_MAX, OCC_QUEUED_S, OCC_SATURATED_S, OCC_IDLE_S = range(8)
 OCC_FIELDS, OCC_BINS = 8, 128
+# per-run tail latency columns (DCSIM_TAIL_*): per group (job type, scope: all DCs, then DC 0 ...) the fields JOBS,
+# UNFINISHED, then per kind the statistics; after the groups SLA_MET per (kind, job type)
+TAIL_JOBS, TAIL_UNFINISHED, TAIL_STATS_BASE = 0, 1, 2
+TAIL_KINDS = ("latency", "wait", "response")
+TAIL_STATS = ("p50", "p95", "p99", "p999", "max")
+TAIL_QUANTILES = (0.5, 0.95, 0.99, 0.999)
+TAIL_GROUP_FIELDS = 2 + len(TAIL_KINDS) * len(TAIL_STATS)
+
+
+def tail_cols(n_dc: int) -> int:
+    return 2 * (n_dc + 1) * TAIL_GROUP_FIELDS + 2 * len(TAIL_KINDS)
+
+
+def tail_col(n_dc: int, jt: int, field: int, dc: int = -1) -> int:
+    """Column of group (jt, dc) (dc = -1: all DCs) and field (TAIL_JOBS, TAIL_UNFINISHED or TAIL_STATS_BASE + kind * 5 +
+    stat)."""
+    return (jt * (n_dc + 1) + dc + 1) * TAIL_GROUP_FIELDS + field
+
+
+def tail_sla_col(n_dc: int, kind: int, jt: int) -> int:
+    return 2 * (n_dc + 1) * TAIL_GROUP_FIELDS + kind * 2 + jt
 
 
 class Coeffs(C.Structure):

@@ -528,6 +528,54 @@ int dcsim_occupancy_moments(dcsim_t* h, double* dev_out);
 int dcsim_occupancy_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                            double* dev_m2_out, uint64_t* dev_hist_out);
 
+/* Per-run tail latency: for EVERY replica, exact order statistics of its own finished jobs.  For a job that finished
+ * (status 0 replica) with arrival instant arr (the ingress arrival, simulator_paper_multi.py:539-540), xfer_done instant
+ * tx (SIM:580-588), start and finish, each one f64 subtraction:
+ *   latency  = finish - start   (SIM:820: the latency_s column, the reference's p99 monitor sample)
+ *   wait     = start - tx       (as dcsim_enable_job_waits)
+ *   response = finish - arr     (as dcsim_enable_job_waits)
+ * A group is (job type, scope): scope 0 all DCs, scope 1 + d DC d (the DC the job ran in).  Per replica and group:
+ *   JOBS        jobs of the group that finished;
+ *   UNFINISHED  jobs the run created (a jid, SIM:541) of that type, routed to that DC, not finished at end_time
+ *               (in transfer, queued or running); summed over types and DCs: JOBS_CREATED - JOBS_FINISHED;
+ *   per kind K: P50, P95, P99, P999 — the q-quantile of the group's n values is the k-th smallest, k = max(ceil(fl(n *
+ *               q)), 1) with fl the f64 product (numpy.quantile(..., method="inverted_cdf")) — and MAX; NaN for an
+ *               empty group.
+ * Then per (kind, job type) SLA_MET: 1.0 when the run's P99 of the all-DC group is <= sla_s, else 0.0; NaN without a
+ * finished job of that type, or with sla_s = +inf (no SLA).  Column of group (jt, scope), field f:
+ * (jt * (n_dc + 1) + scope) * DCSIM_TAIL_GROUP_FIELDS + f, f = JOBS, UNFINISHED or DCSIM_TAIL_STAT(kind, stat); column
+ * of SLA_MET: 2 * (n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS + kind * 2 + jt.  Device layout [DCSIM_TAIL_COLS(n_dc)]
+ * [n_replicas] doubles, replica fastest; every column of a replica whose status is not 0 is NaN. */
+enum {
+  DCSIM_TAIL_JOBS = 0, DCSIM_TAIL_UNFINISHED = 1,
+  DCSIM_TAIL_LATENCY = 0, DCSIM_TAIL_WAIT = 1, DCSIM_TAIL_RESPONSE = 2, DCSIM_TAIL_KINDS = 3,
+  DCSIM_TAIL_P50 = 0, DCSIM_TAIL_P95 = 1, DCSIM_TAIL_P99 = 2, DCSIM_TAIL_P999 = 3, DCSIM_TAIL_MAX = 4,
+  DCSIM_TAIL_QUANTILES = 4, /* P50 .. P999: order statistics */
+  DCSIM_TAIL_STATS = 5,
+  DCSIM_TAIL_GROUP_FIELDS = 2 + DCSIM_TAIL_KINDS * DCSIM_TAIL_STATS
+};
+#define DCSIM_TAIL_STAT(kind, stat) (2 + (kind) * DCSIM_TAIL_STATS + (stat))
+#define DCSIM_TAIL_COLS(n_dc) (2 * ((n_dc) + 1) * DCSIM_TAIL_GROUP_FIELDS + 2 * DCSIM_TAIL_KINDS)
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, cleared by it).  Each finished job stores its
+ * start and finish into a per-arrival slot buffer [n_replicas][cap_arrivals][2] doubles (16 bytes per slot, NaN until
+ * it finishes); the running records carry the job id (the layout job_log.csv uses).  DCSIM_E_INVALID for a NaN or
+ * negative sla_s (+inf: no SLA), DCSIM_E_STATE after the first advance or on a member of a shared group, DCSIM_E_NOMEM
+ * (with the byte count in dcsim_last_error) when the buffers do not fit. */
+int dcsim_enable_tail_latency(dcsim_t* h, double sla_s);
+/* The columns to host memory, [DCSIM_TAIL_COLS(n_dc)][n_replicas] doubles (synchronises).  The columns are made from
+ * the slot buffer by one selection pass on the handle's stream, run by the first of this call, _moments or _spread
+ * after the batch is done (every later advance or reset makes them stale); DCSIM_E_STATE while a replica is still
+ * running.  A smaller buffer is DCSIM_E_INVALID. */
+int dcsim_fetch_tail_latency(dcsim_t* h, double* out, size_t out_bytes);
+/* The raw slot buffer of local replicas [first, first + count): [count][cap_arrivals][2] doubles, (start, finish) of
+ * arrival slot jid - 1 (synchronises).  A range, because a large batch's buffer takes tens of GB. */
+int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* out, size_t out_bytes);
+/* The two passes over the DCSIM_TAIL_COLS(n_dc) columns: the contract of dcsim_ensemble_moments / _spread.  A replica
+ * counts in a column when its status is 0 and the value is not NaN.  JOBS, UNFINISHED and SLA_MET are integer columns. */
+int dcsim_tail_latency_moments(dcsim_t* h, double* dev_out);
+int dcsim_tail_latency_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                              double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant
  * batch with the same keys (a member's dcsim_summary_device_ptr or a copy of it: [n][DCSIM_SUMMARY_K] doubles on the
  * base's device).  Replica r counts in a column when both rows have status 0 and the metric is defined in both (a

@@ -1,16 +1,17 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy, the job-log ensemble / the power
-profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder) at bench size: the event loop with
-the recorder off and on, the two reduction kernels, the recorder's bytes per replica.  One JSON line on stdout; writes
-nothing else.
+"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy / tail, the job-log ensemble / the
+power profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder / the per-run tail-latency
+recorder) at bench size: the event loop with the recorder off and on, the two reduction kernels, the recorder's bytes per
+replica.  One JSON line on stdout; writes nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy|tail] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
 (off on / on off / ...), the seeds are the same, times are CUDA events on the launching stream (bench.timed_batch: one
 warm-up batch, then one timed).  The reductions are timed on their second pass; the moments pass includes the capacity
-check's host round trip (the job-log ensemble has none).
+check's host round trip (the job-log ensemble has none).  For the tail recorder the first moments pass also runs the
+selection pass (with its all-done check): `selection_ms` is that first pass less the second.
 """
 import argparse
 import json
@@ -29,7 +30,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -56,6 +57,8 @@ def main():
             e.enable_power_profile(sp.power_cap if sp.power_cap > 0 else None)
         elif arm == "on" and args.recorder == "occupancy":
             e.enable_occupancy()
+        elif arm == "on" and args.recorder == "tail":
+            e.enable_tail_latency(0.5)
         elif arm == "on":
             e.enable_cluster_ensemble()
         return e
@@ -82,6 +85,11 @@ def main():
             cols = (S.OCC_FIELDS + 2 * S.OCC_BINS) * sp.n_dc
             moments_into, spread_into = on.occupancy_moments_into, on.occupancy_spread_into
             rows, recorder_bytes = cols + 1, (cols + 1) * 8 + sp.n_dc * 11 * 8   # columns + working rows (DCSIM_OCCW_N)
+        elif args.recorder == "tail":
+            cols = S.tail_cols(sp.n_dc)
+            moments_into, spread_into = on.tail_latency_moments_into, on.tail_latency_spread_into
+            cap = sp.cap_arrivals if sp.cap_arrivals > 0 else 16384
+            rows, recorder_bytes = cols, cols * 8 + cap * 16     # columns + the slot buffer (16 B per arrival slot)
         elif args.recorder == "waits":
             cols = (on.job_ensemble_windows + 1) * len(EN.WAIT_FIELDS) * sp.n_dc * 2
             moments_into, spread_into = on.job_waits_moments_into, on.job_waits_spread_into
@@ -106,6 +114,7 @@ def main():
         m2 = torch.zeros(cols, dtype=torch.float64, device="cuda")
         hist = torch.zeros((cols, EN.BINS), dtype=torch.int64, device="cuda")
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
+        first_moments_ms = None
         for _ in range(2):
             torch.cuda.synchronize()
             ev[0].record(stream)
@@ -119,6 +128,9 @@ def main():
             spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
             ev[3].record(stream)
             torch.cuda.synchronize()
+            first_moments_ms = ev[0].elapsed_time(ev[1]) if first_moments_ms is None else first_moments_ms
+        if args.recorder == "tail":
+            stats = EN.tail_latency(on).pooled()
         moments_ms, spread_ms = ev[0].elapsed_time(ev[1]), ev[2].elapsed_time(ev[3])
     finally:
         on.close()
@@ -136,7 +148,9 @@ def main():
                       "slowdown_on_vs_off": med(loop_ms["on"]) / med(loop_ms["off"]) - 1.0,
                       "rows": rows, "bytes_per_replica": recorder_bytes, "bytes_total": recorder_bytes * n,
                       "moments_ms": moments_ms, "spread_ms": spread_ms,
-                      **({"waits": stats} if args.recorder == "waits" else {})}), flush=True)
+                      **({"waits": stats} if args.recorder == "waits" else {}),
+                      **({"selection_ms": first_moments_ms - moments_ms, "tail": stats} if args.recorder == "tail" else {})}),
+          flush=True)
 
 
 if __name__ == "__main__":
