@@ -30,6 +30,7 @@ EXPORTS = (
     "dcsim_power_profile_spread",
     "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_job_waits_moments", "dcsim_job_waits_spread",
     "dcsim_fetch_dc_wait_histogram",
+    "dcsim_enable_job_resources", "dcsim_fetch_job_resources", "dcsim_job_resources_moments", "dcsim_job_resources_spread",
     "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy", "dcsim_occupancy_moments",
     "dcsim_occupancy_spread",
     "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs", "dcsim_tail_latency_moments",
@@ -147,6 +148,15 @@ def load():
         L.dcsim_job_waits_spread.argtypes = [vp, vp, vp, vp, vp, vp]
         L.dcsim_fetch_dc_wait_histogram.restype = i32
         L.dcsim_fetch_dc_wait_histogram.argtypes = [vp, vp, C.c_size_t]
+    if hasattr(L, "dcsim_enable_job_resources"):
+        L.dcsim_enable_job_resources.restype = i32
+        L.dcsim_enable_job_resources.argtypes = [vp]
+        L.dcsim_fetch_job_resources.restype = i32
+        L.dcsim_fetch_job_resources.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t]
+        L.dcsim_job_resources_moments.restype = i32
+        L.dcsim_job_resources_moments.argtypes = [vp, vp]
+        L.dcsim_job_resources_spread.restype = i32
+        L.dcsim_job_resources_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_occupancy"):
         L.dcsim_enable_occupancy.restype = i32
         L.dcsim_enable_occupancy.argtypes = [vp]

@@ -36,7 +36,7 @@ extern __shared__ __align__(16) char dcsim_smem[];
  *                      leave the SM below its 32 warps (8 DC x 256: 17 kB -> 12 warps/SM; head ~4 kB -> 32);
  *   DCSIM_MODE_INPLACE nothing is staged (even the head exceeds a CTA's shared memory): same core on the HBM copy. */
 enum { DCSIM_MODE_INPLACE = 0, DCSIM_MODE_STAGED = 1, DCSIM_MODE_HEAD = 2 };
-/* PP = the profile recorders (power profile, occupancy, tail latency) are compiled in (launched when any is enabled):
+/* PP = the profile recorders (power profile, occupancy, tail latency, job resources) are compiled in (launched when any is enabled):
  * the kernels without them keep their registers, spills and code. */
 template <bool CAP, int MODE, bool PP>
 __global__ void __launch_bounds__(DCSIM_MAX_WARPS_PER_CTA * 32, DCSIM_MIN_CTAS_PER_SM)
@@ -91,10 +91,11 @@ static DCSIM_ADV(dcsim_advance_fn) DCSIM_ADV(dcsim_pick_kernel)(bool cap, int mo
 int DCSIM_ADV(dcsim_adv_min_ctas)(void) { return DCSIM_MIN_CTAS_PER_SM; }
 
 /* Launch on `stream`: `ctas` CTAs of `threads` threads (threads / DCSIM_LANES replicas each), `smem` dynamic bytes.  The
- * instantiation with the profile recorders when P->pp, P->occ or P->tail is set. */
+ * instantiation with the profile recorders when P->pp, P->occ, P->tail or P->jres is set. */
 cudaError_t DCSIM_ADV(dcsim_adv_launch)(const dcsim_kparams_t* P, unsigned long long* events, int cap, int mode, int ctas, int threads,
                                         int smem, cudaStream_t stream) {
-  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr || P->occ != nullptr || P->tail != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
+  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr || P->occ != nullptr || P->tail != nullptr ||
+                                           P->jres != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
   return cudaGetLastError();
 }
 

@@ -247,6 +247,50 @@ struct dcsim_ens_wait_src {
   __device__ __forceinline__ bool integral(uint64_t col) const { return (col / cells) % DCSIM_JWAIT_FIELDS == DCSIM_JWAIT_WAITED; }
 };
 
+/* Job resources: first the windowed columns (row, field, dc, jtype) as the job-log ensemble's, `cells` = n_dc * 2 per
+ * field — GPU_SUM, FREQ_SUM and ENERGY_SUM stored ([row][DCSIM_JRES_STORED][cell][replica]) and counted for every valid
+ * replica, MEAN_* = *_SUM / JOBS for those with a job in the cell (JOBS: the job-log ensemble's count of the same cell) —
+ * then the `count_cols` u32 count columns as stored (the mix, then the energy bins: [cells * (MIX_COLS + EBINS)][n]).
+ * Only replicas with status 0 count. */
+struct dcsim_ens_res_src {
+  const double* jres;
+  const double* jens;
+  const uint32_t* counts;
+  const uint32_t* status;
+  uint64_t n;
+  uint32_t cells;
+  uint64_t win_cols; /* (W + 1) * DCSIM_JRES_FIELDS * cells */
+  struct view {
+    const double* x;
+    const double* jobs;
+    const uint32_t* u;
+    const uint32_t* status;
+    bool mean;
+    __device__ __forceinline__ bool get(uint64_t r, double& v) const {
+      if (status[r] != 0u) return false;
+      if (u) { v = (double)u[r]; return true; }
+      if (!mean) { v = x[r]; return true; }
+      const double k = jobs[r];
+      if (!(k > 0.0)) return false;
+      v = x[r] / k;
+      return true;
+    }
+  };
+  __device__ __forceinline__ view at(uint64_t col) const {
+    if (col >= win_cols) return view{nullptr, nullptr, counts + (col - win_cols) * n, status, false};
+    const uint64_t row = col / ((uint64_t)DCSIM_JRES_FIELDS * cells), cell = col % cells;
+    const int field = (int)((col / cells) % DCSIM_JRES_FIELDS);
+    const bool mean = field >= DCSIM_JRES_STORED;
+    const uint64_t stored = mean ? (uint64_t)(field - DCSIM_JRES_STORED) : (uint64_t)field;
+    const double* x = jres + ((row * DCSIM_JRES_STORED + stored) * cells + cell) * n;
+    const double* jobs = jens + ((row * DCSIM_JENS_STORED + DCSIM_JENS_JOBS) * cells + cell) * n;
+    return view{x, jobs, nullptr, status, mean};
+  }
+  __device__ __forceinline__ bool integral(uint64_t col) const {
+    return col >= win_cols || (col / cells) % DCSIM_JRES_FIELDS == DCSIM_JRES_GPU_SUM;
+  }
+};
+
 /* Per-run tail latency: column c of the [DCSIM_TAIL_COLS(n_dc)][n] columns as stored.  A replica counts when its status
  * is 0 and the value is not NaN (an empty group's statistics, SLA_MET without a job or an SLA).  JOBS, UNFINISHED and
  * SLA_MET are the integer columns. */
@@ -556,6 +600,9 @@ struct dcsim {
   double* d_jwait;         /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waiting / response times (opt-in) */
   uint32_t* d_jwait_hist;  /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] their per-DC histograms */
   unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_wait_histogram */
+  double* d_jres;          /* [jens_windows + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas] job resources (opt-in) */
+  uint32_t* d_jres_cnt;    /* [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] mix, then [n_dc][2][DCSIM_JRES_EBINS][n_replicas]
+                              energy bins */
   uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the job ensemble and power profile
                          reductions, refreshed on the stream ahead of every one of them (status_words) */
   unsigned long long events_seen;
@@ -579,6 +626,17 @@ static size_t jwait_row_bytes(const dcsim_t* h) {
   return (size_t)DCSIM_JWAIT_STORED * (size_t)h->spec.n_dc * 2 * (size_t)h->n_replicas * sizeof(double);
 }
 static size_t jwait_hist_bytes(const dcsim_t* h) { return 2 * jens_hist_bytes(h); }
+
+static size_t jres_row_bytes(const dcsim_t* h) {
+  return (size_t)DCSIM_JRES_STORED * (size_t)h->spec.n_dc * 2 * (size_t)h->n_replicas * sizeof(double);
+}
+static uint64_t jres_mix_cols(const dcsim_t* h) { /* per replica */
+  return 2ull * (uint64_t)h->spec.n_dc * (uint64_t)DCSIM_JRES_MIX_COLS(DCSIM_JRES_G(h->spec.max_gpus_per_job));
+}
+static uint64_t jres_hist_cols(const dcsim_t* h) { return 2ull * (uint64_t)h->spec.n_dc * DCSIM_JRES_EBINS; }
+static size_t jres_cnt_bytes(const dcsim_t* h) {
+  return (size_t)(jres_mix_cols(h) + jres_hist_cols(h)) * (size_t)h->n_replicas * sizeof(uint32_t);
+}
 
 static uint64_t pp_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc + DCSIM_PP_BINS); }
 static size_t pp_bytes(const dcsim_t* h) { return (size_t)pp_cols(h) * (size_t)h->n_replicas * sizeof(double); }
@@ -815,7 +873,7 @@ static cudaError_t size_launch(dcsim_t* h) {
  * switching them on or off re-lays the state block out. */
 static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
-  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL || h->d_tail != NULL);
+  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL || h->d_tail != NULL || h->d_jres != NULL);
   if (L.lean == h->L.lean) return DCSIM_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
@@ -1017,6 +1075,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
   }
   if (h->d_tail) CUDA_TRY(h, cudaMemsetAsync(h->d_tail, 0xff, tail_slot_bytes(h), h->g->stream)); /* NaN: not finished */
   h->tail_fresh = 0;
+  if (h->d_jres) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jres, 0, (h->jens_windows + 1) * jres_row_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_jres_cnt, 0, jres_cnt_bytes(h), h->g->stream));
+  }
   if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
     h->g->seed0 = base_seed + first_replica_id;
     h->g->arrivals_ready = 0;
@@ -1102,6 +1164,8 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
   P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
   P->occ = h->d_occ; P->occ_work = h->d_occ_work;
+  P->jres = h->d_jres; P->jres_mix = h->d_jres_cnt;
+  P->jres_hist = h->d_jres ? h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas : NULL;
 }
 
 /* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */
@@ -1450,6 +1514,8 @@ int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
   h->d_jens = NULL; h->d_jens_hist = NULL; h->jens_windows = 0; h->jens_bin = 0.0;
   cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); /* sized by the windows: re-enabled after the job ensemble */
   h->d_jwait = NULL; h->d_jwait_hist = NULL;
+  cudaFree(h->d_jres); cudaFree(h->d_jres_cnt); /* likewise */
+  h->d_jres = NULL; h->d_jres_cnt = NULL;
   const uint64_t windows = dcsim_jens_windows(h->spec.end_time, bin);
   const double need = ((double)windows + 1.0) * (double)jens_row_bytes(h) + (double)jens_hist_bytes(h);
   const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
@@ -1577,6 +1643,65 @@ int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   if (rc != DCSIM_OK) return rc;
   CUDA_TRY(h, hist_reduce(h, h->d_jwait_hist, row_len, h->d_status, h->d_jwait_hist_out, out));
   return DCSIM_OK;
+}
+
+int dcsim_enable_job_resources(dcsim_t* h) {
+  if (!h) return DCSIM_E_INVALID;
+  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "enable_job_resources needs the job ensemble (dcsim_enable_job_ensemble first)%s%lld");
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_job_resources on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_resources must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  const size_t rows_bytes = (h->jens_windows + 1) * jres_row_bytes(h);
+  if (!h->d_jres) {
+    const int rc = recorder_alloc(h, (void**)&h->d_jres, rows_bytes, (void**)&h->d_jres_cnt, jres_cnt_bytes(h),
+                                  "enable_job_resources: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)",
+                                  (long long)(rows_bytes + jres_cnt_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jres, 0, rows_bytes, h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_jres_cnt, 0, jres_cnt_bytes(h), h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* mix, size_t mix_bytes, uint32_t* hist,
+                              size_t hist_bytes) {
+  if (!h) return DCSIM_E_INVALID;
+  const int rc = recorder_ready(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
+  if (rc != DCSIM_OK) return rc;
+  const size_t need_rows = (h->jens_windows + 1) * jres_row_bytes(h);
+  const size_t need_mix = (size_t)jres_mix_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t);
+  const size_t need_hist = (size_t)jres_hist_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t);
+  if ((rows && rows_bytes < need_rows) || (mix && mix_bytes < need_mix) || (hist && hist_bytes < need_hist))
+    return set_err(h, DCSIM_E_INVALID, "fetch_job_resources: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
+  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jres, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
+  if (mix) CUDA_TRY(h, cudaMemcpyAsync(mix, h->d_jres_cnt, need_mix, cudaMemcpyDeviceToHost, h->g->stream));
+  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas, need_hist,
+                                        cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+static dcsim_ens_res_src jres_src(const dcsim_t* h) {
+  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
+  return dcsim_ens_res_src{h->d_jres, h->d_jens, h->d_jres_cnt, h->d_status, h->n_replicas, cells,
+                           (h->jens_windows + 1) * DCSIM_JRES_FIELDS * cells};
+}
+
+int dcsim_job_resources_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_res_src src = jres_src(h);
+  return ens_moments(h, src, h->n_replicas, src.win_cols + jres_mix_cols(h) + jres_hist_cols(h), dev_out);
+}
+
+int dcsim_job_resources_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                               double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_res_src src = jres_src(h);
+  return ens_spread(h, src, h->n_replicas, src.win_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out); /* the counts need no spread */
 }
 
 int dcsim_enable_power_profile(dcsim_t* h, double threshold_w) {
@@ -1839,6 +1964,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_occ); cudaFree(h->d_occ_work);
   cudaFree(h->d_tail); cudaFree(h->d_tail_cols);
   cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
+  cudaFree(h->d_jres); cudaFree(h->d_jres_cnt);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }

@@ -494,6 +494,10 @@ struct dcsim_kparams_t {
                            (needs L.lean == 0), or NULL */
   double* tail_cols;    /* [DCSIM_TAIL_COLS(n_dc)][n_replicas] the per-run tail columns (dcsim_tail_select writes them) */
   double tail_sla;      /* [s], +inf: none */
+  double* jres;         /* [jens_windows + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas] job resources (needs jens and
+                           L.lean == 0), or NULL */
+  uint32_t* jres_mix;   /* [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] (n, f) mix counts (with jres) */
+  uint32_t* jres_hist;  /* [n_dc][2][DCSIM_JRES_EBINS][n_replicas] energy-per-job histograms (with jres) */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -513,6 +517,7 @@ struct dcsim_ctx_t {
                             profile recorders (dcsim_replica_step<..., PP>), so their code does not change */
   bool occ;              /* the occupancy recorder runs: likewise */
   bool tail;             /* the tail-latency recorder runs: likewise */
+  bool jres;             /* the job-resources recorder runs: likewise */
   bool quiet;            /* a ghost lane group of an in-place launch, whose blk is replica n-1's live block in HBM: it must
                             not even publish the pop-min cache there.  A compile-time false in the staged and head-staged
                             instantiations (a ghost's blk is its own shared-memory slot there) */
@@ -1999,6 +2004,55 @@ DCSIM_COLD void dcsim_tail_add(const dcsim_kparams_t* P, uint32_t r, double now,
   slot[1] = now;
 }
 
+/* Quarter-octave bin of an energy E [J] anchored at 1 J: clamp(floor(4 * log2(E)), 0, DCSIM_JRES_EBINS - 1), decided
+ * exactly — the binary exponent gives whole octaves, the significand m in [1, 2) is compared with the smallest doubles
+ * >= 2^(1/4), 2^(1/2), 2^(3/4), so no log2 rounding can move a value across a bin edge. */
+DCSIM_DEV int dcsim_jres_ebin(double e) {
+  if (!(e >= 1.0)) return 0;
+  int ex;
+  const double m = 2.0 * frexp(e, &ex); /* e = m * 2^(ex - 1), m in [1, 2) */
+  const int b = 4 * (ex - 1) + (m >= DCSIM_JRES_OCT1) + (m >= DCSIM_JRES_OCT2) + (m >= DCSIM_JRES_OCT3);
+  return b < DCSIM_JRES_EBINS - 1 ? b : DCSIM_JRES_EBINS - 1;
+}
+
+/* Job resources (opt-in: P->jres, on top of P->jens): the job of running record i (at `rec`, the base of the L.rn_*
+ * offsets) of DC d and type jt with g GPUs finished at `now`; its f, size and n * P_gpu are read here, off the hot path.
+ * The record's n * P_gpu is dcsim_task_power(g, f) bit for bit: written with f at the start (the per-DC memo holds the
+ * same operations' results) and rewritten with the new f by every cap_greedy reschedule, so E_pred = P_pred * T_pred is
+ * the reference's (SIM:715-716).  Same cells, window and write discipline as dcsim_jens_add: one writer per cell, so
+ * every sum is the sequential sum in finish order. */
+DCSIM_COLD void dcsim_jres_add(const dcsim_kparams_t* P, uint32_t r, int d, int jt, int g, double now, char* rec, int i) {
+  const dcsim_dc_t& cfg = P->spec.dc[d];
+  const double f = dcsim_at<double>(rec, P->L.rn_f)[i];
+  const double size = dcsim_at<double>(rec, P->L.rn_size)[i];
+  const double e_job = dcsim_at<double>(rec, P->L.rn_pw)[i] * dcsim_step_time(g, f, cfg.coeffs[jt]) * size;
+  const uint64_t n = P->n_replicas, W = P->jens_windows;
+  const uint64_t fs = 2ull * (uint64_t)P->spec.n_dc * n; /* field stride */
+  const double fw = floor(now / P->jens_bin);
+  const uint64_t k = fw >= (double)(W - 1u) ? W - 1u : (uint64_t)fw;
+  double* win = P->jres + k * (DCSIM_JRES_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  double* all = P->jres + W * (DCSIM_JRES_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
+  const int G = DCSIM_JRES_G(P->spec.max_gpus_per_job);
+  int col = G * DCSIM_MAX_FREQ; /* OFF_LEVEL */
+#pragma unroll 1
+  for (int q = 0; q < cfg.n_freq; ++q)
+    if (cfg.freq_levels[q] == f) { col = ((g < G ? g : G) - 1) * DCSIM_MAX_FREQ + q; break; }
+  uint32_t* mix = P->jres_mix + ((uint64_t)(2 * d + jt) * DCSIM_JRES_MIX_COLS(G) + (uint64_t)col) * n + r;
+  uint32_t* hist = P->jres_hist + ((uint64_t)(2 * d + jt) * DCSIM_JRES_EBINS + (uint64_t)dcsim_jres_ebin(e_job)) * n + r;
+  const double gd = (double)g;
+#ifdef DCSIM_HOST_EMU
+  win[DCSIM_JRES_GPU_SUM * fs] += gd; win[DCSIM_JRES_FREQ_SUM * fs] += f; win[DCSIM_JRES_ENERGY_SUM * fs] += e_job;
+  all[DCSIM_JRES_GPU_SUM * fs] += gd; all[DCSIM_JRES_FREQ_SUM * fs] += f; all[DCSIM_JRES_ENERGY_SUM * fs] += e_job;
+  *mix += 1u; *hist += 1u;
+#else
+  atomicAdd(win + DCSIM_JRES_GPU_SUM * fs, gd); atomicAdd(win + DCSIM_JRES_FREQ_SUM * fs, f);
+  atomicAdd(win + DCSIM_JRES_ENERGY_SUM * fs, e_job);
+  atomicAdd(all + DCSIM_JRES_GPU_SUM * fs, gd); atomicAdd(all + DCSIM_JRES_FREQ_SUM * fs, f);
+  atomicAdd(all + DCSIM_JRES_ENERGY_SUM * fs, e_job);
+  atomicAdd(mix, 1u); atomicAdd(hist, 1u);
+#endif
+}
+
 /* SIM:701-927 minus RL/elastic branches (lane 0 part, after the record was read and before it is erased). */
 DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const dcsim_spec_t& sp = c.P->spec;
@@ -2023,6 +2077,7 @@ DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
     if (c.P->jens) dcsim_jens_add(c.P, c.r, d, jt, now, lat);
     if (c.P->jwait) dcsim_jwait_add(c.P, c.r, d, jt, now, c.rec, i); /* (only with jens, in the layout keeping the jid) */
     if (c.tail) dcsim_tail_add(c.P, c.r, now, c.rec, i);               /* (in the layout keeping the jid) */
+    if (c.jres) dcsim_jres_add(c.P, c.r, d, jt, g, now, c.rec, i);     /* (only with jens, in the layout keeping size / f) */
   }
   if (L.lean == 0) { /* the readers of a finished job's size / f / jid: job_log.csv and the bandit's reward */
     const double f_used = dcsim_at<double>(c.rec, L.rn_f)[i];
@@ -2714,6 +2769,7 @@ DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char
   c.pp = PP && !ghost && P->pp != nullptr;
   c.occ = PP && !ghost && P->occ != nullptr;
   c.tail = PP && !ghost && P->tail != nullptr;
+  c.jres = PP && !ghost && P->jres != nullptr;
   c.quiet = INPLACE && ghost;
   if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing to a
                   replica's state (staged modes: its own shared-memory slot takes the pop-min cache; in place: quiet) */

@@ -23,6 +23,14 @@ ENS_FIELDS = 11     # DCSIM_ENS_FIELDS (names: ensemble.FIELDS)
 ENS_BINS = 1024     # DCSIM_ENS_BINS
 JENS_STORED = 2     # DCSIM_JENS_STORED: jobs, lat_sum per (window, dc, jtype) and replica
 JWAIT_STORED = 3    # DCSIM_JWAIT_STORED: waited, wait_sum, resp_sum per (window, dc, jtype) and replica
+JRES_STORED = 3     # DCSIM_JRES_STORED: gpu_sum, freq_sum, energy_sum per (window, dc, jtype) and replica
+MAX_FREQ = 16       # DCSIM_MAX_FREQ: the mix's frequency stride
+JRES_EBINS = 128    # DCSIM_JRES_EBINS: quarter-octave energy-per-job bins from 1 J
+
+
+def jres_mix_g(max_gpus_per_job) -> int:
+    """G = DCSIM_JRES_G(max_gpus_per_job): the GPU-count rows of the (n, f) mix; the last one takes every g >= G."""
+    return min(max(int(max_gpus_per_job), 1), 32)
 
 
 def latency_bin_edges() -> np.ndarray:
@@ -233,6 +241,7 @@ class BatchedEngine:
         job-latency histogram."""
         if self._jens_bin != (float(bin_s) if bin_s else float(self.spec.log_interval)):
             self._jwait_on = False     # the library drops the waits recorder with the old windows, even when this fails
+            self._jres_on = False      # and the job-resources recorder
         N.check(self._lib.dcsim_enable_job_ensemble(self._h, float(bin_s or 0.0)), self._h)
         w = C.c_uint32(0)
         N.check(self._lib.dcsim_job_ensemble_windows(self._h, C.byref(w)), self._h)
@@ -312,6 +321,45 @@ class BatchedEngine:
         out = np.zeros((self.spec.n_dc, 2, 2, LAT_BINS), dtype=np.uint64)
         N.check(self._lib.dcsim_fetch_dc_wait_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
+
+    # -- job resources (ensemble.job_resources), in the job ensemble's cells ------------------------------------------
+    def enable_job_resources(self):
+        """Opt-in, after enable_job_ensemble and before the first advance of a batch (stays on across reset, zeroed by
+        it): every finished job adds its GPU count, frequency and predicted energy E_pred * size to its cells of the job
+        ensemble, and one count each to its DC's (n, f) mix and energy-per-job histogram.  The running records then
+        carry the size and frequency."""
+        N.check(self._lib.dcsim_enable_job_resources(self._h), self._h)
+        self._jres_on = True
+
+    @property
+    def job_resources_enabled(self) -> bool:
+        return getattr(self, "_jres_on", False) and bool(self._jens_windows)
+
+    def job_resources_rows(self):
+        """(rows [W + 1, JRES_STORED, n_dc, 2, n_replicas] float64 {gpu_sum, freq_sum, energy_sum}, mix [n_dc, 2, G,
+        MAX_FREQ, n_replicas] uint32, off_level [n_dc, 2, n_replicas] uint32, hist [n_dc, 2, JRES_EBINS, n_replicas]
+        uint32): every replica's raw recorder.  For tests and small batches."""
+        if not self.job_resources_enabled:
+            raise RuntimeError("job resources not enabled (enable_job_resources)")
+        n_dc, n, G = self.spec.n_dc, self.n_replicas, jres_mix_g(self.spec.max_gpus_per_job)
+        rows = np.empty((self._jens_windows + 1, JRES_STORED, n_dc, 2, n), dtype=np.float64)
+        mix = np.empty((n_dc, 2, G * MAX_FREQ + 1, n), dtype=np.uint32)
+        hist = np.empty((n_dc, 2, JRES_EBINS, n), dtype=np.uint32)
+        N.check(self._lib.dcsim_fetch_job_resources(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
+                                                    C.c_void_p(mix.ctypes.data), mix.nbytes,
+                                                    C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        return rows, mix[:, :, :-1].reshape(n_dc, 2, G, MAX_FREQ, n), np.ascontiguousarray(mix[:, :, -1]), hist
+
+    def job_resources_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][(W + 1) * 6 * n_dc * 2 + n_dc * 2 * (G * MAX_FREQ + 1 + JRES_EBINS)] float64
+        {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_job_resources_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def job_resources_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream, over the (W + 1) * 6 * n_dc * 2 windowed columns: per column sum
+        (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_job_resources_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                     C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
     # -- power profile (ensemble.power_profile turns it into batch statistics) ----------------------------------------
     def enable_power_profile(self, threshold=None):
@@ -560,11 +608,11 @@ def _pp_key(power_profile, power_threshold):
 
 
 def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False,
-               occupancy=False, tail=None):
+               occupancy=False, tail=None, job_resources=False):
     # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
             os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None),
-            bool(occupancy), tail)
+            bool(occupancy), tail, bool(job_resources and job_bin is not None))
 
 
 def _tail_key(tail_latency, tail_sla_s):
@@ -580,16 +628,17 @@ def _drop_parked_batch_engine():
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
                    job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                   occupancy=False, tail_latency=False, tail_sla_s=None):
+                   occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
     ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
     power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
     response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on;
-    ``tail_latency``: with the per-run tail-latency recorder on, SLA ``tail_sla_s`` seconds (None: none).  A parked
-    engine is only reused by a caller that asks for the same recorders."""
-    job_bin = _job_bin(sp, job_ensemble or job_waits, job_ensemble_bin)
+    ``tail_latency``: with the per-run tail-latency recorder on, SLA ``tail_sla_s`` seconds (None: none);
+    ``job_resources``: with the job-resources recorder on (it implies the job ensemble).  A parked engine is only reused
+    by a caller that asks for the same recorders."""
+    job_bin = _job_bin(sp, job_ensemble or job_waits or job_resources, job_ensemble_bin)
     key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
-                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s))
+                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s), job_resources)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -606,6 +655,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_job_ensemble(job_bin)
         if job_waits:
             eng.enable_job_waits()
+        if job_resources:
+            eng.enable_job_resources()
         if power_profile:
             eng.enable_power_profile(power_threshold)
         if occupancy:
@@ -627,7 +678,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
                                                         eng.job_ensemble_bin,
                                                         _pp_key(eng.power_profile_enabled, eng.power_threshold),
                                                         eng.job_waits_enabled, eng.occupancy_enabled,
-                                                        _tail_key(eng.tail_latency_enabled, eng.tail_latency_sla))
+                                                        _tail_key(eng.tail_latency_enabled, eng.tail_latency_sla),
+                                                        eng.job_resources_enabled)
 
 
 def free_cached_engine():
@@ -677,7 +729,7 @@ class LoggedReplica:
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
                       job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                      occupancy=False, tail_latency=False, tail_sla_s=None):
+                      occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
@@ -686,13 +738,14 @@ def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, d
     window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
     None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble);
     ``occupancy``: with the occupancy recorder on; ``tail_latency``: with the per-run tail-latency recorder on
-    (``tail_sla_s``: its SLA [s], None = none), its slot buffer sized by each attempt's cap_arrivals."""
+    (``tail_sla_s``: its SLA [s], None = none), its slot buffer sized by each attempt's cap_arrivals; ``job_resources``:
+    with the job-resources recorder on (and the job ensemble)."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
                              job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy,
-                             tail_latency, tail_sla_s)
+                             tail_latency, tail_sla_s, job_resources)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

@@ -637,6 +637,234 @@ def job_waits_from_rows(rows: np.ndarray, hist: np.ndarray, jobs: np.ndarray, st
     return waits_finalize(*passes, wait_hist, n_dc, bin_s, end_time, quantiles)
 
 
+# ---- job resources: GPUs, frequency and predicted energy of every finished job ---------------------------------------
+RES_FIELDS = ("gpu_sum", "freq_sum", "energy_sum", "mean_gpus", "mean_freq_ghz", "mean_energy_j")   # DCSIM_JRES_* order
+RES_CSV_FIELDS = ("mean_gpus", "mean_freq_ghz", "mean_energy_j")
+RES_EBINS = 128                                        # DCSIM_JRES_EBINS
+RES_MAX_FREQ = 16                                      # DCSIM_MAX_FREQ: the mix's frequency stride
+RES_OCT = (float.fromhex("0x1.306fe0a31b716p+0"), float.fromhex("0x1.6a09e667f3bcdp+0"),
+           float.fromhex("0x1.ae89f995ad3aep+0"))     # DCSIM_JRES_OCT1..3: the smallest doubles >= 2^(1/4, 1/2, 3/4)
+
+
+def energy_bin(e) -> np.ndarray:
+    """dcsim_jres_ebin: clamp(floor(4 * log2(E)), 0, RES_EBINS - 1), decided exactly from the binary exponent and the
+    significand's place among RES_OCT."""
+    e = np.asarray(e, dtype=np.float64)
+    m, ex = np.frexp(np.where(e >= 1.0, e, 1.0))
+    m = 2.0 * m
+    b = 4 * (ex.astype(np.int64) - 1) + sum((m >= t).astype(np.int64) for t in RES_OCT)
+    return np.where(e >= 1.0, np.minimum(b, RES_EBINS - 1), 0)
+
+
+def energy_bin_edges() -> np.ndarray:
+    """Lower edges [J] of the RES_EBINS energy bins (+ the upper edge of the last): 2^(k / 4)."""
+    return 2.0 ** (np.arange(RES_EBINS + 1) / 4.0)
+
+
+def _res_columns(rows: np.ndarray, mix: np.ndarray, hist: np.ndarray, jobs: np.ndarray, status: np.ndarray):
+    """rows [W + 1, 3, n_dc, 2, R] {gpu_sum, freq_sum, energy_sum}, mix [n_dc, 2, G * RES_MAX_FREQ + 1, R] (the stored
+    layout, OFF_LEVEL last), hist [n_dc, 2, RES_EBINS, R], jobs [W + 1, n_dc, 2, R] (the job ensemble's counts) ->
+    (x, ok) [columns, R] as the kernels' column source: the windowed (row, RES_FIELDS, dc, jtype) columns, then the mix
+    and the energy bins as stored."""
+    R = rows.shape[-1]
+    with np.errstate(invalid="ignore", divide="ignore"):
+        x = np.concatenate([rows, rows / jobs[:, None]], axis=1)
+    good = np.broadcast_to((np.asarray(status) == 0)[None, None, None, :], jobs.shape)
+    has = good & (jobs > 0)
+    ok = np.stack([good, good, good, has, has, has], axis=1)
+    counts = np.concatenate([np.asarray(mix).reshape(-1, R), np.asarray(hist).reshape(-1, R)]).astype(np.float64)
+    x = np.concatenate([x.reshape(-1, R), counts])
+    ok = np.concatenate([ok.reshape(-1, R), np.broadcast_to((np.asarray(status) == 0)[None, :], counts.shape)])
+    return x, ok
+
+
+def _res_integral(n_cols: int, n_dc: int) -> np.ndarray:
+    return (np.arange(n_cols) // (2 * n_dc)) % len(RES_FIELDS) == 0
+
+
+@dataclass
+class JobResourcesResult:
+    """Per (row, field, dc, jtype) statistics over every replica of the batch; arrays are [W + 1, len(fields), n_dc, 2],
+    rows as JobEnsembleResult's.  Per job: g its GPU count, f its frequency [GHz] (f_used), E_job = E_pred * size its
+    predicted energy [J].  Whole run, pooled over the valid replicas: ``mix`` [n_dc, 2, G, RES_MAX_FREQ] jobs per GPU
+    count (row g - 1; the last row holds g >= G) and frequency level (column q: ``levels[d, q]``, NaN past the DC's
+    levels), ``off_level`` [n_dc, 2] jobs whose f matched no level, ``energy_histogram`` [n_dc, 2, RES_EBINS]."""
+    t0_s: np.ndarray
+    t1_s: np.ndarray
+    bin_s: float
+    end_time: float
+    fields: Tuple[str, ...]
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray                              # [Q, W + 1, fields, n_dc, 2]
+    levels: np.ndarray                                 # [n_dc, RES_MAX_FREQ] frequency levels [GHz], NaN past n_freq
+    jobs: np.ndarray                                   # [n_dc, 2]: finished jobs of the valid replicas, whole run
+    gpu_sum: np.ndarray                                # [n_dc, 2]: their sums, pooled over replicas
+    freq_sum: np.ndarray
+    energy_sum: np.ndarray
+    mix: np.ndarray                                    # [n_dc, 2, G, RES_MAX_FREQ] uint64
+    off_level: np.ndarray                              # [n_dc, 2] uint64
+    energy_histogram: np.ndarray                       # [n_dc, 2, RES_EBINS] uint64
+
+    def quantile_names(self):
+        return [f"p{int(round(q * 100)):02d}" for q in self.q]
+
+    def mix_shares(self, d: int, jt: int) -> np.ndarray:
+        """[G, RES_MAX_FREQ] share of DC d's finished jobs of type jt at each (GPU count, level); NaN without jobs."""
+        total = float(self.mix[d, jt].sum() + self.off_level[d, jt])
+        return self.mix[d, jt] / total if total else np.full(self.mix[d, jt].shape, np.nan)
+
+    def mix_labels(self, d: int):
+        """((g row, level column, label) for every GPU count and level of DC d), label "n{g}_f{level}" ("n{G}+" for the
+        last row)."""
+        G = self.mix.shape[2]
+        out = []
+        for gi in range(G):
+            for qi in range(self.levels.shape[1]):
+                if self.levels[d, qi] == self.levels[d, qi]:
+                    out.append((gi, qi, f"n{gi + 1}{'+' if gi == G - 1 else ''}_f{float(self.levels[d, qi])!r}"))
+        return out
+
+    def energy_quantiles(self, d: int, jt: int, qs=None) -> list:
+        """Quantiles [J] of E_job of DC d's jobs of type jt, pooled over the replicas, log-interpolated in the
+        quarter-octave bin that holds each; NaN without jobs."""
+        qs = self.q if qs is None else qs
+        h = np.asarray(self.energy_histogram[d, jt], dtype=np.float64)
+        total = h.sum()
+        if total == 0:
+            return [float("nan")] * len(qs)
+        edges, cum, out = energy_bin_edges(), np.cumsum(h), []
+        for q in qs:
+            b = min(int(np.searchsorted(cum, q * total, side="left")), RES_EBINS - 1)
+            below = cum[b - 1] if b else 0.0
+            frac = (q * total - below) / h[b] if h[b] else 0.0
+            out.append(float(edges[b] * (edges[b + 1] / edges[b]) ** frac))
+        return out
+
+    def pooled(self, qs=(0.5, 0.95, 0.99)) -> dict:
+        """Per DC (index) and job type: jobs, pooled mean GPUs / frequency / energy per job, energy quantiles, and the
+        (n, f) mix as shares (the occupied cells only, plus off_level)."""
+        out = {}
+        nan = float("nan")
+        for d in range(self.jobs.shape[0]):
+            row = {}
+            for jt, name in enumerate(JOB_TYPES):
+                jobs = float(self.jobs[d, jt])
+                e = {"jobs": int(jobs), "mean_gpus": float(self.gpu_sum[d, jt]) / jobs if jobs else nan,
+                     "mean_freq_ghz": float(self.freq_sum[d, jt]) / jobs if jobs else nan,
+                     "mean_energy_j": float(self.energy_sum[d, jt]) / jobs if jobs else nan}
+                for q, v in zip(qs, self.energy_quantiles(d, jt, qs)):
+                    e[f"p{int(round(q * 100)):02d}_energy_j"] = v
+                shares = self.mix_shares(d, jt)
+                e["mix"] = {lab: float(shares[gi, qi]) for gi, qi, lab in self.mix_labels(d) if self.mix[d, jt, gi, qi]}
+                e["off_level_share"] = float(self.off_level[d, jt]) / jobs if jobs else nan
+                row[name] = e
+            out[d] = row
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """The job ensemble's long format (t0_s,t1_s,dc,type,field,n,mean,std,min,p05,...,p95,max).  Per window, then for
+        the whole run, the rows of ``mean_gpus``, ``mean_freq_ghz`` and ``mean_energy_j`` per DC and type; then per DC
+        and type the whole-run rows ``energy_j`` (n = jobs, mean = the pooled mean, quantiles from the per-DC histogram;
+        std / min / max empty), one ``mix_n{g}_f{level}`` row per GPU count and level (n = jobs, mean = their share) and
+        ``mix_off_level``."""
+        rows, F, D, J = self.n.shape
+        keep = [self.fields.index(f) for f in RES_CSV_FIELDS]
+        nan = float("nan")
+        with open(path, "w", newline="") as f:
+            w = csv.writer(f)
+            w.writerow(JOB_CSV_HEADER_HEAD + self.quantile_names() + ["max"])
+            for k in range(rows):
+                for d in range(D):
+                    for jt in range(J):
+                        for i in keep:
+                            w.writerow([repr(float(self.t0_s[k])), repr(float(self.t1_s[k])), dc_names[d], JOB_TYPES[jt],
+                                        self.fields[i], int(self.n[k, i, d, jt]), repr(float(self.mean[k, i, d, jt])),
+                                        repr(float(self.std[k, i, d, jt])), repr(float(self.min[k, i, d, jt]))]
+                                       + [repr(float(self.quantiles[j, k, i, d, jt])) for j in range(len(self.q))]
+                                       + [repr(float(self.max[k, i, d, jt]))])
+            head = [repr(0.0), repr(float(self.end_time))]
+            blank = [""] * len(self.q) + [""]
+            for d in range(D):
+                for jt in range(J):
+                    jobs = float(self.jobs[d, jt])
+                    w.writerow(head + [dc_names[d], JOB_TYPES[jt], "energy_j", int(jobs),
+                                       repr(float(self.energy_sum[d, jt]) / jobs if jobs else nan), "", ""]
+                               + [repr(float(v)) for v in self.energy_quantiles(d, jt)] + [""])
+                    shares = self.mix_shares(d, jt)
+                    for gi, qi, lab in self.mix_labels(d):
+                        w.writerow(head + [dc_names[d], JOB_TYPES[jt], "mix_" + lab, int(self.mix[d, jt, gi, qi]),
+                                           repr(float(shares[gi, qi])), "", ""] + blank)
+                    w.writerow(head + [dc_names[d], JOB_TYPES[jt], "mix_off_level", int(self.off_level[d, jt]),
+                                       repr(float(self.off_level[d, jt]) / jobs if jobs else nan), "", ""] + blank)
+
+
+def _res_levels(sp) -> np.ndarray:
+    lv = np.full((sp.n_dc, RES_MAX_FREQ), np.nan)
+    for d in range(sp.n_dc):
+        lv[d, :sp.dc[d].n_freq] = [sp.dc[d].freq_levels[q] for q in range(sp.dc[d].n_freq)]
+    return lv
+
+
+def res_finalize(mom, m2, hist, n_dc: int, G: int, levels, bin_s: float, end_time: float,
+                 quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobResourcesResult:
+    """All-reduced moments [4, columns] (windowed, then the counts), m2 and histograms over the windowed columns ->
+    statistics."""
+    F, J = len(RES_FIELDS), 2
+    mom = np.asarray(mom, dtype=np.float64)
+    mix_cols = G * RES_MAX_FREQ + 1
+    win = mom.shape[1] - n_dc * J * (mix_cols + RES_EBINS)
+    rows = win // (F * n_dc * J)
+    shape = (rows, F, n_dc, J)
+    st = column_stats(mom[:, :win], np.asarray(m2)[:win], np.asarray(hist)[:win], _res_integral(win, n_dc), quantiles)
+    s4 = mom[1, :win].reshape(shape)[-1]               # whole-run sums over the valid replicas
+    mix = np.rint(mom[1, win:win + n_dc * J * mix_cols]).astype(np.uint64).reshape(n_dc, J, mix_cols)
+    eh = np.rint(mom[1, win + n_dc * J * mix_cols:]).astype(np.uint64).reshape(n_dc, J, RES_EBINS)
+    k = np.arange(rows - 1, dtype=np.float64)
+    return JobResourcesResult(t0_s=np.append(k * bin_s, 0.0), t1_s=np.append((k + 1.0) * bin_s, float(end_time)),
+                              bin_s=float(bin_s), end_time=float(end_time), fields=RES_FIELDS, **st.result_fields(shape),
+                              levels=np.asarray(levels, dtype=np.float64), jobs=eh.sum(axis=-1), gpu_sum=s4[0],
+                              freq_sum=s4[1], energy_sum=s4[2], mix=mix[:, :, :-1].reshape(n_dc, J, G, RES_MAX_FREQ),
+                              off_level=mix[:, :, -1].copy(), energy_histogram=eh)
+
+
+def job_resources(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobResourcesResult:
+    """Statistics of the job-resources recorder of ``engine`` (a finished BatchedEngine with enable_job_resources()),
+    over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
+    import torch
+    from .engine import jres_mix_g
+    if not engine.job_resources_enabled:
+        raise RuntimeError("job resources not enabled (enable_job_resources)")
+    dev = torch.device("cuda", engine.device)
+    sp = engine.spec
+    G = jres_mix_g(sp.max_gpus_per_job)
+    win = (engine.job_ensemble_windows + 1) * len(RES_FIELDS) * sp.n_dc * 2
+    cols = win + sp.n_dc * 2 * (G * RES_MAX_FREQ + 1 + RES_EBINS)
+    passes = device_passes(dev, cols, engine.job_resources_moments_into, engine.job_resources_spread_into, stat_cols=win)
+    return res_finalize(*passes, sp.n_dc, G, _res_levels(sp), engine.job_ensemble_bin, sp.end_time, quantiles)
+
+
+def job_resources_from_rows(rows: np.ndarray, mix: np.ndarray, off_level: np.ndarray, hist: np.ndarray, jobs: np.ndarray,
+                            status: np.ndarray, levels, bin_s: float, end_time: float,
+                            quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobResourcesResult:
+    """The same statistics from host arrays in the layout of BatchedEngine.job_resources_rows — rows [W + 1, 3, n_dc, 2,
+    R], mix [n_dc, 2, G, RES_MAX_FREQ, R], off_level [n_dc, 2, R], hist [n_dc, 2, RES_EBINS, R] — the job ensemble's
+    counts [W + 1, n_dc, 2, R] (job_ensemble_rows()[0][:, 0]) and the levels [n_dc, RES_MAX_FREQ] (NaN past a DC's
+    n_freq), through the numpy mirror of both passes; replicas with status != 0 are left out.  All-reduced over the
+    ranks like job_resources."""
+    n_dc, G, R = rows.shape[2], mix.shape[2], rows.shape[-1]
+    stored = np.concatenate([np.asarray(mix).reshape(n_dc, 2, G * RES_MAX_FREQ, R),
+                             np.asarray(off_level).reshape(n_dc, 2, 1, R)], axis=2)
+    x, ok = _res_columns(rows, stored, hist, jobs, status)
+    win = rows.shape[0] * len(RES_FIELDS) * n_dc * 2
+    passes = host_passes(x, ok, _res_integral(win, n_dc), win)
+    return res_finalize(*passes, n_dc, G, levels, bin_s, end_time, quantiles)
+
+
 # ---- power profile ---------------------------------------------------------------------------------------------------
 PP_FIELDS = ("profile_s", "peak_w", "t_peak_s", "over_s", "over_j", "excursions", "longest_over_s", "out_of_range")
 PP_INTEGER_FIELDS = (5, 7)                             # excursions, out_of_range: unit bins, exact quantiles

@@ -65,11 +65,17 @@ def parse_args(argv=None):
                    help="write, per finish window and for the whole run, statistics of every DC's job counts and mean "
                         "latencies per job type over all replicas (long format), and per-DC latency quantiles, to this file")
     p.add_argument("--job-ensemble-bin", type=float, default=None, metavar="SECONDS",
-                   help="finish-window width of --job-ensemble-csv and --job-waits-csv (default: --log-interval)")
+                   help="finish-window width of --job-ensemble-csv, --job-waits-csv and --job-resources-csv (default: "
+                        "--log-interval)")
     p.add_argument("--job-waits-csv", type=str, default=None, metavar="PATH",
                    help="write, per finish window and for the whole run, statistics of every DC's jobs that waited, mean "
                         "wait (start - xfer_done) and mean response time (finish - arrival) per job type over all "
                         "replicas (the --job-ensemble-csv format), and per-DC wait and response quantiles, to this file")
+    p.add_argument("--job-resources-csv", type=str, default=None, metavar="PATH",
+                   help="write, per finish window and for the whole run, statistics of every DC's mean GPUs, mean "
+                        "frequency and mean predicted energy (E_pred * size) per finished job and job type over all "
+                        "replicas (the --job-ensemble-csv format), per-DC energy-per-job quantiles and the pooled "
+                        "(GPU count, frequency) mix, to this file")
     p.add_argument("--occupancy-csv", type=str, default=None, metavar="PATH",
                    help="write batch statistics of every DC's time-averaged queue lengths and running jobs, longest "
                         "queues and shares of time queued / saturated / idle, measured between every two events, and "
@@ -127,7 +133,8 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
         job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
         power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None,
-        occupancy=args.occupancy_csv is not None, tail_latency=args.tail_latency_csv is not None)
+        occupancy=args.occupancy_csv is not None, tail_latency=args.tail_latency_csv is not None,
+        job_resources=args.job_resources_csv is not None)
     return sim
 
 
@@ -168,6 +175,7 @@ def main(argv=None):
     _add_job_waits(stats, sim.job_waits)
     _add_occupancy(stats, sim.occupancy, sim)
     _add_tail_latency(stats, sim.tail_latency)
+    _add_job_resources(stats, sim.job_resources, sim)
     _report(args, stats)
     return sim
 
@@ -185,6 +193,8 @@ def _write_ensemble(args, sim):
         sim.occupancy.to_csv(args.occupancy_csv, [dc.name for dc in sim.dcs.values()])
     if args.tail_latency_csv:
         sim.tail_latency.to_csv(args.tail_latency_csv, [dc.name for dc in sim.dcs.values()])
+    if args.job_resources_csv:
+        sim.job_resources.to_csv(args.job_resources_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -223,6 +233,14 @@ def _add_tail_latency(stats, res):
     the mean / p05 / p50 / p95 over the runs of the per-run p99."""
     if res is not None:
         stats["tail_latency"] = res.pooled()
+
+
+def _add_job_resources(stats, res, sim):
+    """Per DC and job type, for --summary-json: pooled jobs, mean GPUs / frequency / predicted energy per job, energy
+    quantiles and the (GPU count, frequency) mix as shares."""
+    if res is not None:
+        names = [dc.name for dc in sim.dcs.values()]
+        stats["job_resources"] = {names[d]: v for d, v in res.pooled().items()}
 
 
 def _add_latency_quantiles(stats, hist):
@@ -271,6 +289,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--occupancy-csv needs at least one replica per rank")
     if args.tail_latency_csv and count == 0:
         raise SystemExit("--tail-latency-csv needs at least one replica per rank")
+    if args.job_resources_csv and count == 0:
+        raise SystemExit("--job-resources-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -308,6 +328,7 @@ def _main_sharded(args, world, rank):
         _add_job_waits(stats, sim.job_waits)
         _add_occupancy(stats, sim.occupancy, sim)
         _add_tail_latency(stats, sim.tail_latency)
+        _add_job_resources(stats, sim.job_resources, sim)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -334,6 +355,9 @@ def _main_compare(args, world, rank):
     if args.tail_latency_csv:
         raise SystemExit("--tail-latency-csv is not available with --compare-algos (run each algo on its own for its "
                          "per-run tail latency)")
+    if args.job_resources_csv:
+        raise SystemExit("--job-resources-csv is not available with --compare-algos (run each algo on its own for its "
+                         "GPU, frequency and energy-per-job statistics)")
     if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
         raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
                          "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")

@@ -62,7 +62,7 @@ class MultiIngressPaperSimulator:
                  cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
                  job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None, power_profile: bool = False,
                  power_threshold: Optional[float] = None, job_waits: bool = False, occupancy: bool = False,
-                 tail_latency: bool = False):
+                 tail_latency: bool = False, job_resources: bool = False):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -124,6 +124,12 @@ class MultiIngressPaperSimulator:
         # whose p99 met sla_p99_ms, ensemble.TailLatencyResult
         self._want_tail_latency = bool(tail_latency)
         self.tail_latency = None
+        # job_resources=True: after run(), per finish window of job_ensemble_bin seconds and for the whole run, statistics
+        # of every finished job's GPU count, frequency and predicted energy E_pred * size over all replicas (all ranks, as
+        # above), the pooled (n, f) mix and energy-per-job quantiles, ensemble.JobResourcesResult.  It runs the job
+        # ensemble's recorder too (its windows and job counts)
+        self._want_job_resources = bool(job_resources)
+        self.job_resources = None
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -178,6 +184,7 @@ class MultiIngressPaperSimulator:
                                           job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
                                           power_threshold=self._power_threshold, job_waits=self._want_job_waits,
                                           occupancy=self._want_occupancy, tail_latency=self._want_tail_latency,
+                                          job_resources=self._want_job_resources,
                                           tail_sla_s=float(self.sla_p99_ms) / 1000.0)
         except BaseException:
             if companion is not None:
@@ -205,6 +212,9 @@ class MultiIngressPaperSimulator:
             if self._want_tail_latency:
                 from ..ensemble import tail_latency
                 self.tail_latency = tail_latency(eng)
+            if self._want_job_resources:
+                from ..ensemble import job_resources
+                self.job_resources = job_resources(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

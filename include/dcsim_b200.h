@@ -440,6 +440,61 @@ int dcsim_job_waits_spread(dcsim_t* h, const double* dev_mean, const double* dev
  * (synchronises). */
 int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
+/* Job resources (beside the job-log ensemble, in its cells): what every finished job (the set the job ensemble counts)
+ * ran on and what the model predicted it would cost.  For a job of DC d with GPU count g (job_log.csv n_gpus), frequency
+ * f (its f_used: the frequency of its running record at finish, SIM:713-716, the value job_log.csv writes) and size:
+ *   E_job = E_pred * size,  E_pred = P_pred * T_pred = task_power_w(g, f) * step_time_s(g, f)   [J]
+ * (SIM:715-716, policy_paper.py:7-16; the oracle's product order, oracle/dcsim_oracle.c:696).
+ * Windowed, per replica and cell (the job ensemble's window k and row W, DC, job type), added in finish order:
+ * GPU_SUM (sum of g), FREQ_SUM (sum of f [GHz]), ENERGY_SUM (sum of E_job [J]).  Device layout
+ * [W + 1][DCSIM_JRES_STORED][n_dc][2 jtypes][n_replicas] doubles, replica fastest.
+ * Whole run, per replica, DC d and job type, u32 counts of the finished jobs:
+ *   MIX      [DCSIM_JRES_MIX_COLS(G)]: column (min(g, G) - 1) * DCSIM_MAX_FREQ + q for f == freq_levels_d[q] (exact
+ *            equality, q < n_freq_d: the match dcsim_bandit_update makes), G = DCSIM_JRES_G(max_gpus_per_job), and a last
+ *            column OFF_LEVEL = G * DCSIM_MAX_FREQ for an f that matches no level;
+ *   E_HIST   [DCSIM_JRES_EBINS]: quarter-octave bins of E_job anchored at 1 J, bin = clamp(floor(4 * log2(E_job)), 0,
+ *            127), decided exactly (DCSIM_JRES_OCT1..3 are the smallest doubles >= 2^(1/4), 2^(1/2), 2^(3/4)).
+ * Device layouts [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] and [n_dc][2][DCSIM_JRES_EBINS][n_replicas] u32.
+ * Bytes per replica: 8 * (W + 1) * 3 * 2 * n_dc + 4 * 2 * n_dc * (MIX_COLS(G) + 128); the bench workload (4 DCs,
+ * max_gpus_per_job 8, 120 s in 5 s windows: W = 24) 13 024 B, 854 MB at 65 536 replicas.
+ * The reductions' columns: first (row, field, dc, jtype) over DCSIM_JRES_FIELDS fields — the three stored sums over every
+ * valid replica, then MEAN_GPUS = GPU_SUM / JOBS, MEAN_FREQ = FREQ_SUM / JOBS and MEAN_ENERGY = ENERGY_SUM / JOBS over
+ * the replicas with JOBS > 0 in the cell (JOBS from the job ensemble) — then the mix and the energy bins as stored. */
+enum {
+  DCSIM_JRES_GPU_SUM = 0,     /* sum of the GPU counts of the cell's finished jobs */
+  DCSIM_JRES_FREQ_SUM = 1,    /* sum of their frequencies [GHz] */
+  DCSIM_JRES_ENERGY_SUM = 2,  /* sum of their E_job [J] */
+  DCSIM_JRES_STORED = 3,      /* fields the recorder stores per replica */
+  DCSIM_JRES_MEAN_GPUS = 3,   /* GPU_SUM / JOBS (reductions only) */
+  DCSIM_JRES_MEAN_FREQ = 4,   /* FREQ_SUM / JOBS (reductions only) */
+  DCSIM_JRES_MEAN_ENERGY = 5, /* ENERGY_SUM / JOBS (reductions only) */
+  DCSIM_JRES_FIELDS = 6       /* fields of the reductions' windowed columns */
+};
+#define DCSIM_JRES_MAX_G 32
+#define DCSIM_JRES_G(max_gpus_per_job) ((max_gpus_per_job) < 1 ? 1 : ((max_gpus_per_job) > DCSIM_JRES_MAX_G ? DCSIM_JRES_MAX_G : (max_gpus_per_job)))
+#define DCSIM_JRES_MIX_COLS(G) ((G) * DCSIM_MAX_FREQ + 1)
+#define DCSIM_JRES_EBINS 128
+#define DCSIM_JRES_OCT1 0x1.306fe0a31b716p+0
+#define DCSIM_JRES_OCT2 0x1.6a09e667f3bcdp+0
+#define DCSIM_JRES_OCT3 0x1.ae89f995ad3aep+0
+/* Opt-in, after dcsim_enable_job_ensemble and before the first advance of a batch (stays on across dcsim_reset, zeroed
+ * by it; a later dcsim_enable_job_ensemble with another bin_s switches it off).  The running-job records then carry the
+ * size and frequency (the layout job_log.csv uses).  DCSIM_E_STATE without the job ensemble, after the first advance or
+ * on a member of a shared group; DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the buffers do not fit. */
+int dcsim_enable_job_resources(dcsim_t* h);
+/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas]
+ * doubles, `mix` [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] u32, `hist` [n_dc][2][DCSIM_JRES_EBINS][n_replicas] u32.
+ * Any may be NULL; a buffer smaller than its array is DCSIM_E_INVALID. */
+int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* mix, size_t mix_bytes, uint32_t* hist,
+                              size_t hist_bytes);
+/* Pass 1 over every column, (W + 1) * DCSIM_JRES_FIELDS * n_dc * 2 windowed, then n_dc * 2 * (MIX_COLS(G) + EBINS)
+ * counts: dev_out = [4][columns] {n, sum, min, max}; the count columns' sums are the pooled mix and energy histogram.
+ * Pass 2 over the windowed columns only: the contract of dcsim_job_ensemble_spread, GPU_SUM the integer field.  Replicas with
+ * status 0 count.  Both on the handle's stream, with device pointers. */
+int dcsim_job_resources_moments(dcsim_t* h, double* dev_out);
+int dcsim_job_resources_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                               double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Power profile: for EVERY replica, the cluster power P(t) its total energy integrates, as a step function, and what a
  * site is sized by — peak, time and energy over a threshold, a time-weighted power histogram.
  *   - Each inter-event interval (t_{k-1}, t_k] of positive length has power sum_d P_d, summed in DC order from 0.0,

@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy / tail, the job-log ensemble / the
-power profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder / the per-run tail-latency
-recorder) at bench size: the event loop with the recorder off and on, the two reduction kernels, the recorder's bytes per
+"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy / tail / resources, the job-log
+ensemble / the power profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder / the per-run
+tail-latency recorder / the job-resources recorder on top of the job ensemble) at bench size: the event loop with the recorder off and on, the two reduction kernels, the recorder's bytes per
 replica.  One JSON line on stdout; writes nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy|tail] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy|tail|resources] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
@@ -30,7 +30,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail", "resources"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -47,10 +47,10 @@ def main():
 
     def make(arm):
         e = BatchedEngine(sp, n, base_seed=seed, cuda_stream=stream.cuda_stream)
-        if args.recorder == "waits":            # the waits' own cost: both arms run the job ensemble they need
+        if args.recorder in ("waits", "resources"):  # their own cost: both arms run the job ensemble they need
             e.enable_job_ensemble()
             if arm == "on":
-                e.enable_job_waits()
+                e.enable_job_waits() if args.recorder == "waits" else e.enable_job_resources()
         elif arm == "on" and args.recorder == "job":
             e.enable_job_ensemble()
         elif arm == "on" and args.recorder == "power":
@@ -101,6 +101,14 @@ def main():
                 fin = summ[:, S.S_FIN_INF if jt == 0 else S.S_FIN_TRN].sum()
                 lat = summ[:, S.S_LAT_SUM_INF if jt == 0 else S.S_LAT_SUM_TRN].sum()
                 stats[name]["mean_service_s"] = float(lat / fin) if fin else float("nan")
+        elif args.recorder == "resources":
+            win = on.job_ensemble_windows + 1
+            G = min(max(sp.max_gpus_per_job, 1), 32)
+            counts = sp.n_dc * 2 * (G * EN.RES_MAX_FREQ + 1 + EN.RES_EBINS)
+            cols = win * len(EN.RES_FIELDS) * sp.n_dc * 2 + counts
+            moments_into, spread_into = on.job_resources_moments_into, on.job_resources_spread_into
+            rows, recorder_bytes = win, win * 3 * sp.n_dc * 2 * 8 + counts * 4
+            stats = EN.job_resources(on).pooled()
         elif args.recorder == "job":
             cols = (on.job_ensemble_windows + 1) * len(EN.JOB_FIELDS) * sp.n_dc * 2
             moments_into, spread_into = on.job_ensemble_moments_into, on.job_ensemble_spread_into
@@ -149,6 +157,7 @@ def main():
                       "rows": rows, "bytes_per_replica": recorder_bytes, "bytes_total": recorder_bytes * n,
                       "moments_ms": moments_ms, "spread_ms": spread_ms,
                       **({"waits": stats} if args.recorder == "waits" else {}),
+                      **({"resources": stats} if args.recorder == "resources" else {}),
                       **({"selection_ms": first_moments_ms - moments_ms, "tail": stats} if args.recorder == "tail" else {})}),
           flush=True)
 
