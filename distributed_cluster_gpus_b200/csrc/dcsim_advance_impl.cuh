@@ -94,8 +94,7 @@ int DCSIM_ADV(dcsim_adv_min_ctas)(void) { return DCSIM_MIN_CTAS_PER_SM; }
  * instantiation with the profile recorders when P->pp, P->occ, P->tail or P->jres is set. */
 cudaError_t DCSIM_ADV(dcsim_adv_launch)(const dcsim_kparams_t* P, unsigned long long* events, int cap, int mode, int ctas, int threads,
                                         int smem, cudaStream_t stream) {
-  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, P->pp != nullptr || P->occ != nullptr || P->tail != nullptr ||
-                                           P->jres != nullptr)<<<ctas, threads, smem, stream>>>(*P, events);
+  DCSIM_ADV(dcsim_pick_kernel)(cap != 0, mode, dcsim_profile_recorders(P))<<<ctas, threads, smem, stream>>>(*P, events);
   return cudaGetLastError();
 }
 

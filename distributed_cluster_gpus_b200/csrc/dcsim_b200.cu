@@ -869,11 +869,11 @@ static cudaError_t size_launch(dcsim_t* h) {
   return cudaSuccess;
 }
 
-/* job_log.csv needs size / f / jid in the running records, the waiting-time and tail-latency recorders the jid;
- * switching them on or off re-lays the state block out. */
+/* job_log.csv and some recorders need job fields in the running records (dcsim_job_fields); switching them on or off
+ * re-lays the state block out. */
 static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
-  dcsim_make_layout(&h->spec, &L, job_log || h->d_jwait != NULL || h->d_tail != NULL || h->d_jres != NULL);
+  dcsim_make_layout(&h->spec, &L, dcsim_job_fields(job_log, h->d_jwait, h->d_tail, h->d_jres));
   if (L.lean == h->L.lean) return DCSIM_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
@@ -909,16 +909,12 @@ int dcsim_create(const void* spec_blob, size_t spec_bytes, uint64_t n_replicas, 
   g->spec = sp;
   g->n_replicas = n_replicas;
   g->seed0 = base_seed + first_replica_id;
-  g->cap_arr = (uint32_t)(sp.cap_arrivals > 0 ? sp.cap_arrivals : 16384);
-  for (int i = 0; i < sp.n_ing; ++i)
-    for (int d = 0; d < sp.n_dc; ++d)
-      for (int jt = 0; jt < 2; ++jt) {
-        const double v = sp.transfer_s[i][d][jt];
-        if (v == v && v < 1e300 && v > g->max_transfer) g->max_transfer = v; /* finite ones only */
-      }
+  g->cap_arr = dcsim_cap_arr(&sp);
 #ifdef DCSIM_TEST_HOOKS
   g->test_quantum = g_test_time_quantum;
-  g->max_transfer += g->test_quantum; /* a rounded-up xfer_done instant may lie up to one quantum past t + transfer_s */
+  g->max_transfer = dcsim_max_transfer(&sp, g->test_quantum);
+#else
+  g->max_transfer = dcsim_max_transfer(&sp, 0.0);
 #endif
 
 #define GROUP_TRY(call)                                                                   \
@@ -1146,9 +1142,7 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->n_replicas = h->n_replicas;
   P->seed0 = h->g->seed0;
   P->max_events = max_events;
-  P->budget32 = (max_events == 0ull || max_events > 0xfffffffeull) ? 0xffffffffu : (uint32_t)max_events;
   P->state = h->d_state; P->queues = h->d_queues; P->summary = h->d_summary;
-  P->end_eps = h->spec.end_time + 1e-9; /* SIM:161 */
   P->arr_t = h->g->d_arr_t; P->arr_raw = h->g->d_arr_raw; P->arr_meta = h->g->d_arr_meta; P->arr_pred = h->g->d_arr_pred;
   P->arr_tx = h->g->d_arr_tx; P->arr_fin = h->g->d_arr_fin;
   P->ml_t = h->g->d_ml_t; P->ml_aux = h->g->d_ml_aux; P->ml_meta = h->g->d_ml_meta;
@@ -1159,13 +1153,12 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->ens = h->d_ens; P->ens_cap = h->ens_cap;
   P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
   P->tail = h->d_tail; P->tail_cols = h->d_tail_cols; P->tail_sla = h->tail_sla;
-  P->finish_rec = (P->lat_hist || P->jens || P->tail) ? 1u : 0u;
   P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
-  P->pp_hi = h->d_pp ? dcsim_pp_range(&h->spec) : 0.0;
   P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
   P->occ = h->d_occ; P->occ_work = h->d_occ_work;
   P->jres = h->d_jres; P->jres_mix = h->d_jres_cnt;
   P->jres_hist = h->d_jres ? h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas : NULL;
+  dcsim_derive_kparams(P);
 }
 
 /* A member whose batch was set up for an earlier generation of the group's lists must be reset first. */

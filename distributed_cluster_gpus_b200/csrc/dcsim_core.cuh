@@ -75,6 +75,19 @@ static inline bool dcsim_event_any_full(bool p) { return p; }
 static inline void dcsim_sync_full() {}
 static inline uint32_t dcsim_event_bcast_u32(uint32_t x, int) { return x; }
 static inline uint32_t dcsim_event_pick_u32(bool, uint32_t v) { return v; }
+/* the CUDA intrinsics and atomics the shared code calls, for one thread (an atomic is a plain read-modify-write), so
+ * that code has one body for both builds */
+static inline double __hiloint2double(int hi, int lo) {
+  const uint64_t u = ((uint64_t)(uint32_t)hi << 32) | (uint64_t)(uint32_t)lo; double x; memcpy(&x, &u, 8); return x;
+}
+static inline double atomicAdd(double* a, double v) { const double o = *a; *a = o + v; return o; }
+static inline uint32_t atomicAdd(uint32_t* a, uint32_t v) { const uint32_t o = *a; *a = o + v; return o; }
+static inline unsigned long long atomicMin(unsigned long long* a, unsigned long long v) { const unsigned long long o = *a; if (v < o) *a = v; return o; }
+static inline unsigned long long atomicMax(unsigned long long* a, unsigned long long v) { const unsigned long long o = *a; if (v > o) *a = v; return o; }
+static inline void dcsim_tail_sync() {}
+static inline unsigned long long dcsim_tail_bits(double x) { unsigned long long u; memcpy(&u, &x, 8); return u; }
+static inline double dcsim_tail_double(unsigned long long u) { double x; memcpy(&x, &u, 8); return x; }
+static inline int dcsim_tail_clz64(unsigned long long x) { return __builtin_clzll(x); }
 #define DCSIM_INF (__builtin_inf())
 #else
 #define DCSIM_DEV __device__ __forceinline__
@@ -178,30 +191,23 @@ DCSIM_DEV uint32_t dcsim_event_pick_u32(bool mine, uint32_t v) { /* dcsim_pick_u
   return dcsim_event_min_u32(mine ? v : 0xffffffffu);
 #endif
 }
+/* the tail-latency selection pass (one CTA per replica) */
+__device__ __forceinline__ void dcsim_tail_sync() { __syncthreads(); }
+__device__ __forceinline__ unsigned long long dcsim_tail_bits(double x) { return (unsigned long long)__double_as_longlong(x); }
+__device__ __forceinline__ double dcsim_tail_double(unsigned long long u) { return __longlong_as_double((long long)u); }
+__device__ __forceinline__ int dcsim_tail_clz64(unsigned long long x) { return __clzll((long long)x); }
 #define DCSIM_INF (__longlong_as_double(0x7ff0000000000000LL))
 #endif
 
 DCSIM_DEV double dcsim_hilo_f64(uint32_t hi, uint32_t lo) {
-#ifdef DCSIM_HOST_EMU
-  const uint64_t u = ((uint64_t)hi << 32) | (uint64_t)lo; double x; memcpy(&x, &u, 8); return x;
-#else
   return __hiloint2double((int)hi, (int)lo);
-#endif
 }
 
 DCSIM_DEV double dcsim_bcast_f64(double x, int src) {
-#ifdef DCSIM_HOST_EMU
-  (void)src; return x;
-#else
   return __hiloint2double((int)dcsim_bcast_u32(dcsim_hi(x), src), (int)dcsim_bcast_u32(dcsim_lo(x), src));
-#endif
 }
 DCSIM_DEV double dcsim_event_bcast_f64(double x, int src) {
-#ifdef DCSIM_HOST_EMU
-  (void)src; return x;
-#else
   return __hiloint2double((int)dcsim_event_bcast_u32(dcsim_hi(x), src), (int)dcsim_event_bcast_u32(dcsim_lo(x), src));
-#endif
 }
 
 /* Histogram bin of a positive latency: 4 bins per octave from 2^-20 s, from the IEEE exponent and the top two
@@ -230,11 +236,7 @@ DCSIM_DEV int dcsim_lat_bin(double lat) {
 /* One count into replica r's [2][DCSIM_LAT_BINS] histogram in HBM — fire-and-forget, nothing waits for it. */
 DCSIM_COLD void dcsim_hist_add(uint32_t* hist, uint64_t r, int jt, double lat) {
   uint32_t* cell = hist + r * (uint64_t)(2 * DCSIM_LAT_BINS) + (uint32_t)(jt * DCSIM_LAT_BINS + dcsim_lat_bin(lat));
-#ifdef DCSIM_HOST_EMU
-  *cell += 1u;
-#else
   atomicAdd(cell, 1u);
-#endif
 }
 
 /* ---- candidate slots (the event set, one slot per lane) -------------------------------------- */
@@ -414,6 +416,30 @@ static inline void dcsim_make_layout(const dcsim_spec_t* sp, dcsim_layout_t* L, 
   L->queue_bytes = (uint64_t)sp->n_dc * ((uint64_t)L->cap_q[0] + (uint64_t)L->cap_q[1]) * 16ull;
 }
 
+/* Host-side launch-parameter rules, shared by the library and the host build of the core. */
+/* The `job_log` argument of dcsim_make_layout: job_log.csv needs size / f / jid in the running records, the waiting-time
+ * and tail-latency recorders the jid, the job-resources recorder size and f. */
+static inline int dcsim_job_fields(int job_log, const void* jwait, const void* tail, const void* jres) {
+  return (job_log || jwait || tail || jres) ? 1 : 0;
+}
+/* Arrival slots per replica. */
+static inline uint32_t dcsim_cap_arr(const dcsim_spec_t* sp) {
+  return (uint32_t)(sp->cap_arrivals > 0 ? sp->cap_arrivals : 16384);
+}
+/* The largest finite transfer_s of the scenario, plus the tie hook's quantum (0 outside the tests): a rounded-up
+ * xfer_done instant may lie up to one quantum past t + transfer_s. */
+static inline double dcsim_max_transfer(const dcsim_spec_t* sp, double quantum) {
+  double max_transfer = 0.0;
+  for (int i = 0; i < sp->n_ing; ++i)
+    for (int d = 0; d < sp->n_dc; ++d)
+      for (int jt = 0; jt < 2; ++jt) {
+        const double v = sp->transfer_s[i][d][jt];
+        if (v == v && v < 1e300 && v > max_transfer) max_transfer = v; /* finite ones only */
+      }
+  max_transfer += quantum;
+  return max_transfer;
+}
+
 /* One FIFO entry in HBM: the part of a Job that survives queueing (models.py:5-27). */
 struct alignas(16) dcsim_qent_t {
   double size;
@@ -453,7 +479,7 @@ struct dcsim_kparams_t {
   uint64_t seed0;       /* Philox key of local replica 0 (base_seed + first_replica_id) */
   uint64_t max_events;  /* per replica per launch; 0 = run to the end */
   uint32_t budget32;    /* the same as one 32-bit compare: 0 (unlimited) and anything >= 2^32 become 0xffffffff (host-computed) */
-  uint32_t finish_rec;  /* lat_hist or jens is set: the finish handler's one test for both opt-in recorders */
+  uint32_t finish_rec;  /* lat_hist, jens or tail is set: the finish handler's one test for the opt-in recorders */
   char* state;          /* [n_replicas][L.total_bytes] */
   char* queues;         /* [n_replicas][L.queue_bytes] */
   double* summary;      /* [n_replicas][DCSIM_SUMMARY_K] */
@@ -1462,6 +1488,18 @@ static inline double dcsim_pp_range(const dcsim_spec_t* sp) {
   return total > 0.0 ? total : 1.0;
 }
 
+/* Host code: the fields of a launch's parameters derived from its spec, max_events and recorder pointers (set first). */
+static inline void dcsim_derive_kparams(dcsim_kparams_t* P) {
+  P->budget32 = (P->max_events == 0ull || P->max_events > 0xfffffffeull) ? 0xffffffffu : (uint32_t)P->max_events;
+  P->end_eps = P->spec.end_time + 1e-9; /* SIM:161 */
+  P->finish_rec = (P->lat_hist || P->jens || P->tail) ? 1u : 0u;
+  P->pp_hi = P->pp ? dcsim_pp_range(&P->spec) : 0.0;
+}
+/* Host code: the launch runs the instantiation with the profile recorders (dcsim_replica_step<..., PP = true>). */
+static inline bool dcsim_profile_recorders(const dcsim_kparams_t* P) {
+  return P->pp != nullptr || P->occ != nullptr || P->tail != nullptr || P->jres != nullptr;
+}
+
 DCSIM_DEV bool dcsim_same_bits(double a, double b) { return dcsim_hi(a) == dcsim_hi(b) && dcsim_lo(a) == dcsim_lo(b); }
 
 /* Level [s, e] of power p closes: its histogram bin (a fire-and-forget RED; one writer per replica, so each bin is the
@@ -1472,11 +1510,7 @@ DCSIM_DEV void dcsim_pp_close(const dcsim_kparams_t* P, double* w, uint32_t r, d
   int b = f >= (double)(DCSIM_PP_BINS - 1) ? DCSIM_PP_BINS - 1 : (f > 0.0 ? (int)f : 0);
   if (!(p >= 0.0 && p <= hi)) w[DCSIM_PPW_OOR] += 1.0;
   double* cell = P->pp + (uint64_t)(DCSIM_PP_FIELDS + P->spec.n_dc + b) * P->n_replicas + r;
-#ifdef DCSIM_HOST_EMU
-  *cell += len;
-#else
   atomicAdd(cell, len);
-#endif
   if (w[DCSIM_PPW_LEVELS] == 0.0 || p > w[DCSIM_PPW_PEAK]) { w[DCSIM_PPW_PEAK] = p; w[DCSIM_PPW_T_PEAK] = s; }
   w[DCSIM_PPW_LEVELS] += 1.0;
   const double thr = P->pp_threshold;
@@ -1584,11 +1618,7 @@ DCSIM_DEV void dcsim_occ_close(const dcsim_kparams_t* P, uint32_t r, int d, int 
 #undef DCSIM_OCC_SUM
   if (bin >= 0) {
     double* cell = o + (uint64_t)(1 + bin) * n;
-#ifdef DCSIM_HOST_EMU
-    *cell += len;
-#else
     atomicAdd(cell, len);
-#endif
   }
 }
 
@@ -1949,15 +1979,9 @@ DCSIM_COLD void dcsim_jens_add(const dcsim_kparams_t* P, uint32_t r, int d, int 
   double* all = P->jens + W * (DCSIM_JENS_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
   uint32_t* cell = P->jens_hist + ((uint64_t)r * (uint64_t)P->spec.n_dc + (uint64_t)d) * (2 * DCSIM_LAT_BINS) +
                    (uint32_t)(jt * DCSIM_LAT_BINS + dcsim_lat_bin(lat));
-#ifdef DCSIM_HOST_EMU
-  win[DCSIM_JENS_JOBS * fs] += 1.0; win[DCSIM_JENS_LAT_SUM * fs] += lat;
-  all[DCSIM_JENS_JOBS * fs] += 1.0; all[DCSIM_JENS_LAT_SUM * fs] += lat;
-  *cell += 1u;
-#else
   atomicAdd(win + DCSIM_JENS_JOBS * fs, 1.0); atomicAdd(win + DCSIM_JENS_LAT_SUM * fs, lat);
   atomicAdd(all + DCSIM_JENS_JOBS * fs, 1.0); atomicAdd(all + DCSIM_JENS_LAT_SUM * fs, lat);
   atomicAdd(cell, 1u);
-#endif
 }
 
 /* Waiting and response times (opt-in: P->jwait, on top of P->jens): the job of running record i (at `rec`, the base of
@@ -1978,19 +2002,11 @@ DCSIM_COLD void dcsim_jwait_add(const dcsim_kparams_t* P, uint32_t r, int d, int
   double* all = P->jwait + W * (DCSIM_JWAIT_STORED * fs) + (uint64_t)(2 * d + jt) * n + r;
   uint32_t* cell = P->jwait_hist + ((uint64_t)r * (uint64_t)P->spec.n_dc + (uint64_t)d) * (4 * DCSIM_LAT_BINS) +
                    (uint32_t)(jt * DCSIM_LAT_BINS);
-#ifdef DCSIM_HOST_EMU
-  if (wait > 0.0) { win[DCSIM_JWAIT_WAITED * fs] += 1.0; all[DCSIM_JWAIT_WAITED * fs] += 1.0; }
-  win[DCSIM_JWAIT_WAIT_SUM * fs] += wait; win[DCSIM_JWAIT_RESP_SUM * fs] += resp;
-  all[DCSIM_JWAIT_WAIT_SUM * fs] += wait; all[DCSIM_JWAIT_RESP_SUM * fs] += resp;
-  cell[dcsim_lat_bin(wait)] += 1u;
-  cell[2 * DCSIM_LAT_BINS + dcsim_lat_bin(resp)] += 1u;
-#else
   if (wait > 0.0) { atomicAdd(win + DCSIM_JWAIT_WAITED * fs, 1.0); atomicAdd(all + DCSIM_JWAIT_WAITED * fs, 1.0); }
   atomicAdd(win + DCSIM_JWAIT_WAIT_SUM * fs, wait); atomicAdd(win + DCSIM_JWAIT_RESP_SUM * fs, resp);
   atomicAdd(all + DCSIM_JWAIT_WAIT_SUM * fs, wait); atomicAdd(all + DCSIM_JWAIT_RESP_SUM * fs, resp);
   atomicAdd(cell + dcsim_lat_bin(wait), 1u);
   atomicAdd(cell + 2 * DCSIM_LAT_BINS + dcsim_lat_bin(resp), 1u);
-#endif
 }
 
 /* Per-run tail latency (opt-in: P->tail): the job of running record i (at `rec`, the base of the L.rn_* offsets) finished
@@ -2040,17 +2056,11 @@ DCSIM_COLD void dcsim_jres_add(const dcsim_kparams_t* P, uint32_t r, int d, int 
   uint32_t* mix = P->jres_mix + ((uint64_t)(2 * d + jt) * DCSIM_JRES_MIX_COLS(G) + (uint64_t)col) * n + r;
   uint32_t* hist = P->jres_hist + ((uint64_t)(2 * d + jt) * DCSIM_JRES_EBINS + (uint64_t)dcsim_jres_ebin(e_job)) * n + r;
   const double gd = (double)g;
-#ifdef DCSIM_HOST_EMU
-  win[DCSIM_JRES_GPU_SUM * fs] += gd; win[DCSIM_JRES_FREQ_SUM * fs] += f; win[DCSIM_JRES_ENERGY_SUM * fs] += e_job;
-  all[DCSIM_JRES_GPU_SUM * fs] += gd; all[DCSIM_JRES_FREQ_SUM * fs] += f; all[DCSIM_JRES_ENERGY_SUM * fs] += e_job;
-  *mix += 1u; *hist += 1u;
-#else
   atomicAdd(win + DCSIM_JRES_GPU_SUM * fs, gd); atomicAdd(win + DCSIM_JRES_FREQ_SUM * fs, f);
   atomicAdd(win + DCSIM_JRES_ENERGY_SUM * fs, e_job);
   atomicAdd(all + DCSIM_JRES_GPU_SUM * fs, gd); atomicAdd(all + DCSIM_JRES_FREQ_SUM * fs, f);
   atomicAdd(all + DCSIM_JRES_ENERGY_SUM * fs, e_job);
   atomicAdd(mix, 1u); atomicAdd(hist, 1u);
-#endif
 }
 
 /* SIM:701-927 minus RL/elastic branches (lane 0 part, after the record was read and before it is erased). */
@@ -2068,11 +2078,7 @@ DCSIM_DEV void dcsim_finish_account(dcsim_ctx_t& c, int d, int slot) {
   const double lat = now - dcsim_at<double>(c.rec, L.rn_start)[i]; /* SIM:820 */
   H->lat_sum += lat;
   if (jt == DCSIM_JT_INFERENCE) { H->lat_sum_inf += lat; H->n_fin_inf++; } else { H->lat_sum_trn += lat; H->n_fin_trn++; }
-#ifdef DCSIM_HOST_EMU
-  if (c.P->lat_hist || c.P->jens || c.P->tail) { /* (the host builds set the pointers only) */
-#else
   if (__builtin_expect(c.P->finish_rec != 0u, 0)) { /* opt-in recorders: off, they cost this one test */
-#endif
     if (c.P->lat_hist) dcsim_hist_add(c.P->lat_hist, (uint64_t)c.r, jt, lat);
     if (c.P->jens) dcsim_jens_add(c.P, c.r, d, jt, now, lat);
     if (c.P->jwait) dcsim_jwait_add(c.P, c.r, d, jt, now, c.rec, i); /* (only with jens, in the layout keeping the jid) */
@@ -2761,6 +2767,13 @@ DCSIM_DEV void dcsim_write_summary(dcsim_ctx_t& c, double* out) {
  * ghost's blk is replica n-1's live block (see dcsim_ctx_t::quiet). */
 template <bool CAP, bool RECG, bool PP = false, bool INPLACE = false>
 DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char* blk, char* rec, bool fresh, bool ghost = false) {
+#ifdef DCSIM_HOST_EMU
+  /* the host build has no launch of its own: a host driver's parameters get the fields the library derives
+   * (fill_kparams), so the handlers below test what the device tests whatever the driver set */
+  dcsim_kparams_t derived = *P;
+  dcsim_derive_kparams(&derived);
+  P = &derived;
+#endif
   dcsim_ctx_t c;
   c.P = P; c.blk = blk; c.rec = rec; c.H = reinterpret_cast<dcsim_hdr_t*>(blk); c.lane = dcsim_lane();
   c.r = (uint32_t)r; /* n_replicas < 2^32 (checked by dcsim_create) */
@@ -2823,24 +2836,6 @@ struct dcsim_tail_smem_t {
   uint32_t jobs[DCSIM_TAIL_GROUPS_MAX], unfinished[DCSIM_TAIL_GROUPS_MAX];
 };
 
-#ifdef DCSIM_HOST_EMU
-static inline void dcsim_tail_sync() {}
-static inline void dcsim_tail_add_u32(uint32_t* a, uint32_t v) { *a += v; }
-static inline void dcsim_tail_min_u64(unsigned long long* a, unsigned long long v) { if (v < *a) *a = v; }
-static inline void dcsim_tail_max_u64(unsigned long long* a, unsigned long long v) { if (v > *a) *a = v; }
-static inline unsigned long long dcsim_tail_bits(double x) { unsigned long long u; memcpy(&u, &x, 8); return u; }
-static inline double dcsim_tail_double(unsigned long long u) { double x; memcpy(&x, &u, 8); return x; }
-static inline int dcsim_tail_clz64(unsigned long long x) { return __builtin_clzll(x); }
-#else
-__device__ __forceinline__ void dcsim_tail_sync() { __syncthreads(); }
-__device__ __forceinline__ void dcsim_tail_add_u32(uint32_t* a, uint32_t v) { atomicAdd(a, v); }
-__device__ __forceinline__ void dcsim_tail_min_u64(unsigned long long* a, unsigned long long v) { atomicMin(a, v); }
-__device__ __forceinline__ void dcsim_tail_max_u64(unsigned long long* a, unsigned long long v) { atomicMax(a, v); }
-__device__ __forceinline__ unsigned long long dcsim_tail_bits(double x) { return (unsigned long long)__double_as_longlong(x); }
-__device__ __forceinline__ double dcsim_tail_double(unsigned long long u) { return __longlong_as_double((long long)u); }
-__device__ __forceinline__ int dcsim_tail_clz64(unsigned long long x) { return __clzll((long long)x); }
-#endif
-
 /* Keys that order like the values (IEEE patterns with the sign folded in), and back. */
 DCSIM_DEV unsigned long long dcsim_tail_key(double v) {
   const unsigned long long b = dcsim_tail_bits(v);
@@ -2892,14 +2887,14 @@ DCSIM_DEV void dcsim_tail_select(const dcsim_kparams_t* P, uint64_t r, int tid, 
     int g[2];
     unsigned long long v[DCSIM_TAIL_KINDS];
     if (!dcsim_tail_job(P, base, k, &g[0], &g[1], v)) {
-      dcsim_tail_add_u32(&S->unfinished[g[0]], 1u); dcsim_tail_add_u32(&S->unfinished[g[1]], 1u);
+      atomicAdd(&S->unfinished[g[0]], 1u); atomicAdd(&S->unfinished[g[1]], 1u);
       continue;
     }
     for (int j = 0; j < 2; ++j) {
-      dcsim_tail_add_u32(&S->jobs[g[j]], 1u);
+      atomicAdd(&S->jobs[g[j]], 1u);
       for (int c = 0; c < DCSIM_TAIL_KINDS; ++c) {
-        dcsim_tail_min_u64(&S->lo[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
-        dcsim_tail_max_u64(&S->hi[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
+        atomicMin(&S->lo[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
+        atomicMax(&S->hi[g[j] * DCSIM_TAIL_KINDS + c], v[c]);
       }
     }
   }
@@ -2933,7 +2928,7 @@ DCSIM_DEV void dcsim_tail_select(const dcsim_kparams_t* P, uint64_t r, int tid, 
           const uint32_t digit = (uint32_t)(v[c] >> s) & (DCSIM_TAIL_RADIX - 1u);
           for (int q = 0; q < DCSIM_TAIL_QUANTILES; ++q)
             if (S->low[t0 + q] == above && dcsim_tail_same_above(v[c], S->key[t0 + q], above))
-              dcsim_tail_add_u32(&S->hist[t0 + q][digit], 1u);
+              atomicAdd(&S->hist[t0 + q][digit], 1u);
         }
     }
     dcsim_tail_sync();

@@ -21,7 +21,7 @@ sys.path.insert(0, os.path.join(ROOT, "oracle"))
 sys.path.insert(0, os.path.join(ROOT, "tests"))
 from distributed_cluster_gpus_b200 import scenarios as S  # noqa: E402
 import ref_harness  # noqa: E402
-import hostemu_pp_lib  # noqa: E402
+import hostemu_lib  # noqa: E402
 
 FIELDS = ["profile_s", "peak_w", "t_peak_s", "over_s", "over_j", "excursions", "longest_over_s", "out_of_range"]
 BINS = 1024
@@ -151,7 +151,7 @@ def main():
     crossing = never = inf_case = False
     for sc, rule in CASES:
         spec = S.to_spec(sc).to_bytes()
-        hi = hostemu_pp_lib.power_range(spec)
+        hi = hostemu_lib.power_range(spec)
         runs = list(RUNS) + ([(123, "mt")] if sc["name"] in MT_SCENARIOS else [])
         thr = None
         cases = []

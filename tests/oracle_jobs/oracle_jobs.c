@@ -1,5 +1,5 @@
 /*
- * TEST-ONLY.  Per-job instants of the C oracle (oracle/dcsim_oracle.c, compiled here unchanged into its own library):
+ * TEST-ONLY.  Per-job instants of the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c):
  * for every job that finished, its arrival instant (simulator_paper_multi.py:539-540), its xfer_done instant
  * (SIM:580-588), its start and finish, and whether it started in the handler of its own xfer_done event (SIM:603-676)
  * rather than in a dequeue loop (SIM:840-927).  The oracle is stepped one event at a time; before each step the event
@@ -10,7 +10,6 @@
  *   - a job_finish finished its job when the finish count went up.
  * Rows come out in finish order.  Nothing here is part of, linked into, or reachable from the product library.
  */
-#include "../../oracle/dcsim_oracle.c"
 
 typedef struct {
   uint32_t jid;
@@ -18,8 +17,6 @@ typedef struct {
   int32_t at_xfer; /* 1: started by its own xfer_done event */
   double arrival, xfer_done, start, finish;
 } oracle_job_row_t;
-
-void oraclejobs_set_test_time_quantum(double q) { g_test_time_quantum = q; }
 
 /* One replica (key `seed`) to the end.  Writes up to `cap` rows; returns the number of finished jobs (> cap: the rows
  * are a prefix), -1 on a malformed spec. */

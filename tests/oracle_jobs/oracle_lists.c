@@ -1,6 +1,6 @@
 /*
- * TEST-ONLY.  The arrivals of one replica as the C oracle (oracle/dcsim_oracle.c, compiled here unchanged into its own
- * library) processes them: the independent reference of the arrival pre-pass (dcsim_generate_arrivals) and of what the
+ * TEST-ONLY.  The arrivals of one replica as the C oracle (oracle/dcsim_oracle.c, compiled unchanged into
+ * oracle_probes.c) processes them: the independent reference of the arrival pre-pass (dcsim_generate_arrivals) and of what the
  * list merge derives from it.  The oracle is stepped one event at a time; before each step the event about to fire is
  * the heap's top, and every event pushed during the step has a seq at or above the counter's value before it.  For each
  * arrival event (SIM:537-592):
@@ -12,7 +12,6 @@
  * Per replica also the RNG words the whole run consumed and first_mask (bit s: stream s's first arrival was pushed).
  * Nothing here is part of, linked into, or reachable from the product library.
  */
-#include "../../oracle/dcsim_oracle.c"
 
 typedef struct {
   double t, size, tx;
@@ -20,8 +19,6 @@ typedef struct {
   int32_t dc;
   uint32_t pred, next;
 } oracle_arr_row_t;
-
-void oraclelists_set_test_time_quantum(double q) { g_test_time_quantum = q; }
 
 /* One replica (key `seed`) to the end.  Writes up to `cap` rows; info[0] = first_mask, info[1] = RNG words.  Returns
  * the number of arrivals processed (> cap: the rows are a prefix), -1 on a malformed spec. */

@@ -1,14 +1,11 @@
 /*
- * TEST-ONLY.  Occupancy checkers on the C oracle (oracle/dcsim_oracle.c, compiled here unchanged into its own library),
+ * TEST-ONLY.  Occupancy checkers on the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c),
  * for tests/test_occupancy.py:
  *   - oracleocc_occupancy steps the oracle one event at a time and applies the definition of include/dcsim_b200.h
  *     (dcsim_enable_occupancy) to each DC's queue lengths, running count and busy GPUs as they stand before each step;
  *   - oracleocc_reached lists every job that reached its DC, with its xfer_done, start and finish instants (Little's law).
  * Nothing here is part of, linked into, or reachable from the product library.
  */
-#include "../../oracle/dcsim_oracle.c"
-
-void oracleocc_set_test_time_quantum(double q) { g_test_time_quantum = q; }
 
 /* One function's open level (include/dcsim_b200.h, dcsim_enable_occupancy): start (-1: none yet) and value. */
 typedef struct { double s, v; } occ_level_t;

@@ -1,5 +1,5 @@
 /*
- * TEST-ONLY.  Every job the C oracle (oracle/dcsim_oracle.c, compiled here unchanged through oracle_jobs.c) creates in
+ * TEST-ONLY.  Every job the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c) creates in
  * one replica, finished or not: its job type, the DC it was routed to, its arrival and xfer_done instants and, when it
  * finished, its start and finish.  The per-run tail-latency tests need the jobs that did not finish (UNFINISHED per type
  * and DC), which the per-job rows of oracle_jobs.c leave out.  The oracle is stepped one event at a time as in
@@ -8,7 +8,6 @@
  * simulator_paper_multi.py:537-577: the size, then the DC).  Nothing here is part of, linked into, or reachable from the
  * product library.
  */
-#include "oracle_jobs.c"
 
 typedef struct {
   uint32_t jid;

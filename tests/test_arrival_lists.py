@@ -18,9 +18,9 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_pair_lib as HP
+import hostemu_lib as H
 import list_reference as LR
-import oracle_lists_lib as OL
+import oracle_probes_lib as OP
 from conftest import ROOT
 from distributed_cluster_gpus_b200 import _native, scenarios as SC, spec as S
 
@@ -142,7 +142,7 @@ def check_arrivals(sp, d, replicas, seed0, rng_kind, quantum, t_rtol=0.0, size_u
     out, worst_t, worst_ulp = [], 0.0, 0
     end_eps = sp.end_time + 1e-9
     for r in replicas:
-        rows, first_mask, rng_words = OL.arrivals(sp.to_bytes(), seed0 + r, rng_kind, quantum)
+        rows, first_mask, rng_words = OP.arrivals(sp.to_bytes(), seed0 + r, rng_kind, quantum)
         h = d["hdr"][r]
         c = int(h["count"])
         if int(h["status"]) & ST_ARRIVALS_OVERFLOW:
@@ -178,12 +178,12 @@ def check_arrivals(sp, d, replicas, seed0, rng_kind, quantum, t_rtol=0.0, size_u
     return out, worst_t, worst_ulp
 
 
-@pytest.mark.parametrize("variant", HP.VARIANTS)
+@pytest.mark.parametrize("variant", H.VARIANTS)
 @pytest.mark.parametrize("name", list(CASES))
 def test_lists_and_arrivals_match_references(name, variant):
     make, n, seed, rng, q = CASES[name]
     sp = make()
-    d = HP.prepass(sp.to_bytes(), n, seed, rng, variant, q)
+    d = H.prepass(sp.to_bytes(), n, seed, rng, variant, q)
     assert np.all((d["hdr"]["status"] | LR.ST_XFER_OVERFLOW) == LR.ST_XFER_OVERFLOW)
     refs = check_lists(sp, d, range(n), q)
     rows, _, _ = check_arrivals(sp, d, range(n), seed, rng, q)
@@ -195,7 +195,7 @@ def test_eco_route_carries_sizes():
     """eco_route draws the size before routing and keeps it (meta bit 0x100); random routing keeps the raw draw."""
     for name, bit in (("eco_route", 1), ("cfg3", 0)):
         make, n, seed, rng, q = CASES[name]
-        d = HP.prepass(make().to_bytes(), n, seed, rng, "plain", q)
+        d = H.prepass(make().to_bytes(), n, seed, rng, "plain", q)
         for r in range(n):
             c = int(d["hdr"]["count"][r])
             assert c > 0 and np.all(((d["arr_meta"][r, :c] >> 8) & 1) == bit), name
@@ -208,7 +208,7 @@ def test_huge_finite_transfer_matches_oracle_end_to_end(oracle):
     blob = sp.to_bytes()
     want, total = oracle.run_batch(blob, 4, 123, 0)
     for uniform in (False, True):
-        got = HP.run(blob, blob, 4, 123, uniform=uniform)
+        got = H.run_batch(blob, 4, 123, uniform=uniform)
         assert got["events"] == total
         assert np.array_equal(got["summary"][:, S.S_EVENTS], want[:, S.S_EVENTS])
         assert np.all(got["summary"][:, S.S_STATUS] == 0)
@@ -228,7 +228,7 @@ COUNT_EDGE_BATCH = ((0, 24), (1, 160), (2, 320))   # (spec, replicas)
 def test_arrival_counts_at_chunk_edges():
     seen = set()
     for (i, n), sp in zip(COUNT_EDGE_BATCH, count_edge_specs()):
-        d = HP.prepass(sp.to_bytes(), n, 4000 + i, 0, "smallring")
+        d = H.prepass(sp.to_bytes(), n, 4000 + i, 0, "smallring")
         counts = d["hdr"]["count"]
         seen |= set(int(c) for c in counts)
         pick = [r for r in range(n) if counts[r] in COUNT_EDGES]
@@ -242,11 +242,11 @@ def test_arrival_capacity_edge_keeps_neighbours():
     keeps the oracle's prefix, and every other row equals the default-capacity run."""
     sc = _short("cfg3_4x64_sinusoid_120s", 10.0)
     n, seed = 12, 600
-    full = HP.prepass(SC.to_spec(sc).to_bytes(), n, seed)
+    full = H.prepass(SC.to_spec(sc).to_bytes(), n, seed)
     counts = full["hdr"]["count"].astype(int)
     cap = int(np.sort(counts)[n // 2])
     sp = SC.to_spec(sc, caps={"cap_arrivals": cap})
-    d = HP.prepass(sp.to_bytes(), n, seed)
+    d = H.prepass(sp.to_bytes(), n, seed)
     over = counts > cap
     assert np.any(counts == cap) and np.any(over)
     assert np.array_equal((d["hdr"]["status"] & ST_ARRIVALS_OVERFLOW) != 0, over)

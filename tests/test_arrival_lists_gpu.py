@@ -24,7 +24,7 @@ import sys
 import numpy as np
 import pytest
 
-import hostemu_pair_lib as HP
+import hostemu_lib as H
 import list_reference as LR
 from conftest import ROOT, has_cuda
 from distributed_cluster_gpus_b200 import scenarios as SC, spec as S
@@ -50,7 +50,7 @@ def _case(name):
 def _cap_specs():
     sc = _short("cfg3_4x64_sinusoid_120s", 10.0)
     full = SC.to_spec(sc)
-    counts = HP.prepass(full.to_bytes(), 12, 600)["hdr"]["count"].astype(int)
+    counts = H.prepass(full.to_bytes(), 12, 600)["hdr"]["count"].astype(int)
     return full, SC.to_spec(sc, caps={"cap_arrivals": int(np.sort(counts)[6])}), counts
 
 
@@ -94,7 +94,7 @@ def dev(tmp_path_factory):
         with np.load(out / (name + ".npz")) as z:
             d = {k: z[k] for k in z.files}
         if "hdr" in d:
-            d["hdr"] = d["hdr"].view(HP.HDR_DTYPE).reshape(-1)
+            d["hdr"] = d["hdr"].view(H.HDR_DTYPE).reshape(-1)
         return d
     return load
 
@@ -126,7 +126,7 @@ def test_device_lists_and_arrivals(dev, name):
     refs = check_lists(sp, d, range(n), q)
     rows, worst_t, worst_ulp = check_arrivals(sp, d, range(n), seed, rng, q, T_RTOL, SIZE_ULP)
     edge_reached(name, sp, refs, rows)
-    h = HP.prepass(sp.to_bytes(), n, seed, rng, "plain", q)
+    h = H.prepass(sp.to_bytes(), n, seed, rng, "plain", q)
     _same_discrete(d, h, range(n), range(n))
     _report(name, worst_t, worst_ulp)
 
@@ -159,7 +159,7 @@ def test_device_counts_at_chunk_edges(dev):
         pick = [r for r in range(n) if counts[r] in COUNT_EDGES]
         _, wt, wu = check_arrivals(sp, d, pick, 4000 + i, 0, 0.0, T_RTOL, SIZE_ULP)
         worst_t, worst_ulp = max(worst_t, wt), max(worst_ulp, wu)
-        _same_discrete(d, HP.prepass(sp.to_bytes(), n, 4000 + i), range(n), range(n))
+        _same_discrete(d, H.prepass(sp.to_bytes(), n, 4000 + i), range(n), range(n))
     assert set(COUNT_EDGES) <= seen, sorted(set(COUNT_EDGES) - seen)
     _report("count edges", worst_t, worst_ulp)
 
@@ -208,7 +208,7 @@ def test_device_bench_batch_sample(dev):
         sub = {k: v[i:i + 1] for k, v in d.items() if k != "replicas"}
         _, wt, wu = check_arrivals(sp, sub, [0], BENCH_SEED + r, 0, 0.0, T_RTOL, SIZE_ULP)
         worst_t, worst_ulp = max(worst_t, wt), max(worst_ulp, wu)
-        h = HP.prepass(sp.to_bytes(), 1, BENCH_SEED + r)
+        h = H.prepass(sp.to_bytes(), 1, BENCH_SEED + r)
         _same_discrete(sub, h, [0], [0])
     _report("bench sample", worst_t, worst_ulp)
 

@@ -10,7 +10,7 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_pair_lib as HP
+import hostemu_lib as H
 from distributed_cluster_gpus_b200 import scenarios as SC, spec as S
 from test_device_core_hostemu import _same
 
@@ -63,7 +63,7 @@ def needs(oracle, kind):
     blob = SC.to_spec(sc).to_bytes()
     want, _ = oracle.run_batch(blob, N, seed, 0, n_threads=os.cpu_count() or 1)
     assert np.all(want[:, S.S_STATUS] == 0)
-    _, hdr = HP.lists(blob, N, seed)
+    _, hdr = H.lists(blob, N, seed)
     assert np.array_equal(hdr["count"], want[:, S.S_EV_ARRIVAL])      # two independent counts of the same arrivals
     need = {"queue": want[:, S.S_MAX_Q], "run": want[:, S.S_MAX_RUN], "arrivals": hdr["count"],
             "ring": hdr["max_ahead"], "stale": None}[kind]
@@ -148,6 +148,6 @@ def test_stale_pool_edge(oracle, hostemu):
 
 def test_slow_wan_ring_need_straddles_8192():
     """The scenario of the device's staged -> in-place XFER retry: every replica's seq-ring need is in [8192, 16384)."""
-    _, hdr = HP.lists(SC.to_spec(SLOW_WAN_SC).to_bytes(), 8, 3)
+    _, hdr = H.lists(SC.to_spec(SLOW_WAN_SC).to_bytes(), 8, 3)
     assert np.all(hdr["status"] == 0) and np.all((hdr["max_ahead"] >= 8192) & (hdr["max_ahead"] < 16384))
     assert largest_fit("ring", 2100) == 8191 and largest_fit("ring", 4200) == 16383

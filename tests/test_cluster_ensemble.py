@@ -1,4 +1,4 @@
-"""Cluster-log ensemble on the CPU: the recorder of the device source (host build, tests/hostemu_ens) against every
+"""Cluster-log ensemble on the CPU: the recorder of the device source (host build, tests/hostemu) against every
 replica's oracle cluster log, the library's default tick capacity, the numpy mirror of the two reductions against numpy,
 and the two-rank all-reduce (gloo) against one rank."""
 import os
@@ -9,7 +9,7 @@ import pytest
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-import hostemu_ens_lib as HE
+import hostemu_lib as H
 from conftest import ROOT, golden_names
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -24,7 +24,7 @@ def _total_gpus(sp):
 def oracle_fields(oracle, sp, seed, rng_kind=0):
     """[ticks, FIELDS, n_dc] of one replica, derived from its oracle cluster log as write_csv_logs derives the CSV."""
     blob = sp.to_bytes()
-    ticks = HE.ens_ticks(blob)
+    ticks = H.ens_ticks(blob)
     sim = oracle.OracleSim(blob, seed, rng_kind=rng_kind, clog_cap=(ticks + 2) * sp.n_dc)
     sim.advance(0)
     log = sim.cluster_log()
@@ -38,8 +38,8 @@ def oracle_rows(oracle, sp, n, first):
 
 
 def _check_recorded(oracle, sp, got, seed0, n, rng_kind=0):
-    ticks = HE.ens_ticks(sp.to_bytes())
-    ens = got["ensemble"]
+    ticks = H.ens_ticks(sp.to_bytes())
+    ens = got["ens"]
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     assert np.all(got["summary"][:, S.S_EV_LOG] == ticks)
     assert np.all(np.isnan(ens[ticks:])), "a tick past the replica's count was written"
@@ -55,7 +55,7 @@ def test_recorder_equals_oracle_cluster_logs(oracle, monkeypatch, name, mode):
     """Every replica's recorded values equal the fields derived from its own oracle cluster log, bit for bit."""
     sp = SC.to_spec(SC.BY_NAME[name])
     blob = sp.to_bytes()
-    ticks = HE.ens_ticks(blob)
+    ticks = H.ens_ticks(blob)
     kw = dict(ens_cap=ticks + 2)
     if mode == "chunks61":
         kw["chunk_events"] = 61
@@ -64,27 +64,27 @@ def test_recorder_equals_oracle_cluster_logs(oracle, monkeypatch, name, mode):
     if mode == "records_global":
         monkeypatch.setenv("DCSIM_RECORDS", "global")
         kw["chunk_events"] = 977
-    got = HE.run_batch(blob, 3, SEED, **kw)
+    got = H.run_batch(blob, 3, SEED, **kw)
     _check_recorded(oracle, sp, got, SEED, 3)
 
 
 def test_recorder_mersenne_twister(oracle):
     sp = SC.to_spec(SC.BY_NAME["ragged_3dc_12_5_40"])
     blob = sp.to_bytes()
-    got = HE.run_batch(blob, 2, 77, ens_cap=HE.ens_ticks(blob), rng_kind=1, chunk_events=61)
+    got = H.run_batch(blob, 2, 77, ens_cap=H.ens_ticks(blob), rng_kind=1, chunk_events=61)
     _check_recorded(oracle, sp, got, 77, 2, rng_kind=1)
 
 
 def test_recorder_off_changes_nothing_and_capacity_is_respected(oracle, hostemu):
     sp = SC.to_spec(dict(SC.CFG3, duration=40.0))
     blob = sp.to_bytes()
-    plain = HE.run_batch(blob, 2, 9, ens_cap=0)
-    full = HE.run_batch(blob, 2, 9, ens_cap=HE.ens_ticks(blob))
-    short = HE.run_batch(blob, 2, 9, ens_cap=3)
+    plain = H.run_batch(blob, 2, 9, ens_cap=0)
+    full = H.run_batch(blob, 2, 9, ens_cap=H.ens_ticks(blob))
+    short = H.run_batch(blob, 2, 9, ens_cap=3)
     assert np.array_equal(plain["summary"], hostemu.run_batch(blob, 2, 9)["summary"])    # == the plain host build
     assert np.array_equal(plain["summary"], full["summary"]) and np.array_equal(plain["summary"], short["summary"])
-    assert np.array_equal(short["ensemble"], full["ensemble"][:3])
-    assert short["summary"][0, S.S_EV_LOG] == HE.ens_ticks(blob) > 3   # counts on past the capacity
+    assert np.array_equal(short["ens"], full["ens"][:3])
+    assert short["summary"][0, S.S_EV_LOG] == H.ens_ticks(blob) > 3   # counts on past the capacity
 
 
 @pytest.mark.parametrize("name", golden_names())
@@ -94,13 +94,13 @@ def test_default_tick_capacity_is_every_replicas_log_count(oracle, name):
         sc = dict(sc, duration=150.0)
     sp = SC.to_spec(sc)
     rows, _ = oracle.run_batch(sp.to_bytes(), 3, 31, 0)
-    assert np.all(rows[:, S.S_EV_LOG] == HE.ens_ticks(sp.to_bytes()))
+    assert np.all(rows[:, S.S_EV_LOG] == H.ens_ticks(sp.to_bytes()))
     for interval, end in ((0.1, 1.0), (0.3, 0.9), (5.0, 4.0), (600.0, 30000.0)):
         sp2 = SC.to_spec(dict(sc, log_interval=interval, duration=end))
         t, n = interval, 0
         while not t > end:
             n, t = n + 1, t + interval
-        assert HE.ens_ticks(sp2.to_bytes()) == n
+        assert H.ens_ticks(sp2.to_bytes()) == n
 
 
 def numpy_reference_check(res, rows, quantiles=EN.DEFAULT_QUANTILES):

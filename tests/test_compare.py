@@ -13,7 +13,7 @@ import pytest
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-import hostemu_pair_lib as HP
+import hostemu_lib as H
 from conftest import ROOT, load_golden
 from distributed_cluster_gpus_b200 import compare as CP, ensemble as EN, scenarios as SC, spec as S
 
@@ -48,8 +48,8 @@ OTHER_CAPS = {"cap_run": 9, "cap_q_inf": 7000, "cap_q_trn": 300, "cap_stale": 99
 
 
 def _same_lists(a, b, n, seed, rng_kind=0):
-    la, ha = HP.lists(a, n, seed, rng_kind)
-    lb, hb = HP.lists(b, n, seed, rng_kind)
+    la, ha = H.lists(a, n, seed, rng_kind)
+    lb, hb = H.lists(b, n, seed, rng_kind)
     if ha.tobytes() != hb.tobytes():
         return False
     return all(x.tobytes() == y.tobytes() for ra, rb in zip(la, lb) for x, y in zip(ra, rb))
@@ -64,9 +64,9 @@ def test_compatible_specs_draw_byte_identical_lists(seed):
     specs += [SC.to_spec(sc).to_bytes() for sc in _hand_picked() + _random_variants(4, seed % 1000)]
     specs.append(SC.to_spec(SC.BY_NAME["sweep_joint_nf"], caps=OTHER_CAPS).to_bytes())   # other capacities, the same ring
     for a, b in itertools.combinations(specs, 2):
-        eq, field = HP.compatible(a, b)
+        eq, field = H.compatible(a, b)
         assert eq and field == "", field
-    ref_lists, ref_hdr = HP.lists(specs[0], 3, seed)
+    ref_lists, ref_hdr = H.lists(specs[0], 3, seed)
     assert np.all(ref_hdr["status"] == 0) and np.all(ref_hdr["ml_count"] > 0)
     for b in specs[1:]:
         assert _same_lists(specs[0], b, 3, seed)
@@ -75,13 +75,13 @@ def test_compatible_specs_draw_byte_identical_lists(seed):
 def test_mersenne_twister_lists_are_shared_too():
     a = SC.to_spec(SC.BY_NAME[BASE]).to_bytes()
     b = SC.to_spec(SC.BY_NAME["cap_greedy_4x64"]).to_bytes()
-    assert HP.compatible(a, b)[0] and _same_lists(a, b, 2, 123, rng_kind=1)
+    assert H.compatible(a, b)[0] and _same_lists(a, b, 2, 123, rng_kind=1)
 
 
 def test_eco_route_is_rejected_and_its_lists_differ():
     eco = SC.to_spec(SC.BY_NAME["sweep_eco_route"]).to_bytes()
     base = SC.to_spec(SC.BY_NAME[BASE]).to_bytes()
-    eq, field = HP.compatible(base, eco)
+    eq, field = H.compatible(base, eco)
     assert not eq and field == "route_rule"
     assert not _same_lists(base, eco, 2, 123)
 
@@ -92,15 +92,15 @@ def test_smaller_seq_ring_is_rejected_and_flagged_like_its_standalone_batch():
     lists would run unflagged).  Its own run flags the overflow."""
     base = SC.to_spec(SC.BY_NAME[BASE]).to_bytes()
     small = SC.to_spec(SC.BY_NAME["sweep_joint_nf"], caps={"cap_xfer": 1}).to_bytes()
-    eq, field = HP.compatible(base, small)
+    eq, field = H.compatible(base, small)
     assert not eq and field == "cap_xfer"
-    _, h_base = HP.lists(base, 3, 123)
-    _, h_small = HP.lists(small, 3, 123)
+    _, h_base = H.lists(base, 3, 123)
+    _, h_small = H.lists(small, 3, 123)
     assert np.all(h_base["status"] == 0) and np.all(h_small["status"] & S.ST_XFER_OVERFLOW)
     assert np.array_equal(h_base["max_ahead"], h_small["max_ahead"])
-    assert np.all(HP.run(small, small, 3, 123)["summary"][:, S.S_STATUS].astype(int) & S.ST_XFER_OVERFLOW)
+    assert np.all(H.run_batch(small, 3, 123, run_spec=small)["summary"][:, S.S_STATUS].astype(int) & S.ST_XFER_OVERFLOW)
     with pytest.raises(ValueError):
-        HP.run(base, small, 3, 123)
+        H.run_batch(base, 3, 123, run_spec=small)
 
 
 def _with(spec, mutate):
@@ -159,22 +159,22 @@ UNLISTED = {
 def test_each_listed_field_flips_the_answer(field):
     base = SC.to_spec(SC.BY_NAME[BASE])
     other = _with(base, LISTED[field])
-    eq, named = HP.compatible(base.to_bytes(), bytes(other))
+    eq, named = H.compatible(base.to_bytes(), bytes(other))
     assert not eq and named == field
-    assert HP.compatible(bytes(other), bytes(other))[0]
+    assert H.compatible(bytes(other), bytes(other))[0]
 
 
 @pytest.mark.parametrize("field", sorted(UNLISTED))
 def test_unlisted_fields_do_not(field):
     base = SC.to_spec(SC.BY_NAME[BASE])
-    assert HP.compatible(base.to_bytes(), bytes(_with(base, UNLISTED[field])))[0]
+    assert H.compatible(base.to_bytes(), bytes(_with(base, UNLISTED[field])))[0]
 
 
 def test_eco_e_unit_counts_only_when_both_route_eco():
     eco = SC.to_spec(SC.BY_NAME["sweep_eco_route"])
-    eq, field = HP.compatible(eco.to_bytes(), bytes(_with(eco, lambda s: s.dc[3].eco_e_unit.__setitem__(1, 1e-3))))
+    eq, field = H.compatible(eco.to_bytes(), bytes(_with(eco, lambda s: s.dc[3].eco_e_unit.__setitem__(1, 1e-3))))
     assert not eq and field == "eco_e_unit"
-    assert HP.compatible(eco.to_bytes(), bytes(_with(eco, lambda s: setattr(s, "algo", S.ALGO_IDS["default_policy"]))))[0]
+    assert H.compatible(eco.to_bytes(), bytes(_with(eco, lambda s: setattr(s, "algo", S.ALGO_IDS["default_policy"]))))[0]
 
 
 def test_library_gives_the_host_builds_answers():
@@ -184,7 +184,7 @@ def test_library_gives_the_host_builds_answers():
     others = [SC.to_spec(SC.BY_NAME[k]) for k in SWEEP + ["sweep_eco_route", "cap_greedy_4x64", "cfg3_4x64_sinusoid_120s"]]
     others += [_with(base, f) for f in list(LISTED.values()) + list(UNLISTED.values())]
     for o in others:
-        assert arrivals_compatible(base, o) == HP.compatible(base.to_bytes(), bytes(o))[0]
+        assert arrivals_compatible(base, o) == H.compatible(base.to_bytes(), bytes(o))[0]
     lib = N.load()
     eq = C.c_int(7)
     blob = base.to_bytes()
@@ -208,7 +208,7 @@ def test_variant_on_the_owners_lists_equals_oracle_and_reference(oracle, variant
     sp_v, sp_o = SC.to_spec(doc["scenario"]).to_bytes(), SC.to_spec(SC.BY_NAME[owner]).to_bytes()
     kw = {"chunk_events": 61} if mode == "chunks61" else ({"uniform": True} if mode == "uniform" else {})
     for run in (r for r in doc["runs"] if r["rng"] == "philox"):
-        got = HP.run(sp_o, sp_v, 1, run["seed"], **kw)
+        got = H.run_batch(sp_o, 1, run["seed"], run_spec=sp_v, **kw)
         want, events = oracle.run_batch(sp_v, 1, run["seed"])
         assert got["events"] == events
         assert np.array_equal(got["summary"][:, :S.S_MAX_XFER], want[:, :S.S_MAX_XFER])
@@ -221,7 +221,7 @@ def test_variant_on_the_owners_lists_mersenne_twister(oracle):
     doc = load_golden("sweep_carbon_cost")
     run = [r for r in doc["runs"] if r["rng"] == "mt"][0]
     sp_v, sp_o = SC.to_spec(doc["scenario"]).to_bytes(), SC.to_spec(SC.BY_NAME["sweep_bandit"]).to_bytes()
-    got = HP.run(sp_o, sp_v, 1, run["seed"], chunk_events=61, rng_kind=1)
+    got = H.run_batch(sp_o, 1, run["seed"], run_spec=sp_v, chunk_events=61, rng_kind=1)
     want, events = oracle.run_batch(sp_v, 1, run["seed"], rng_kind=1)
     assert got["events"] == events == run["events"]
     assert np.array_equal(got["summary"][:, :S.S_MAX_XFER], want[:, :S.S_MAX_XFER])
@@ -230,7 +230,7 @@ def test_variant_on_the_owners_lists_mersenne_twister(oracle):
 
 def test_incompatible_pair_is_refused_by_the_host_run():
     with pytest.raises(ValueError):
-        HP.run(SC.to_spec(SC.BY_NAME[BASE]).to_bytes(), SC.to_spec(SC.BY_NAME["sweep_eco_route"]).to_bytes(), 1, 5)
+        H.run_batch(SC.to_spec(SC.BY_NAME[BASE]).to_bytes(), 1, 5, run_spec=SC.to_spec(SC.BY_NAME["sweep_eco_route"]).to_bytes())
 
 
 # ---- the numpy mirror of the paired reductions ------------------------------------------------------------------------

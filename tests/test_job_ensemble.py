@@ -1,4 +1,4 @@
-"""Job-log ensemble on the CPU: the recorder of the device source (host build, tests/hostemu_ens) against every
+"""Job-log ensemble on the CPU: the recorder of the device source (host build, tests/hostemu) against every
 replica's oracle job log, the window rule, the numpy mirror of the reductions against numpy, the CSV, and the two-rank
 all-reduce (gloo) against one rank."""
 import os
@@ -9,7 +9,7 @@ import pytest
 import torch.distributed as dist
 import torch.multiprocessing as mp
 
-import hostemu_jens_lib as HJ
+import hostemu_lib as H
 from conftest import ROOT
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -33,9 +33,9 @@ def _check_recorded(oracle, sp, got, seed0, n, bin_s, rng_kind=0):
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     for r in range(n):
         rows, hist = oracle_job_rows(oracle, sp, seed0 + r, bin_s, rng_kind)
-        assert np.array_equal(got["rows"][..., r], rows), (r, np.argwhere(got["rows"][..., r] != rows)[:5])
-        assert np.array_equal(got["hist"][r], hist), r
-        assert got["rows"][-1, 0, :, :, r].sum() == got["summary"][r, S.S_JOBS_FINISHED]
+        assert np.array_equal(got["jens"][..., r], rows), (r, np.argwhere(got["jens"][..., r] != rows)[:5])
+        assert np.array_equal(got["jens_hist"][r], hist), r
+        assert got["jens"][-1, 0, :, :, r].sum() == got["summary"][r, S.S_JOBS_FINISHED]
 
 
 @pytest.mark.parametrize("mode", ["one_shot", "chunks61", "uniform", "records_global"])
@@ -52,25 +52,25 @@ def test_recorder_equals_oracle_job_logs(oracle, monkeypatch, name, mode):
     if mode == "records_global":
         monkeypatch.setenv("DCSIM_RECORDS", "global")
         kw["chunk_events"] = 977
-    got = HJ.run_batch(sp.to_bytes(), 3, SEED, sp.log_interval, **kw)
+    got = H.run_batch(sp.to_bytes(), 3, SEED, jens_bin=sp.log_interval, **kw)
     _check_recorded(oracle, sp, got, SEED, 3, sp.log_interval)
 
 
 def test_recorder_mersenne_twister(oracle):
     sp = SC.to_spec(SC.BY_NAME["ragged_3dc_12_5_40"])
-    got = HJ.run_batch(sp.to_bytes(), 2, 77, sp.log_interval, rng_kind=1, chunk_events=61)
+    got = H.run_batch(sp.to_bytes(), 2, 77, jens_bin=sp.log_interval, rng_kind=1, chunk_events=61)
     _check_recorded(oracle, sp, got, 77, 2, sp.log_interval, rng_kind=1)
 
 
 def test_recorder_changes_no_summary_and_splits_the_batch_histogram(hostemu):
     sp = SC.to_spec(dict(SC.CFG3, duration=40.0))
     blob = sp.to_bytes()
-    off = HJ.run_batch(blob, 3, 9, sp.log_interval, record=False)
-    on = HJ.run_batch(blob, 3, 9, sp.log_interval)
+    off = H.run_batch(blob, 3, 9)
+    on = H.run_batch(blob, 3, 9, jens_bin=sp.log_interval)
     assert np.array_equal(off["summary"], hostemu.run_batch(blob, 3, 9)["summary"])    # == the plain host build
     assert np.array_equal(off["summary"], on["summary"])
     assert np.array_equal(off["lat_hist"], on["lat_hist"])
-    assert np.array_equal(on["hist"].sum(axis=1), on["lat_hist"])   # per-DC histogram summed over DCs
+    assert np.array_equal(on["jens_hist"].sum(axis=1), on["lat_hist"])   # per-DC histogram summed over DCs
     assert on["lat_hist"].sum() == on["summary"][:, S.S_JOBS_FINISHED].sum() > 0
 
 
@@ -80,10 +80,10 @@ def test_window_rule(oracle, bin_s, windows):
     (log_interval = 5 s).  Host build, numpy and the recorder agree; every job is in one window and in the whole run."""
     sp = SC.to_spec(dict(SC.CFG3, duration=60.0))
     b = bin_s or sp.log_interval
-    assert HJ.job_windows(sp.to_bytes(), b) == EN.job_windows(sp.end_time, b) == windows
-    got = HJ.run_batch(sp.to_bytes(), 2, 31, b)
-    assert got["rows"].shape[0] == windows + 1
-    assert np.array_equal(got["rows"][:-1, 0].sum(axis=0), got["rows"][-1, 0])
+    assert H.job_windows(sp.to_bytes(), b) == EN.job_windows(sp.end_time, b) == windows
+    got = H.run_batch(sp.to_bytes(), 2, 31, jens_bin=b)
+    assert got["jens"].shape[0] == windows + 1
+    assert np.array_equal(got["jens"][:-1, 0].sum(axis=0), got["jens"][-1, 0])
     _check_recorded(oracle, sp, got, 31, 2, b)
     t = np.array([0.0, b * 0.5, b, 60.0, 60.0 + 1e-9, np.nextafter(b * windows, 0)])
     k = EN.job_window_index(t, b, windows)

@@ -1,5 +1,5 @@
 """GPUs, frequency and predicted energy of every finished job, on the CPU: the recorder of the device source (host
-build, tests/hostemu_ens/hostemu_jres.cpp) against every replica's job records from the C oracle and against the
+build, tests/hostemu) against every replica's job records from the C oracle and against the
 reference goldens (tests/golden/make_golden_jres.py), the off switch, the numpy mirror, and the CLI flag."""
 import json
 import math
@@ -9,7 +9,7 @@ import sys
 import numpy as np
 import pytest
 
-import hostemu_jres_lib as HJ
+import hostemu_lib as H
 from conftest import GOLDEN_DIR
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -51,7 +51,7 @@ def expected(sp, jobs, bin_s):
     """One replica's oracle job log (finish order) -> (rows [W + 1, 3, n_dc, 2], mix [n_dc, 2, G * 16 + 1],
     hist [n_dc, 2, 128], E_job values); each sum a plain sequential f64 sum in finish order."""
     W = EN.job_windows(sp.end_time, bin_s)
-    G = HJ.mix_g(sp.max_gpus_per_job)
+    G = H.jres_g(sp.to_bytes())
     rows = np.zeros((W + 1, 3, sp.n_dc, 2))
     mix = np.zeros((sp.n_dc, 2, G * 16 + 1), dtype=np.uint32)
     hist = np.zeros((sp.n_dc, 2, 128), dtype=np.uint32)
@@ -86,13 +86,13 @@ def check(sp, got, seed0, n, bin_s, rng_kind=0):
     es = []
     for r in range(n):
         rows, mix, hist, e = expected(sp, oracle_job_log(sp, seed0 + r, rng_kind), bin_s)
-        assert np.array_equal(got["rows"][..., r].view(np.uint64), rows.view(np.uint64)), \
-            (r, np.argwhere(got["rows"][..., r] != rows)[:5])
-        assert np.array_equal(got["mix"][..., r], mix), r
-        assert np.array_equal(got["hist"][..., r], hist), r
+        assert np.array_equal(got["jres"][..., r].view(np.uint64), rows.view(np.uint64)), \
+            (r, np.argwhere(got["jres"][..., r] != rows)[:5])
+        assert np.array_equal(got["jres_mix"][..., r], mix), r
+        assert np.array_equal(got["jres_hist"][..., r], hist), r
         # the counts agree with the job ensemble's: every finished job once in the mix and once in the histogram
-        assert np.array_equal(got["mix"][..., r].sum(axis=-1), got["jens"][-1, 0, ..., r])
-        assert np.array_equal(got["hist"][..., r].sum(axis=-1), got["jens"][-1, 0, ..., r])
+        assert np.array_equal(got["jres_mix"][..., r].sum(axis=-1), got["jens"][-1, 0, ..., r])
+        assert np.array_equal(got["jres_hist"][..., r].sum(axis=-1), got["jens"][-1, 0, ..., r])
         es += e
     return es
 
@@ -105,11 +105,11 @@ def test_recorder_equals_oracle_jobs(name, mode):
     its DC's levels (OFF_LEVEL stays 0) and no E_job is clamped into an end bin."""
     sp = SC.to_spec(SC.BY_NAME[name])
     kw = {"chunk_events": 61 if "chunks" in mode else 0, "uniform": mode.startswith("uniform")}
-    got = HJ.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, sp.max_gpus_per_job, **kw)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jres=True, **kw)
     es = check(sp, got, SEED, N_REP, sp.log_interval)
-    assert int(got["mix"][:, :, -1].sum()) == 0, "OFF_LEVEL"
+    assert int(got["jres_mix"][:, :, -1].sum()) == 0, "OFF_LEVEL"
     if name == "all_off_2x8":
-        assert not es and not got["rows"].any()
+        assert not es and not got["jres"].any()
         return
     assert 1.0 <= min(es) and ebin_exact(max(es)) < 127, (min(es), max(es))
 
@@ -117,7 +117,7 @@ def test_recorder_equals_oracle_jobs(name, mode):
 def test_recorder_mt19937():
     """MT19937 replicas (the stock reference's own random stream) on the cap_greedy cluster."""
     sp = SC.to_spec(SC.BY_NAME["cap_greedy_4x64"])
-    got = HJ.run_batch(sp.to_bytes(), 2, SEED, sp.log_interval, sp.max_gpus_per_job, chunk_events=61, rng_kind=1)
+    got = H.run_batch(sp.to_bytes(), 2, SEED, jens_bin=sp.log_interval, jres=True, chunk_events=61, rng_kind=1)
     check(sp, got, SEED, 2, sp.log_interval, rng_kind=1)
 
 
@@ -126,7 +126,7 @@ def test_recorder_head_staged_records(monkeypatch):
     log_interval."""
     monkeypatch.setenv("DCSIM_RECORDS", "global")
     sp = SC.to_spec(SC.BY_NAME["cap_greedy_4x64"])
-    got = HJ.run_batch(sp.to_bytes(), 2, SEED, 7.0, sp.max_gpus_per_job, chunk_events=977)
+    got = H.run_batch(sp.to_bytes(), 2, SEED, jens_bin=7.0, jres=True, chunk_events=977)
     check(sp, got, SEED, 2, 7.0)
 
 
@@ -136,8 +136,8 @@ def test_mix_tells_the_policies_apart():
     seen = {}
     for name in ("sweep_joint_nf", "sweep_bandit", "sweep_default_perf_first"):
         sp = SC.to_spec(SC.BY_NAME[name])
-        got = HJ.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, sp.max_gpus_per_job)
-        m = got["mix"][:, :, :-1].sum(axis=(0, 1, 3)).reshape(HJ.mix_g(sp.max_gpus_per_job), 16)
+        got = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jres=True)
+        m = got["jres_mix"][:, :, :-1].sum(axis=(0, 1, 3)).reshape(H.jres_g(sp.to_bytes()), 16)
         seen[name] = (np.count_nonzero(m.sum(axis=1)), np.count_nonzero(m.sum(axis=0)))
     assert seen["sweep_bandit"][1] > 1 and seen["sweep_joint_nf"] != seen["sweep_default_perf_first"], seen
 
@@ -147,9 +147,8 @@ def test_summaries_unchanged_by_the_recorder(name):
     """With the recorder on (the records then carry size / f / jid) every summary row, and the job ensemble, are
     bit-identical to the recorder off."""
     sp = SC.to_spec(SC.BY_NAME[name])
-    on = HJ.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, sp.max_gpus_per_job, chunk_events=61)
-    off = HJ.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, sp.max_gpus_per_job, chunk_events=61,
-                       resources=False)
+    on = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jres=True, chunk_events=61)
+    off = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, chunk_events=61)
     assert np.array_equal(on["summary"], off["summary"]) and on["events"] == off["events"]
     assert np.array_equal(on["jens"], off["jens"]) and np.array_equal(on["jens_hist"], off["jens_hist"])
 
@@ -167,12 +166,12 @@ def test_golden_from_reference(fname):
         doc = json.load(f)
     sp = SC.to_spec(doc["scenario"])
     for case in doc["cases"]:
-        got = HJ.run_batch(sp.to_bytes(), 1, case["seed"], sp.log_interval, sp.max_gpus_per_job,
+        got = H.run_batch(sp.to_bytes(), 1, case["seed"], jens_bin=sp.log_interval, jres=True,
                            rng_kind=RNG[case["rng"]])
         rows, mix, hist = golden_arrays(case)
         assert got["summary"][0, S.S_JOBS_FINISHED] == case["jobs_finished"]
-        assert np.array_equal(got["rows"][..., 0].view(np.uint64), rows.view(np.uint64)), (fname, case["seed"])
-        assert np.array_equal(got["mix"][..., 0], mix) and np.array_equal(got["hist"][..., 0], hist), (fname, case["seed"])
+        assert np.array_equal(got["jres"][..., 0].view(np.uint64), rows.view(np.uint64)), (fname, case["seed"])
+        assert np.array_equal(got["jres_mix"][..., 0], mix) and np.array_equal(got["jres_hist"][..., 0], hist), (fname, case["seed"])
 
 
 def test_goldens_cover_the_edges():
@@ -187,11 +186,11 @@ def test_goldens_cover_the_edges():
 
 def _mirror_inputs(name="ragged_3dc_12_5_40", n=4, bad=(1,)):
     sp = SC.to_spec(SC.BY_NAME[name])
-    got = HJ.run_batch(sp.to_bytes(), n, SEED, sp.log_interval, sp.max_gpus_per_job)
+    got = H.run_batch(sp.to_bytes(), n, SEED, jens_bin=sp.log_interval, jres=True)
     status = np.zeros(n)
     status[list(bad)] = 1
-    G = HJ.mix_g(sp.max_gpus_per_job)
-    mix = got["mix"][:, :, :-1].reshape(sp.n_dc, 2, G, 16, n)
+    G = H.jres_g(sp.to_bytes())
+    mix = got["jres_mix"][:, :, :-1].reshape(sp.n_dc, 2, G, 16, n)
     return sp, got, status, mix
 
 
@@ -200,18 +199,18 @@ def test_mirror_statistics():
     the valid replicas; MEAN_* columns are *_SUM / JOBS per replica; the energy quantiles lie in their bins."""
     sp, got, status, mix = _mirror_inputs()
     good = status == 0
-    res = EN.job_resources_from_rows(got["rows"], mix, got["mix"][:, :, -1], got["hist"], got["jens"][:, 0], status,
+    res = EN.job_resources_from_rows(got["jres"], mix, got["jres_mix"][:, :, -1], got["jres_hist"], got["jens"][:, 0], status,
                                      EN._res_levels(sp), sp.log_interval, sp.end_time)
     assert np.array_equal(res.jobs, got["jens"][-1, 0][..., good].sum(axis=-1))
     assert np.array_equal(res.mix, mix[..., good].sum(axis=-1))
-    assert np.array_equal(res.energy_histogram, got["hist"][..., good].sum(axis=-1))
-    assert np.allclose(res.energy_sum, got["rows"][-1, 2][..., good].sum(axis=-1), rtol=1e-12)
-    W = got["rows"].shape[0] - 1
+    assert np.array_equal(res.energy_histogram, got["jres_hist"][..., good].sum(axis=-1))
+    assert np.allclose(res.energy_sum, got["jres"][-1, 2][..., good].sum(axis=-1), rtol=1e-12)
+    W = got["jres"].shape[0] - 1
     i = res.fields.index("mean_gpus")
     for d in range(sp.n_dc):
         for jt in range(2):
             jobs = got["jens"][W, 0, d, jt][good]
-            vals = got["rows"][W, 0, d, jt][good][jobs > 0] / jobs[jobs > 0]
+            vals = got["jres"][W, 0, d, jt][good][jobs > 0] / jobs[jobs > 0]
             assert res.n[W, i, d, jt] == len(vals)
             if len(vals):
                 assert res.min[W, i, d, jt] == vals.min() and res.max[W, i, d, jt] == vals.max()
@@ -242,7 +241,7 @@ def test_mirror_csv_and_accessors(tmp_path):
     """The CSV: window rows of the three means, then per DC and type energy_j, one mix row per (n, f) and the
     off-level row; the mix rows' counts add up to the jobs."""
     sp, got, status, mix = _mirror_inputs()
-    res = EN.job_resources_from_rows(got["rows"], mix, got["mix"][:, :, -1], got["hist"], got["jens"][:, 0], status,
+    res = EN.job_resources_from_rows(got["jres"], mix, got["jres_mix"][:, :, -1], got["jres_hist"], got["jens"][:, 0], status,
                                      EN._res_levels(sp), sp.log_interval, sp.end_time)
     names = [f"DC{d}" for d in range(sp.n_dc)]
     out = tmp_path / "r.csv"
@@ -250,7 +249,7 @@ def test_mirror_csv_and_accessors(tmp_path):
     import csv as _csv
     rows = list(_csv.reader(open(out)))
     assert rows[0] == EN.JOB_CSV_HEADER_HEAD + res.quantile_names() + ["max"]
-    W = got["rows"].shape[0] - 1
+    W = got["jres"].shape[0] - 1
     win = [r for r in rows[1:] if r[4] in EN.RES_CSV_FIELDS]
     assert len(win) == (W + 1) * sp.n_dc * 2 * 3
     for d in range(sp.n_dc):
@@ -259,7 +258,7 @@ def test_mirror_csv_and_accessors(tmp_path):
             e = [r for r in mine if r[4] == "energy_j"][0]
             assert int(e[5]) == int(res.jobs[d, jt])
             m = [r for r in mine if r[4].startswith("mix_")]
-            assert len(m) == HJ.mix_g(sp.max_gpus_per_job) * sp.dc[d].n_freq + 1
+            assert len(m) == H.jres_g(sp.to_bytes()) * sp.dc[d].n_freq + 1
             assert sum(int(r[5]) for r in m) == int(res.jobs[d, jt])
             assert m[-1][4] == "mix_off_level" and int(m[-1][5]) == 0
 
@@ -275,7 +274,7 @@ def test_cli_flag_summary_and_compare_refusal():
         R.main(["--compare-algos", "default_policy,cap_greedy", "--job-resources-csv", "r.csv"])
     assert "--job-resources-csv" in str(ei.value)
     sp, got, status, mix = _mirror_inputs()
-    res = EN.job_resources_from_rows(got["rows"], mix, got["mix"][:, :, -1], got["hist"], got["jens"][:, 0], status,
+    res = EN.job_resources_from_rows(got["jres"], mix, got["jres_mix"][:, :, -1], got["jres_hist"], got["jens"][:, 0], status,
                                      EN._res_levels(sp), sp.log_interval, sp.end_time)
 
     class _Sim:

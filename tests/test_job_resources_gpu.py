@@ -13,7 +13,7 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_jres_lib as HJ
+import hostemu_lib as H
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import _native as N, ensemble as EN, scenarios as SC, spec as S
 from test_job_resources import GOLDEN_FILES, JRES_GOLDEN, expected, golden_arrays, oracle_job_log
@@ -64,7 +64,7 @@ def test_device_equals_host_build(monkeypatch, lanes, mode, name):
     force_mode(monkeypatch, lanes, mode)
     sp = spec_for(SCENARIOS[name], mode)
     n = 7
-    host = HJ.run_batch(sp.to_bytes(), n, SEED, sp.log_interval, sp.max_gpus_per_job)
+    host = H.run_batch(sp.to_bytes(), n, SEED, jens_bin=sp.log_interval, jres=True)
     for chunk in (0, 61):
         with _engine(sp, n) as eng:
             eng.enable_job_ensemble()
@@ -84,8 +84,8 @@ def test_device_equals_host_build(monkeypatch, lanes, mode, name):
         assert same_bits(rows[..., LOGGED], w_rows), (chunk, np.argwhere(rows[..., LOGGED] != w_rows)[:5])
         assert np.array_equal(mix[..., LOGGED], w_mix) and np.array_equal(hist[..., LOGGED], w_hist), chunk
         for r in range(n):
-            close_to(rows[..., r], mix[..., r], hist[..., r], host["rows"][..., r], host["mix"][..., r],
-                     host["hist"][..., r], (chunk, r))
+            close_to(rows[..., r], mix[..., r], hist[..., r], host["jres"][..., r], host["jres_mix"][..., r],
+                     host["jres_hist"][..., r], (chunk, r))
         assert int(mix[:, :, -1].sum()) == 0
         if name not in _FIRST:
             _FIRST[name] = (rows, mix, hist)
@@ -166,7 +166,7 @@ def test_bench_batch():
         w_rows, w_mix, w_hist, _ = expected(sp, oracle_job_log(sp, 123 + r), sp.log_interval)
         close_to(rows[..., r], mix[..., r], hist[..., r], w_rows, w_mix, w_hist, r)
     n_dc = sp.n_dc
-    G = HJ.mix_g(sp.max_gpus_per_job)
+    G = H.jres_g(sp.to_bytes())
     host = EN.job_resources_from_rows(rows, mix[:, :, :-1].reshape(n_dc, 2, G, 16, BENCH_N), mix[:, :, -1], hist,
                                       jobs[:, 0], on[:, S.S_STATUS], EN._res_levels(sp), sp.log_interval, sp.end_time)
     check_reductions(res, host)
@@ -229,7 +229,7 @@ def test_error_codes_and_reset():
     with _engine(sp, n) as eng:
         eng.enable_job_ensemble(1.0)
         W = eng.job_ensemble_windows
-        G = HJ.mix_g(sp.max_gpus_per_job)
+        G = H.jres_g(sp.to_bytes())
         need = (W + 1) * 3 * sp.n_dc * 2 * n * 8 + sp.n_dc * 2 * (G * 16 + 1 + 128) * n * 4
         torch.cuda.synchronize()
         free, _ = torch.cuda.mem_get_info()

@@ -1,4 +1,4 @@
-"""Waiting and response times on the CPU: the recorder of the device source (host build, tests/hostemu_ens) against
+"""Waiting and response times on the CPU: the recorder of the device source (host build, tests/hostemu) against
 every replica's per-job instants from the oracle (tests/oracle_jobs), the wait invariants, the off switch, and the
 numpy mirror's CSV against a pinned fixture."""
 import importlib.util
@@ -7,7 +7,8 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_jwait_lib as HW
+import hostemu_lib as H
+import oracle_probes_lib as OP
 from conftest import GOLDEN_DIR
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -46,14 +47,14 @@ def _check(sp, got, seed0, n, bin_s):
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     all_jobs = []
     for r in range(n):
-        jobs = HW.oracle_jobs(sp.to_bytes(), seed0 + r)
+        jobs = OP.oracle_jobs(sp.to_bytes(), seed0 + r)
         assert len(jobs) == got["summary"][r, S.S_JOBS_FINISHED]
         rows, hist = expected_rows(jobs, sp.n_dc, bin_s, sp.end_time)
-        assert np.array_equal(got["rows"][..., r], rows), (r, np.argwhere(got["rows"][..., r] != rows)[:5])
-        assert np.array_equal(got["hist"][r], hist), r
+        assert np.array_equal(got["jwait"][..., r], rows), (r, np.argwhere(got["jwait"][..., r] != rows)[:5])
+        assert np.array_equal(got["jwait_hist"][r], hist), r
         # WAITED <= jobs in every cell; the histograms count every finished job once per kind
-        assert np.all(got["rows"][:, 0, ..., r] <= got["jens"][:, 0, ..., r])
-        assert np.array_equal(got["hist"][r].sum(axis=-1)[:, 0], got["jens"][-1, 0, :, :, r])
+        assert np.all(got["jwait"][:, 0, ..., r] <= got["jens"][:, 0, ..., r])
+        assert np.array_equal(got["jwait_hist"][r].sum(axis=-1)[:, 0], got["jens"][-1, 0, :, :, r])
         all_jobs.append(jobs)
     return np.concatenate(all_jobs)
 
@@ -73,7 +74,7 @@ def test_recorder_equals_oracle_jobs(name, mode):
     in finish order, bit for bit; plain and warp-uniform loop, one shot and in chunks."""
     sp = SC.to_spec(SC.BY_NAME[name])
     kw = {"chunk_events": 61 if "chunks" in mode else 0, "uniform": mode.startswith("uniform")}
-    got = HW.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, **kw)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jwait=True, **kw)
     jobs = _check(sp, got, SEED, N_REP, sp.log_interval)
     wait, at = _invariants(jobs)
     if name != "sweep_eco_route":                    # (eco_route spreads this load without queueing)
@@ -84,13 +85,18 @@ def test_recorder_head_staged_records(monkeypatch):
     """The head-staged host mode (the running records used where they live)."""
     monkeypatch.setenv("DCSIM_RECORDS", "global")
     sp = SC.to_spec(SC.BY_NAME["cap_greedy_4x64"])
-    _check(sp, HW.run_batch(sp.to_bytes(), 2, SEED, 7.0, chunk_events=977), SEED, 2, 7.0)
+    _check(sp, H.run_batch(sp.to_bytes(), 2, SEED, jens_bin=7.0, jwait=True, chunk_events=977), SEED, 2, 7.0)
+
+
+def _set_quantum(q):
+    H.set_test_time_quantum(q)
+    OP.set_test_time_quantum(q)
 
 
 @pytest.fixture
 def quantum():
-    yield HW.set_test_time_quantum
-    HW.set_test_time_quantum(0.0)
+    yield _set_quantum
+    _set_quantum(0.0)
 
 
 @pytest.mark.parametrize("uniform", [False, True])
@@ -100,7 +106,7 @@ def test_tie_hook_run(quantum, uniform):
     sc = dict(SC.BY_NAME["cfg3_4x64_sinusoid_120s"])
     sp = SC.to_spec(sc, caps={"cap_xfer": 4096})
     quantum(0.25)
-    got = HW.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, chunk_events=61, uniform=uniform)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jwait=True, chunk_events=61, uniform=uniform)
     jobs = _check(sp, got, SEED, N_REP, sp.log_interval)
     wait, at = _invariants(jobs)
     assert np.count_nonzero(wait > 0.0) > 0 and np.count_nonzero(at) > 0
@@ -117,14 +123,14 @@ def test_same_instant_dequeue_does_not_count_as_waited(quantum, uniform):
     k = sp.dc[0].coeffs[0]
     k.alpha_t, k.beta_t, k.gamma_t = 1e-30, 0.0, 0.0
     quantum(0.25)
-    got = HW.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, chunk_events=61, uniform=uniform)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jwait=True, chunk_events=61, uniform=uniform)
     jobs = _check(sp, got, SEED, N_REP, sp.log_interval)
     wait, at = _invariants(jobs)
     dequeued_at_once = np.count_nonzero(~at & (wait == 0.0))
     assert dequeued_at_once > 0, "no job was dequeued at its own xfer_done instant"
     assert np.count_nonzero(wait > 0.0) > 0
     # the recorder's whole-run WAITED counts only the jobs that waited, not every job that went through a queue
-    assert got["rows"][-1, 0].sum() == np.count_nonzero(wait > 0.0) < np.count_nonzero(~at)
+    assert got["jwait"][-1, 0].sum() == np.count_nonzero(wait > 0.0) < np.count_nonzero(~at)
 
 
 @pytest.mark.parametrize("name", FIXTURES)
@@ -132,8 +138,8 @@ def test_summaries_unchanged_by_the_recorder(name):
     """With the recorder on (the records then carry the job id) every summary row, and the job ensemble, are
     bit-identical to the recorder off."""
     sp = SC.to_spec(SC.BY_NAME[name])
-    on = HW.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, chunk_events=61)
-    off = HW.run_batch(sp.to_bytes(), N_REP, SEED, sp.log_interval, chunk_events=61, waits=False)
+    on = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, jwait=True, chunk_events=61)
+    off = H.run_batch(sp.to_bytes(), N_REP, SEED, jens_bin=sp.log_interval, chunk_events=61)
     assert np.array_equal(on["summary"], off["summary"]) and on["events"] == off["events"]
     assert np.array_equal(on["jens"], off["jens"]) and np.array_equal(on["jens_hist"], off["jens_hist"])
 

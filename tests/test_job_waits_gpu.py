@@ -4,7 +4,7 @@ recorder on against the recorder off."""
 import numpy as np
 import pytest
 
-import hostemu_jwait_lib as HW
+import oracle_probes_lib as OP
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import _native as N, ensemble as EN, scenarios as SC, spec as S
 from test_job_waits import expected_rows
@@ -27,7 +27,7 @@ def _engine(sp, n, seed=SEED):
 def _oracle(name, n):
     if (name, n) not in _ORACLE:
         sp = SC.to_spec(SCENARIOS[name])
-        _ORACLE[(name, n)] = [expected_rows(HW.oracle_jobs(sp.to_bytes(), SEED + r), sp.n_dc, sp.log_interval,
+        _ORACLE[(name, n)] = [expected_rows(OP.oracle_jobs(sp.to_bytes(), SEED + r), sp.n_dc, sp.log_interval,
                                             sp.end_time) for r in range(n)]
     return _ORACLE[(name, n)]
 

@@ -10,7 +10,7 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_pp_lib as HPP
+import hostemu_lib as H
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import scenarios as SC, spec as S
 from test_gpu_parity import assert_rows_match
@@ -98,7 +98,7 @@ def test_kernel_matches_oracle(oracle, monkeypatch, lanes, mode, cap, pp):
             assert np.array_equal(got.view(np.uint64), first[1].view(np.uint64)), \
                 (what, "differs from", first[0], np.argwhere(got != first[1])[:6])
             if pp:
-                ref = HPP.run_batch(SC.to_spec(sc).to_bytes(), n, SEED, threshold=thr)["rows"]
+                ref = H.run_batch(SC.to_spec(sc).to_bytes(), n, SEED, pp=True, pp_threshold=thr)["pp"]
                 assert_close(rows, ref, str(what))
     _TABLE.append((lanes, mode, cap, pp, info["lanes_per_replica"], info["staging_mode"], info["regs_per_thread"],
                    info["smem_bytes_per_cta"]))

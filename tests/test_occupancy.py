@@ -1,4 +1,4 @@
-"""Occupancy on the CPU: the recorder of the device source (host build, tests/hostemu_ens/hostemu_occ.cpp) against the
+"""Occupancy on the CPU: the recorder of the device source (host build, tests/hostemu) against the
 unmodified reference's fixtures and the C oracle stepped one event at a time (tests/oracle_jobs/oracle_occ.c), Little's
 law against the oracle's per-job instants, the recorder's invariants and off switch, and the numpy mirror's CSV against
 pinned fixtures."""
@@ -8,7 +8,8 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_occ_lib as HO
+import hostemu_lib as H
+import oracle_probes_lib as OP
 from conftest import GOLDEN_DIR
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -51,7 +52,7 @@ REF_FIXTURES = sorted(f[:-5] for f in os.listdir(REF_DIR) if f.endswith(".json")
 def reference_column(doc, case):
     """One run of a fixture of tests/golden/make_golden_occupancy.py -> the library's column of one replica."""
     D = doc["scenario"]["n_dc"]
-    col = np.zeros(HO.n_rows(D))
+    col = np.zeros(H.occ_rows(D))
     col[0] = float.fromhex(case["profile_s"])
     col[1:1 + S.OCC_FIELDS * D] = [float.fromhex(x) for x in case["fields"]]
     for i, x in case["bins"].items():
@@ -68,20 +69,20 @@ def test_recorder_equals_reference_fixtures(name, chunk):
         doc = json.load(f)
     sp = SC.to_spec(doc["scenario"])
     for case in doc["cases"]:
-        got = HO.run_batch(sp.to_bytes(), 1, case["seed"], chunk_events=chunk, rng_kind=int(case["rng"] == "mt"),
+        got = H.run_batch(sp.to_bytes(), 1, case["seed"], occ=True, chunk_events=chunk, rng_kind=int(case["rng"] == "mt"),
                            uniform=bool(chunk))
         assert int(got["summary"][0, S.S_EVENTS]) == case["events"]
         want = reference_column(doc, case)
-        bad = np.nonzero(got["rows"][:, 0] != want)[0]
-        assert len(bad) == 0, (case["seed"], case["rng"], bad[:8], got["rows"][bad[:4], 0], want[bad[:4]])
+        bad = np.nonzero(got["occ"][:, 0] != want)[0]
+        assert len(bad) == 0, (case["seed"], case["rng"], bad[:8], got["occ"][bad[:4], 0], want[bad[:4]])
 
 
 def _check_oracle(sp, got, seed0, n, rng_kind=0):
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     for r in range(n):
-        want = HO.oracle_occupancy(sp.to_bytes(), seed0 + r, rng_kind)
-        bad = np.nonzero(got["rows"][:, r] != want)[0]
-        assert len(bad) == 0, (r, bad[:8], got["rows"][bad[:4], r], want[bad[:4]])
+        want = OP.oracle_occupancy(sp.to_bytes(), seed0 + r, rng_kind)
+        bad = np.nonzero(got["occ"][:, r] != want)[0]
+        assert len(bad) == 0, (r, bad[:8], got["occ"][bad[:4], r], want[bad[:4]])
 
 
 @pytest.mark.parametrize("mode", ["one_shot", "chunks61", "uniform", "uniform_chunks61"])
@@ -90,7 +91,7 @@ def test_recorder_equals_oracle(name, mode):
     """Every field and bin equals the definition applied to the oracle's state before every event, bit for bit; plain
     and warp-uniform loop, one shot and in chunks of 61 events."""
     sp = _spec_of(name)
-    got = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61 if "chunks" in mode else 0,
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True, chunk_events=61 if "chunks" in mode else 0,
                        uniform=mode.startswith("uniform"))
     _check_oracle(sp, got, SEED, N_REP)
 
@@ -98,20 +99,25 @@ def test_recorder_equals_oracle(name, mode):
 @pytest.mark.parametrize("name", MT_SCENARIOS)
 def test_recorder_equals_oracle_mt19937(name):
     sp = _spec_of(name)
-    _check_oracle(sp, HO.run_batch(sp.to_bytes(), N_REP, 124, chunk_events=61, rng_kind=1), 124, N_REP, rng_kind=1)
+    _check_oracle(sp, H.run_batch(sp.to_bytes(), N_REP, 124, occ=True, chunk_events=61, rng_kind=1), 124, N_REP, rng_kind=1)
 
 
 def test_recorder_head_staged_records(monkeypatch):
     """The head-staged host mode (the running records used where they live)."""
     monkeypatch.setenv("DCSIM_RECORDS", "global")
     sp = _spec_of("cap_greedy_4x64")
-    _check_oracle(sp, HO.run_batch(sp.to_bytes(), N_REP, 124, chunk_events=977), 124, N_REP)
+    _check_oracle(sp, H.run_batch(sp.to_bytes(), N_REP, 124, occ=True, chunk_events=977), 124, N_REP)
+
+
+def _set_quantum(q):
+    H.set_test_time_quantum(q)
+    OP.set_test_time_quantum(q)
 
 
 @pytest.fixture
 def quantum():
-    yield HO.set_test_time_quantum
-    HO.set_test_time_quantum(0.0)
+    yield _set_quantum
+    _set_quantum(0.0)
 
 
 @pytest.mark.parametrize("uniform", [False, True])
@@ -120,7 +126,7 @@ def test_tie_hook_run(quantum, uniform):
     start at the same instant must leave one level of busy GPUs, not two."""
     sp = SC.to_spec(dict(SC.BY_NAME["cfg3_4x64_sinusoid_120s"]), caps={"cap_xfer": 4096})
     quantum(0.25)
-    got = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, uniform=uniform)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True, chunk_events=61, uniform=uniform)
     _check_oracle(sp, got, SEED, N_REP)
 
 
@@ -130,7 +136,7 @@ def test_coverage():
     last_bin = saturated = never_queued = 0
     for name in SCENARIOS:
         sp = _spec_of(name)
-        rows = HO.run_batch(sp.to_bytes(), N_REP, SEED)["rows"]
+        rows = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True)["occ"]
         for d in range(sp.n_dc):
             last_bin += np.count_nonzero(_qbins(rows, sp, d)[-1] > 0)
             saturated += np.count_nonzero(_field(rows, sp, S.OCC_SATURATED_S, d) > 0.5 * rows[0])
@@ -141,8 +147,8 @@ def test_coverage():
 def test_empty_profile():
     """A run that ends before its first event has PROFILE_S = 0 and nothing else."""
     sp = _spec_of("cfg3_4x64_sinusoid_120s", duration=1e-4)
-    got = HO.run_batch(sp.to_bytes(), N_REP, SEED)
-    assert np.all(got["summary"][:, S.S_EVENTS] == 0) and np.all(got["rows"] == 0.0)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True)
+    assert np.all(got["summary"][:, S.S_EVENTS] == 0) and np.all(got["occ"] == 0.0)
     _check_oracle(sp, got, SEED, N_REP)
 
 
@@ -156,12 +162,12 @@ def test_littles_law(name):
     """Q_*_AREA of a DC = sum over the jobs that reached it of min(start, end_time) - xfer_done, RUN_AREA = sum over the
     started jobs of min(finish, end_time) - start, per job type, from the oracle's per-job instants."""
     sp = _spec_of(name)
-    got = HO.run_batch(sp.to_bytes(), N_REP, SEED)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True)
     end = sp.end_time
     checked = 0
     for r in range(N_REP):
-        jobs = HO.oracle_reached(sp.to_bytes(), SEED + r)
-        rows = got["rows"][:, r]
+        jobs = OP.oracle_reached(sp.to_bytes(), SEED + r)
+        rows = got["occ"][:, r]
         for d in range(sp.n_dc):
             at = jobs["dc"] == d
             run = 0.0
@@ -181,9 +187,9 @@ def test_invariants(name):
     """Each DC's queue bins and busy bins sum to PROFILE_S; sum_k k * bin_k of B is the summary's util_gpu_time when the
     bin width is 1; the maxima are integers no larger than the engine's instantaneous S_MAX_Q."""
     sp = _spec_of(name)
-    got = HO.run_batch(sp.to_bytes(), N_REP, SEED)
+    got = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True)
     for r in range(N_REP):
-        rows, summ = got["rows"][:, r], got["summary"][r]
+        rows, summ = got["occ"][:, r], got["summary"][r]
         prof = rows[0]
         assert prof == (sp.end_time - summ[S.S_UTIL_BEGIN] if summ[S.S_EVENTS] else 0.0)
         for d in range(sp.n_dc):
@@ -202,13 +208,13 @@ def test_no_side_effects(name):
     """With the recorder on every summary row is bit-identical to it off, and the power profile's rows with the
     occupancy recorder beside it are bit-identical to the power profile alone."""
     sp = _spec_of(name)
-    off = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, occ=False)
-    on = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61)
-    pp = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, occ=False, pp=True)
-    both = HO.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, pp=True)
+    off = H.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61)
+    on = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True, chunk_events=61)
+    pp = H.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, pp=True)
+    both = H.run_batch(sp.to_bytes(), N_REP, SEED, occ=True, chunk_events=61, pp=True)
     assert np.array_equal(on["summary"], off["summary"]) and on["events"] == off["events"]
     assert np.array_equal(both["summary"], off["summary"])
-    assert np.array_equal(both["pp"], pp["pp"]) and np.array_equal(both["rows"], on["rows"])
+    assert np.array_equal(both["pp"], pp["pp"]) and np.array_equal(both["occ"], on["occ"])
 
 
 def test_mirror_csv_pinned(tmp_path):
@@ -225,16 +231,16 @@ def test_mirror_csv_pinned(tmp_path):
 def test_mirror_on_recorded_rows():
     """The mirror's statistics on real rows: counts, batch means, and pooled curves that are the bins' sums."""
     sp = _spec_of("ragged_3dc_12_5_40")
-    got = HO.run_batch(sp.to_bytes(), 4, SEED)
+    got = H.run_batch(sp.to_bytes(), 4, SEED, occ=True)
     w = [(g.total_gpus + S.OCC_BINS) // S.OCC_BINS for g in sp.dc[:sp.n_dc]]
-    res = EN.occupancy_from_rows(got["rows"], got["summary"], w)
+    res = EN.occupancy_from_rows(got["occ"], got["summary"], w)
     assert res.replicas == 4
     for d in range(sp.n_dc):
-        prof = got["rows"][0]
+        prof = got["occ"][0]
         c = res.column("mean_q_inf", d)
-        assert res.mean[c] == np.sum(_field(got["rows"], sp, S.OCC_Q_INF_AREA, d) / prof) / 4
-        assert np.array_equal(res.queue_curve(d)[1], _qbins(got["rows"], sp, d).sum(axis=1))
-        assert np.array_equal(res.busy_curve(d)[1], _bbins(got["rows"], sp, d).sum(axis=1))
+        assert res.mean[c] == np.sum(_field(got["occ"], sp, S.OCC_Q_INF_AREA, d) / prof) / 4
+        assert np.array_equal(res.queue_curve(d)[1], _qbins(got["occ"], sp, d).sum(axis=1))
+        assert np.array_equal(res.busy_curve(d)[1], _bbins(got["occ"], sp, d).sum(axis=1))
         top = res.time_quantiles("queue", d, [1e-9])[0]
         assert top == np.nonzero(res.queue_curve(d)[1] > 0)[0].max()
 

@@ -7,7 +7,7 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_occ_lib as HO
+import hostemu_lib as H
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import ensemble as E, scenarios as SC, spec as S
 from test_launch_modes_gpu import MODES, SCENARIOS as LM_SCENARIOS, force_mode, spec_for
@@ -85,7 +85,7 @@ def test_every_profile_instantiation(monkeypatch, lanes, mode, cap):
     sc = LM_SCENARIOS[cap]
     sp = spec_for(sc, mode)
     for n in (5, 7):
-        want = HO.run_batch(SC.to_spec(sc).to_bytes(), n, 31)["rows"]
+        want = H.run_batch(SC.to_spec(sc).to_bytes(), n, 31, occ=True)["occ"]
         for chunk in (0, 61):
             with _engine(sp, n, 31) as eng:
                 eng.enable_occupancy()
@@ -130,7 +130,7 @@ def test_bench_batch_with_the_recorder_on():
     assert res.replicas == n and list(widths) == [1] * sp.n_dc
     check_reductions(res, E.occupancy_from_rows(rows, on, widths))
     for r in np.linspace(0, n - 1, 16).astype(np.int64):
-        want = HO.run_batch(sp.to_bytes(), 1, SEED + int(r))["rows"][:, 0]
+        want = H.run_batch(sp.to_bytes(), 1, SEED + int(r), occ=True)["occ"][:, 0]
         assert_close(rows[:, r], want, sp.n_dc, f"replica {r}")
 
 

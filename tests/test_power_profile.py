@@ -9,7 +9,7 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_pp_lib as H
+import hostemu_lib as H
 from distributed_cluster_gpus_b200 import ensemble as E
 from distributed_cluster_gpus_b200 import scenarios as SC
 from distributed_cluster_gpus_b200 import spec as S
@@ -42,7 +42,7 @@ def expected_column(doc, case):
 
 def run_case(doc, case, **kw):
     rng = 1 if case["rng"] == "mt" else 0
-    return H.run_batch(SC.to_spec(doc["scenario"]).to_bytes(), 1, case["seed"], threshold=threshold_of(doc),
+    return H.run_batch(SC.to_spec(doc["scenario"]).to_bytes(), 1, case["seed"], pp=True, pp_threshold=threshold_of(doc),
                        rng_kind=rng, **kw)
 
 
@@ -81,25 +81,25 @@ def test_host_build_equals_reference_fixture_bit_for_bit(name, uniform):
     for case in doc["cases"]:
         got = run_case(doc, case, uniform=uniform)
         assert got["events"] == case["events"], (name, case["seed"], case["rng"])
-        assert_bits(got["rows"][:, 0], expected_column(doc, case), f"{name} {case['rng']} {case['seed']}")
+        assert_bits(got["pp"][:, 0], expected_column(doc, case), f"{name} {case['rng']} {case['seed']}")
 
 
 @pytest.mark.parametrize("name", ["cap_greedy_4x64", "cfg3_4x64_sinusoid_120s", "zero_xfer_4x64_sin10_60s"])
 def test_chunked_and_head_staged_give_identical_rows(name, monkeypatch):
     doc = load(name)
     case = doc["cases"][0]
-    one = run_case(doc, case)["rows"]
+    one = run_case(doc, case)["pp"]
     for chunk in (13, 61):
-        assert_bits(run_case(doc, case, chunk_events=chunk)["rows"], one, f"chunk {chunk}")
+        assert_bits(run_case(doc, case, chunk_events=chunk)["pp"], one, f"chunk {chunk}")
     monkeypatch.setenv("DCSIM_RECORDS", "global")
-    assert_bits(run_case(doc, case, chunk_events=61, uniform=True)["rows"], one, "head-staged, chunked")
+    assert_bits(run_case(doc, case, chunk_events=61, uniform=True)["pp"], one, "head-staged, chunked")
 
 
 def test_summaries_do_not_depend_on_the_recorder():
     for name in ("cap_greedy_4x64", "sweep_joint_nf", "ragged_3dc_12_5_40"):
         blob = SC.to_spec(SC.BY_NAME[name]).to_bytes()
-        on = H.run_batch(blob, 3, 123, threshold=20000.0)
-        off = H.run_batch(blob, 3, 123, record=False)
+        on = H.run_batch(blob, 3, 123, pp=True, pp_threshold=20000.0)
+        off = H.run_batch(blob, 3, 123)
         assert_bits(on["summary"].ravel(), off["summary"].ravel(), name)
 
 
@@ -133,9 +133,9 @@ def test_identities_on_random_scenarios():
         blob = SC.to_spec(sc).to_bytes()
         hi = H.power_range(blob)
         thr = sc["power_cap"] if sc.get("power_cap", 0) > 0 else hi / 4
-        got = H.run_batch(blob, 2, c["run"]["seed"], threshold=thr)
+        got = H.run_batch(blob, 2, c["run"]["seed"], pp=True, pp_threshold=thr)
         assert np.all(got["summary"][:, S.S_STATUS] == 0), sc["name"]
-        check_identities(got["rows"], got["summary"], hi, sc["n_dc"], sc["name"])
+        check_identities(got["pp"], got["summary"], hi, sc["n_dc"], sc["name"])
 
 
 def test_one_level_profile_carries_the_reference_energy():
@@ -144,7 +144,7 @@ def test_one_level_profile_carries_the_reference_energy():
     doc = load("all_off_2x8")
     for case in doc["cases"]:
         got = run_case(doc, case)
-        peak, prof = got["rows"][S.PP_PEAK_W, 0], got["rows"][S.PP_PROFILE_S, 0]
+        peak, prof = got["pp"][S.PP_PEAK_W, 0], got["pp"][S.PP_PROFILE_S, 0]
         e = float.fromhex(case["total_energy_j"])
         assert abs(peak * prof - e) <= 1e-12 * e
 
@@ -161,8 +161,8 @@ def test_numpy_mirror_matches_brute_force():
     blob = SC.to_spec(SC.BY_NAME["ragged_3dc_12_5_40"]).to_bytes()
     n_dc, R = 3, 40
     hi = H.power_range(blob)
-    got = H.run_batch(blob, R, 500, threshold=6000.0)
-    rows, summary = got["rows"], got["summary"].copy()
+    got = H.run_batch(blob, R, 500, pp=True, pp_threshold=6000.0)
+    rows, summary = got["pp"], got["summary"].copy()
     summary[[3, 17], S.S_STATUS] = 4.0                  # two replicas left out
     good = summary[:, S.S_STATUS] == 0
     res = E.power_profile_from_rows(rows, summary, hi, 6000.0)
@@ -190,10 +190,10 @@ def test_numpy_mirror_matches_brute_force():
 
 def test_csv_layout(tmp_path):
     blob = SC.to_spec(SC.BY_NAME["eco_route_cap_2x16"]).to_bytes()
-    got = H.run_batch(blob, 8, 7, threshold=1000.0)
+    got = H.run_batch(blob, 8, 7, pp=True, pp_threshold=1000.0)
     hi = H.power_range(blob)
     for thr in (1000.0, None):
-        res = E.power_profile_from_rows(got["rows"], got["summary"], hi, thr)
+        res = E.power_profile_from_rows(got["pp"], got["summary"], hi, thr)
         p = tmp_path / "pp.csv"
         res.to_csv(str(p), ["dc-a", "dc-b"])
         lines = p.read_text().splitlines()
@@ -211,7 +211,7 @@ def test_csv_layout(tmp_path):
 def test_abi_constants_agree():
     hdr = open(os.path.join(os.path.dirname(POWER_DIR), "..", "..", "include", "dcsim_b200.h")).read()
     assert "#define DCSIM_PP_BINS 1024" in hdr and "DCSIM_PP_FIELDS = 8" in hdr
-    assert S.PP_BINS == E.PP_BINS == H.PP_BINS == 1024 and S.PP_FIELDS == len(E.PP_FIELDS) == H.PP_FIELDS
+    assert S.PP_BINS == E.PP_BINS == 1024 and S.PP_FIELDS == len(E.PP_FIELDS)
 
 
 def test_cli_flags_and_compare_refusal():

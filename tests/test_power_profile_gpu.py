@@ -7,7 +7,7 @@ import sys
 import numpy as np
 import pytest
 
-import hostemu_pp_lib as H
+import hostemu_lib as H
 from conftest import ROOT, has_cuda
 from distributed_cluster_gpus_b200 import ensemble as E, scenarios as SC, spec as S
 from test_power_profile import FIXTURES, NF, expected_column, load, threshold_of
@@ -85,7 +85,7 @@ def test_bench_batch_with_the_recorder_on():
     assert np.all(lo_e <= energy * (1 + 1e-12)) and np.all(energy <= hi_e * (1 + 1e-12))
     ids = np.linspace(0, n - 1, 64).astype(np.int64)
     for r in ids:
-        want = H.run_batch(sp.to_bytes(), 1, 123 + int(r), threshold=30000.0)["rows"][:, 0]
+        want = H.run_batch(sp.to_bytes(), 1, 123 + int(r), pp=True, pp_threshold=30000.0)["pp"][:, 0]
         assert_close(rows[:, r], want, f"replica {r}")
     assert res.replicas == n and res.n[S.PP_PEAK_W] == n
     mirror = E.power_profile_from_rows(rows, on, hi, 30000.0)

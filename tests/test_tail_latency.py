@@ -1,5 +1,5 @@
 """Per-run tail latency on the CPU: the recorder and the selection pass of the device source (host build,
-tests/hostemu_ens/hostemu_tail.cpp) against numpy's inverted_cdf order statistics over the oracle's per-job instants
+tests/hostemu) against numpy's inverted_cdf order statistics over the oracle's per-job instants
 (tests/oracle_jobs/oracle_tail.c) and against golden columns from the unmodified reference; the selection pass alone on
 synthetic edge cases; the off switch; the numpy mirror's CSV against a pinned fixture; and the CLI."""
 import importlib.util
@@ -10,7 +10,8 @@ import os
 import numpy as np
 import pytest
 
-import hostemu_tail_lib as HT
+import hostemu_lib as H
+import oracle_probes_lib as OP
 from conftest import GOLDEN_DIR
 from distributed_cluster_gpus_b200 import ensemble as EN, scenarios as SC, spec as S
 
@@ -28,6 +29,11 @@ FIXTURES = ["cfg3_4x64_sinusoid_120s", "cap_greedy_4x64", "sweep_eco_route", "ra
 TAIL_GOLDEN = os.path.join(GOLDEN_DIR, "tail")
 
 
+def _run(blob, n, seed0, **kw):
+    """The host build with the tail recorder alone among the finish-time recorders (it alone then sets finish_rec)."""
+    return H.run_batch(blob, n, seed0, tail=True, lat_hist=False, prepass=True, **kw)
+
+
 def same(a, b):
     """Bit-identical, NaN where the other is NaN."""
     a, b = np.asarray(a, dtype=np.float64), np.asarray(b, dtype=np.float64)
@@ -40,8 +46,8 @@ def _check(sp, got, seed0, n, rng_kind=0):
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     for r in range(n):
         created = int(got["summary"][r, S.S_JOBS_CREATED])
-        dev = HT.jobs_from_slots(got["slots"][r], got["arr_t"][r], got["arr_tx"][r], got["arr_meta"][r], created)
-        ora = HT.oracle_created(sp.to_bytes(), seed0 + r, rng_kind)
+        dev = H.jobs_from_slots(got["tail"][r], got["arr_t"][r], got["arr_tx"][r], got["arr_meta"][r], created)
+        ora = OP.oracle_created(sp.to_bytes(), seed0 + r, rng_kind)
         assert len(ora) == created
         for f in ("jtype", "dc"):
             assert np.array_equal(dev[f], ora[f]), (r, f)
@@ -52,10 +58,10 @@ def _check(sp, got, seed0, n, rng_kind=0):
             assert same(dev[f][fin], ora[f][fin]), (r, f)
         assert same(dev["xfer_done"][fin], ora["xfer_done"][fin])
         want = EN.tail_rows_from_jobs([ora], [0], sp.n_dc, SLA)[:, 0]
-        assert same(got["cols"][:, r], want), (r, np.argwhere(~((got["cols"][:, r] == want) | np.isnan(want)))[:5].ravel())
-        unf = sum(got["cols"][S.tail_col(sp.n_dc, jt, S.TAIL_UNFINISHED), r] for jt in range(2))
+        assert same(got["tail_cols"][:, r], want), (r, np.argwhere(~((got["tail_cols"][:, r] == want) | np.isnan(want)))[:5].ravel())
+        unf = sum(got["tail_cols"][S.tail_col(sp.n_dc, jt, S.TAIL_UNFINISHED), r] for jt in range(2))
         assert unf == created - got["summary"][r, S.S_JOBS_FINISHED]
-        per_dc = sum(got["cols"][S.tail_col(sp.n_dc, jt, S.TAIL_JOBS, d), r] for jt in range(2) for d in range(sp.n_dc))
+        per_dc = sum(got["tail_cols"][S.tail_col(sp.n_dc, jt, S.TAIL_JOBS, d), r] for jt in range(2) for d in range(sp.n_dc))
         assert per_dc == got["summary"][r, S.S_JOBS_FINISHED]
 
 
@@ -65,8 +71,8 @@ def test_columns_equal_numpy_over_oracle_jobs(name, mode):
     """Every column of every replica is numpy's inverted_cdf order statistic (and count, max, SLA bit) over the oracle's
     per-job instants, bit for bit; plain and warp-uniform loop, one shot and in chunks of 61 events."""
     sp = SC.to_spec(SC.BY_NAME[name])
-    got = HT.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61 if "chunks" in mode else 0,
-                       uniform=mode.startswith("uniform"), sla_s=SLA)
+    got = _run(sp.to_bytes(), N_REP, SEED, chunk_events=61 if "chunks" in mode else 0,
+               uniform=mode.startswith("uniform"), tail_sla=SLA)
     _check(sp, got, SEED, N_REP)
 
 
@@ -74,7 +80,7 @@ def test_head_staged_records(monkeypatch):
     """The head-staged host mode (the running records used where they live)."""
     monkeypatch.setenv("DCSIM_RECORDS", "global")
     sp = SC.to_spec(SC.BY_NAME["cap_greedy_4x64"])
-    _check(sp, HT.run_batch(sp.to_bytes(), 2, SEED, chunk_events=977, sla_s=SLA), SEED, 2)
+    _check(sp, _run(sp.to_bytes(), 2, SEED, chunk_events=977, tail_sla=SLA), SEED, 2)
 
 
 def test_fixtures_reach_their_edges():
@@ -82,7 +88,7 @@ def test_fixtures_reach_their_edges():
     unfinished jobs and empty groups."""
     def cols(name):
         sp = SC.to_spec(SC.BY_NAME[name])
-        return sp, HT.run_batch(sp.to_bytes(), N_REP, SEED, sla_s=SLA)["cols"]
+        return sp, _run(sp.to_bytes(), N_REP, SEED, tail_sla=SLA)["tail_cols"]
     sp, c = cols("short_0p3s_4x64")
     jobs = c[[S.tail_col(sp.n_dc, jt, S.TAIL_JOBS, d) for jt in range(2) for d in range(-1, sp.n_dc)]]
     assert np.any(jobs == 1) and np.any(jobs == 2)
@@ -95,10 +101,15 @@ def test_fixtures_reach_their_edges():
     assert np.all(c[S.tail_col(sp.n_dc, 0, S.TAIL_UNFINISHED)] > 0)
 
 
+def _set_quantum(q):
+    H.set_test_time_quantum(q)
+    OP.set_test_time_quantum(q)
+
+
 @pytest.fixture
 def quantum():
-    yield HT.set_test_time_quantum
-    HT.set_test_time_quantum(0.0)
+    yield _set_quantum
+    _set_quantum(0.0)
 
 
 def test_tie_hook_run(quantum):
@@ -106,13 +117,13 @@ def test_tie_hook_run(quantum):
     oracle's instants."""
     sp = SC.to_spec(dict(SC.BY_NAME["cfg3_4x64_sinusoid_120s"]), caps={"cap_xfer": 4096})
     quantum(0.25)
-    _check(sp, HT.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, uniform=True, sla_s=SLA), SEED, N_REP)
+    _check(sp, _run(sp.to_bytes(), N_REP, SEED, chunk_events=61, uniform=True, tail_sla=SLA), SEED, N_REP)
 
 
 def test_mt19937_replicas():
     """MT19937 replicas (the stock reference's generator)."""
     sp = SC.to_spec(SC.BY_NAME["ragged_3dc_12_5_40"])
-    _check(sp, HT.run_batch(sp.to_bytes(), 2, 123, rng_kind=1, sla_s=SLA), 123, 2, rng_kind=1)
+    _check(sp, _run(sp.to_bytes(), 2, 123, rng_kind=1, tail_sla=SLA), 123, 2, rng_kind=1)
 
 
 GOLDEN_FILES = sorted(f for f in os.listdir(TAIL_GOLDEN) if f.endswith(".json"))
@@ -126,12 +137,12 @@ def test_golden_from_reference(fname):
         doc = json.load(f)
     sp = SC.to_spec(doc["scenario"])
     for case in doc["cases"]:
-        got = HT.run_batch(sp.to_bytes(), 1, case["seed"], rng_kind=1 if case["rng"] == "mt" else 0,
-                           sla_s=doc["meta"]["sla_s"])
+        got = _run(sp.to_bytes(), 1, case["seed"], rng_kind=1 if case["rng"] == "mt" else 0,
+                   tail_sla=doc["meta"]["sla_s"])
         assert got["summary"][0, S.S_JOBS_CREATED] == case["jobs_created"]
         assert got["summary"][0, S.S_JOBS_FINISHED] == case["jobs_finished"]
         want = np.array([np.nan if v is None else float.fromhex(v) for v in case["cols"]])
-        assert same(got["cols"][:, 0], want), (fname, case["seed"], case["rng"])
+        assert same(got["tail_cols"][:, 0], want), (fname, case["seed"], case["rng"])
 
 
 def test_golden_covers_the_edges():
@@ -148,8 +159,8 @@ def test_summaries_unchanged_by_the_recorder(name):
     """With the recorder on (the records then carry the job id) every summary row is bit-identical to the recorder
     off."""
     sp = SC.to_spec(SC.BY_NAME[name])
-    on = HT.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, sla_s=SLA)
-    off = HT.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, tail=False)
+    on = _run(sp.to_bytes(), N_REP, SEED, chunk_events=61, tail_sla=SLA)
+    off = H.run_batch(sp.to_bytes(), N_REP, SEED, chunk_events=61, lat_hist=False)
     assert same(on["summary"], off["summary"]) and on["events"] == off["events"]
 
 
@@ -182,7 +193,7 @@ def test_selection_matches_numpy(n, kind):
     tx = rng.uniform(0.0, 1.0, n)
     start = tx + wait
     finish = start + lat
-    cols = HT.select_synthetic(tx, start, finish)
+    cols = H.select_synthetic(tx, start, finish)
     kinds = (finish - start, start - tx, finish)
     for k, v in enumerate(kinds):
         base = S.tail_col(1, 0, S.TAIL_STATS_BASE + k * 5)
@@ -216,17 +227,17 @@ def test_selection_unfinished_types_and_status():
     fin = ~np.isnan(finish)
     p99 = np.quantile((finish - start)[fin & (jt == 0)], 0.99, method="inverted_cdf")
     for sla, want in ((p99, 1.0), (np.nextafter(p99, 0.0), 0.0), (None, np.nan)):
-        cols = HT.select_synthetic(tx, start, finish, jt, sla_s=sla)
+        cols = H.select_synthetic(tx, start, finish, jt, sla_s=sla)
         assert same(cols[S.tail_sla_col(1, 0, 0)], want)
         for t in range(2):
             assert cols[S.tail_col(1, t, S.TAIL_JOBS)] == np.count_nonzero(fin & (jt == t))
             assert cols[S.tail_col(1, t, S.TAIL_UNFINISHED)] == np.count_nonzero(~fin & (jt == t))
             v = (finish - start)[fin & (jt == t)]
             assert same(cols[S.tail_col(1, t, S.TAIL_STATS_BASE + 2)], np.quantile(v, 0.99, method="inverted_cdf"))
-    only_inf = HT.select_synthetic(tx, start, finish, np.zeros(n, dtype=np.int32), sla_s=1.0)
+    only_inf = H.select_synthetic(tx, start, finish, np.zeros(n, dtype=np.int32), sla_s=1.0)
     assert np.isnan(only_inf[S.tail_sla_col(1, 0, 1)]) and not np.isnan(only_inf[S.tail_sla_col(1, 0, 0)])
-    assert np.all(np.isnan(HT.select_synthetic(tx, start, finish, jt, sla_s=1.0, status=4.0)))
-    empty = HT.select_synthetic(np.zeros(0), np.zeros(0), np.zeros(0), sla_s=1.0)
+    assert np.all(np.isnan(H.select_synthetic(tx, start, finish, jt, sla_s=1.0, status=4.0)))
+    empty = H.select_synthetic(np.zeros(0), np.zeros(0), np.zeros(0), sla_s=1.0)
     assert np.all(empty[[S.tail_col(1, t, f, d) for t in range(2) for d in (-1, 0) for f in (0, 1)]] == 0)
     assert np.all(np.isnan(empty[[S.tail_sla_col(1, k, t) for k in range(3) for t in range(2)]]))
 

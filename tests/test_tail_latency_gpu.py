@@ -13,7 +13,8 @@ import sys
 import numpy as np
 import pytest
 
-import hostemu_tail_lib as HT
+import hostemu_lib as H
+import oracle_probes_lib as OP
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import ensemble as E, scenarios as SC, spec as S
 from test_launch_modes_gpu import SCENARIOS as LM_SCENARIOS, force_mode, spec_for
@@ -72,10 +73,10 @@ def check_replica(sp, rows, slots, pre, i, r, summ, seed, rng_kind=0):
     """Replica r (row i of the pre-pass arrays): the columns are numpy's order statistics over the device's own
     instants bit for bit; the instants and columns are the oracle's within RTOL, counts exact."""
     created = int(summ[r, S.S_JOBS_CREATED])
-    dev = HT.jobs_from_slots(slots[r], pre["arr_t"][i], pre["arr_tx"][i], pre["arr_meta"][i], created)
+    dev = H.jobs_from_slots(slots[r], pre["arr_t"][i], pre["arr_tx"][i], pre["arr_meta"][i], created)
     want = E.tail_rows_from_jobs([dev], [0], sp.n_dc, SLA)[:, 0]
     assert same(rows[:, r], want), (r, np.argwhere(~((rows[:, r] == want) | np.isnan(want)))[:5].ravel())
-    ora = HT.oracle_created(sp.to_bytes(), seed + r, rng_kind)
+    ora = OP.oracle_created(sp.to_bytes(), seed + r, rng_kind)
     assert len(ora) == created
     assert np.array_equal(dev["jtype"], ora["jtype"]) and np.array_equal(dev["dc"], ora["dc"])
     fin = ~np.isnan(ora["finish"])
