@@ -96,7 +96,7 @@ class BatchedEngine:
         if cuda_stream:
             self.set_stream(cuda_stream)
         self._trace_cap = self._jobs_cap = self._cluster_cap = 0
-        self._ens_cap = 0
+        self._ens_cap, self._ens_on = 0, False
         self._jens_windows, self._jens_bin = 0, None
 
     @classmethod
@@ -201,11 +201,11 @@ class BatchedEngine:
         N.check(self._lib.dcsim_enable_cluster_ensemble(self._h, int(max_ticks or 0)), self._h)
         cap = C.c_uint32(0)
         N.check(self._lib.dcsim_cluster_ensemble_capacity(self._h, C.byref(cap)), self._h)
-        self._ens_cap = int(cap.value)
+        self._ens_cap, self._ens_on = int(cap.value), True
 
     @property
     def cluster_ensemble_capacity(self) -> int:
-        """Log ticks the recorder holds (0: not enabled)."""
+        """Log ticks the recorder holds (0: not enabled, or a spec without a log tick: log_interval > duration)."""
         return self._ens_cap
 
     def _ens_check(self, rc):
@@ -218,7 +218,7 @@ class BatchedEngine:
     def cluster_ensemble_rows(self) -> np.ndarray:
         """[ticks, FIELDS, n_dc, n_replicas] float64, ticks = the most any replica recorded; NaN where a replica did not
         reach a tick.  Raises RecorderOverflow if a replica went past the capacity.  For tests and small batches."""
-        if not self._ens_cap:
+        if not self._ens_on:
             raise RuntimeError("cluster ensemble not enabled (enable_cluster_ensemble)")
         ticks = min(int(self.summary()[:, S.S_EV_LOG].max()), self._ens_cap)
         out = np.empty((ticks, ENS_FIELDS, self.spec.n_dc, self.n_replicas), dtype=np.float64)

@@ -1,7 +1,7 @@
 /*
  * TEST-ONLY.  The oracle probes of the CPU tests in one library: the C oracle (oracle/dcsim_oracle.c, unchanged) and,
  * on top of it, the per-job instants (oracle_jobs.c), the per-arrival record (oracle_lists.c), the occupancy checkers
- * (oracle_occ.c) and every created job (oracle_tail.c).  Nothing here is part of, linked into, or reachable from the
+ * (oracle_occ.c), every created job (oracle_tail.c) and the power profile (oracle_power.c).  Nothing here is part of, linked into, or reachable from the
  * product library.  The oracle's tie hook is its own dcoracle_set_test_time_quantum.
  */
 #include "../../oracle/dcsim_oracle.c"
@@ -10,3 +10,4 @@
 #include "oracle_lists.c"
 #include "oracle_occ.c"
 #include "oracle_tail.c"
+#include "oracle_power.c"

@@ -1,5 +1,5 @@
 """TEST-ONLY ctypes access to the probes of the stepped C oracle (tests/oracle_jobs/oracle_probes.c): per-job instants,
-the per-arrival record, the occupancy checkers and every created job."""
+the per-arrival record, the occupancy checkers, every created job and the power profile."""
 import ctypes as C
 import os
 import subprocess
@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _DIR = os.path.join(_HERE, "oracle_jobs")
 _SO = os.path.join(_DIR, "_build", "liboracle_probes.so")
 _SRCS = tuple(os.path.join(_DIR, f) for f in ("oracle_probes.c", "oracle_jobs.c", "oracle_lists.c", "oracle_occ.c",
-                                              "oracle_tail.c", "build.sh")) + (
+                                              "oracle_tail.c", "oracle_power.c", "build.sh")) + (
     os.path.join(_HERE, "..", "oracle", "dcsim_oracle.c"), os.path.join(_HERE, "..", "include", "dcsim_b200.h"))
 JOB_ROW_DTYPE = np.dtype([("jid", "<u4"), ("dc", "<i4"), ("jtype", "<i4"), ("at_xfer", "<i4"), ("arrival", "<f8"),
                           ("xfer_done", "<f8"), ("start", "<f8"), ("finish", "<f8")])
@@ -38,6 +38,8 @@ def lib():
                             ("oracletail_run", [C.c_uint32])):
             getattr(L, name).restype = C.c_longlong
             getattr(L, name).argtypes = [vp, C.c_size_t, u64, C.c_int, vp] + extra
+        L.oraclepower_profile.restype = C.c_longlong
+        L.oraclepower_profile.argtypes = [vp, C.c_size_t, u64, C.c_int, vp, C.c_double, C.c_double]
         _lib = L
     return _lib
 
@@ -80,6 +82,24 @@ def oracle_occupancy(spec_bytes, seed, rng_kind=0):
     n_dc = S.Spec.from_buffer_copy(spec_bytes).n_dc
     row = np.zeros(1 + S.OCC_FIELDS * n_dc + 2 * S.OCC_BINS * n_dc)
     if lib().oracleocc_occupancy(spec_bytes, len(spec_bytes), seed & (2**64 - 1), rng_kind, row.ctypes.data) < 0:
+        raise ValueError("the oracle rejected the spec blob")
+    return row
+
+
+def oracle_power_profile(spec_bytes, seed, threshold, rng_kind=0, hi=None):
+    """One replica's power-profile column [PP_FIELDS + n_dc + PP_BINS] from the oracle stepped one event at a time,
+    over `threshold` (+inf: none).  `hi`: the histogram range; None takes the library's (dcsim_power_profile_range
+    through the host build), which tests/test_power_profile.py pins against the reference fixtures."""
+    if hi is None:
+        import hostemu_lib
+        hi = hostemu_lib.power_range(spec_bytes)
+    n_dc = S.Spec.from_buffer_copy(spec_bytes).n_dc
+    row = np.zeros(S.PP_FIELDS + n_dc + S.PP_BINS)
+    n = lib().oraclepower_profile(spec_bytes, len(spec_bytes), seed & (2**64 - 1), rng_kind, row.ctypes.data,
+                                  float(threshold), float(hi))
+    if n == -2:
+        raise AssertionError("the oracle's DCs accrued energy at different instants")
+    if n < 0:
         raise ValueError("the oracle rejected the spec blob")
     return row
 

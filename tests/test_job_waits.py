@@ -43,11 +43,11 @@ def expected_rows(jobs, n_dc, bin_s, end_time):
     return rows, hist
 
 
-def _check(sp, got, seed0, n, bin_s):
+def _check(sp, got, seed0, n, bin_s, rng_kind=0):
     assert np.all(got["summary"][:, S.S_STATUS] == 0)
     all_jobs = []
     for r in range(n):
-        jobs = OP.oracle_jobs(sp.to_bytes(), seed0 + r)
+        jobs = OP.oracle_jobs(sp.to_bytes(), seed0 + r, rng_kind)
         assert len(jobs) == got["summary"][r, S.S_JOBS_FINISHED]
         rows, hist = expected_rows(jobs, sp.n_dc, bin_s, sp.end_time)
         assert np.array_equal(got["jwait"][..., r], rows), (r, np.argwhere(got["jwait"][..., r] != rows)[:5])
