@@ -35,6 +35,7 @@ EXPORTS = (
     "dcsim_occupancy_spread",
     "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs", "dcsim_tail_latency_moments",
     "dcsim_tail_latency_spread",
+    "dcsim_enable_energy_cost", "dcsim_fetch_energy_cost", "dcsim_energy_cost_moments", "dcsim_energy_cost_spread",
 )
 
 _lib = None
@@ -190,6 +191,15 @@ def load():
         L.dcsim_power_profile_moments.argtypes = [vp, vp]
         L.dcsim_power_profile_spread.restype = i32
         L.dcsim_power_profile_spread.argtypes = [vp, vp, vp, vp, vp, vp]
+    if hasattr(L, "dcsim_enable_energy_cost"):
+        L.dcsim_enable_energy_cost.restype = i32
+        L.dcsim_enable_energy_cost.argtypes = [vp]
+        L.dcsim_fetch_energy_cost.restype = i32
+        L.dcsim_fetch_energy_cost.argtypes = [vp, vp, C.c_size_t]
+        L.dcsim_energy_cost_moments.restype = i32
+        L.dcsim_energy_cost_moments.argtypes = [vp, vp]
+        L.dcsim_energy_cost_spread.restype = i32
+        L.dcsim_energy_cost_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

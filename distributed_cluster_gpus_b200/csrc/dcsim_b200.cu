@@ -396,6 +396,17 @@ struct dcsim_ens_pp_src {
   }
 };
 
+/* Energy cost: column c = n contiguous doubles ([DCSIM_COST_COLS(n_dc)][n]), counted by the replicas with status 0; no
+ * integer columns. */
+struct dcsim_ens_cost_src {
+  const double* cost;
+  const uint32_t* status;
+  uint64_t n;
+  using view = dcsim_ens_pp_src::view;
+  __device__ __forceinline__ view at(uint64_t col) const { return view{cost + col * n, status}; }
+  __device__ __forceinline__ bool integral(uint64_t) const { return false; }
+};
+
 /* Occupancy: the first DCSIM_OCC_FIELDS * n_dc columns are the statistics (field, dc) — the stored per-DC field over
  * PROFILE_S, the two maxima as stored — then the 2 * DCSIM_OCC_BINS * n_dc bins as stored
  * ([1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n], column c of the source at stored column 1 + c).  A
@@ -603,6 +614,8 @@ struct dcsim {
   double* d_jres;          /* [jens_windows + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas] job resources (opt-in) */
   uint32_t* d_jres_cnt;    /* [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] mix, then [n_dc][2][DCSIM_JRES_EBINS][n_replicas]
                               energy bins */
+  double* d_cost;          /* [DCSIM_COST_COLS(n_dc)][n_replicas] energy cost and carbon (opt-in) */
+  double* d_cost_work;     /* [n_replicas][n_dc][DCSIM_COSTW_N] its working state */
   uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the job ensemble and power profile
                          reductions, refreshed on the stream ahead of every one of them (status_words) */
   unsigned long long events_seen;
@@ -647,6 +660,12 @@ static uint64_t occ_cols(const dcsim_t* h) { return occ_stat_cols(h) + 2ull * DC
 static size_t occ_bytes(const dcsim_t* h) { return (size_t)(1 + occ_cols(h)) * (size_t)h->n_replicas * sizeof(double); }
 static size_t occ_work_bytes(const dcsim_t* h) {
   return (size_t)h->n_replicas * (size_t)h->spec.n_dc * DCSIM_OCCW_N * sizeof(double);
+}
+
+static uint64_t cost_cols(const dcsim_t* h) { return (uint64_t)DCSIM_COST_COLS(h->spec.n_dc); }
+static size_t cost_bytes(const dcsim_t* h) { return (size_t)cost_cols(h) * (size_t)h->n_replicas * sizeof(double); }
+static size_t cost_work_bytes(const dcsim_t* h) {
+  return (size_t)h->n_replicas * (size_t)h->spec.n_dc * DCSIM_COSTW_N * sizeof(double);
 }
 
 static size_t tail_slot_bytes(const dcsim_t* h) { return (size_t)h->n_replicas * (size_t)h->g->cap_arr * 2 * sizeof(double); }
@@ -1065,6 +1084,10 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_occ, 0, occ_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_occ_work, 0, occ_work_bytes(h), h->g->stream));
   }
+  if (h->d_cost) {
+    CUDA_TRY(h, cudaMemsetAsync(h->d_cost, 0, cost_bytes(h), h->g->stream));
+    CUDA_TRY(h, cudaMemsetAsync(h->d_cost_work, 0, cost_work_bytes(h), h->g->stream));
+  }
   if (h->d_jwait) {
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, (h->jens_windows + 1) * jwait_row_bytes(h), h->g->stream));
     CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
@@ -1156,6 +1179,7 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
   P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
   P->occ = h->d_occ; P->occ_work = h->d_occ_work;
+  P->cost = h->d_cost; P->cost_work = h->d_cost_work;
   P->jres = h->d_jres; P->jres_mix = h->d_jres_cnt;
   P->jres_hist = h->d_jres ? h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas : NULL;
   dcsim_derive_kparams(P);
@@ -1751,6 +1775,51 @@ int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double*
   return ens_spread(h, src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
+int dcsim_enable_energy_cost(dcsim_t* h) {
+  if (!h) return DCSIM_E_INVALID;
+  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_energy_cost on a member of a shared group%s%lld");
+  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_energy_cost must precede the first advance%s%lld");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+  if (!h->d_cost) {
+    const int rc = recorder_alloc(h, (void**)&h->d_cost, cost_bytes(h), (void**)&h->d_cost_work, cost_work_bytes(h),
+                                  "enable_energy_cost: %s%lld bytes of device memory do not fit (run fewer replicas)",
+                                  (long long)(cost_bytes(h) + cost_work_bytes(h)));
+    if (rc != DCSIM_OK) return rc;
+  }
+  CUDA_TRY(h, cudaMemsetAsync(h->d_cost, 0, cost_bytes(h), h->g->stream));
+  CUDA_TRY(h, cudaMemsetAsync(h->d_cost_work, 0, cost_work_bytes(h), h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  const int rc = recorder_ready(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
+  if (rc != DCSIM_OK) return rc;
+  if (out_bytes < cost_bytes(h))
+    return set_err(h, DCSIM_E_INVALID, "fetch_energy_cost: buffer too small (need %s%lld bytes)", "", (long long)cost_bytes(h));
+  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_cost, cost_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
+  return DCSIM_OK;
+}
+
+int dcsim_energy_cost_moments(dcsim_t* h, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_cost_src src{h->d_cost, h->d_status, h->n_replicas};
+  return ens_moments(h, src, h->n_replicas, cost_cols(h), dev_out);
+}
+
+int dcsim_energy_cost_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                             double* dev_m2_out, uint64_t* dev_hist_out) {
+  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
+  const int rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
+  if (rc != DCSIM_OK) return rc;
+  const dcsim_ens_cost_src src{h->d_cost, h->d_status, h->n_replicas};
+  return ens_spread(h, src, h->n_replicas, cost_cols(h), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
+}
+
 int dcsim_enable_tail_latency(dcsim_t* h, double sla_s) {
   if (!h) return DCSIM_E_INVALID;
   if (!(sla_s >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_tail_latency: sla_s must be >= 0 (+inf: none)%s%lld");
@@ -1955,6 +2024,7 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
   cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
   cudaFree(h->d_occ); cudaFree(h->d_occ_work);
+  cudaFree(h->d_cost); cudaFree(h->d_cost_work);
   cudaFree(h->d_tail); cudaFree(h->d_tail_cols);
   cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
   cudaFree(h->d_jres); cudaFree(h->d_jres_cnt);

@@ -524,6 +524,8 @@ struct dcsim_kparams_t {
                            L.lean == 0), or NULL */
   uint32_t* jres_mix;   /* [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] (n, f) mix counts (with jres) */
   uint32_t* jres_hist;  /* [n_dc][2][DCSIM_JRES_EBINS][n_replicas] energy-per-job histograms (with jres) */
+  double* cost;         /* [DCSIM_COST_COLS(n_dc)][n_replicas] energy cost and carbon, or NULL */
+  double* cost_work;    /* [n_replicas][n_dc][DCSIM_COSTW_N] its working state (with cost) */
 };
 
 /* ---- small typed views ------------------------------------------------------------------------ */
@@ -544,6 +546,7 @@ struct dcsim_ctx_t {
   bool occ;              /* the occupancy recorder runs: likewise */
   bool tail;             /* the tail-latency recorder runs: likewise */
   bool jres;             /* the job-resources recorder runs: likewise */
+  bool cost;             /* the energy-cost recorder runs: likewise */
   bool quiet;            /* a ghost lane group of an in-place launch, whose blk is replica n-1's live block in HBM: it must
                             not even publish the pop-min cache there.  A compile-time false in the staged and head-staged
                             instantiations (a ghost's blk is its own shared-memory slot there) */
@@ -1497,7 +1500,7 @@ static inline void dcsim_derive_kparams(dcsim_kparams_t* P) {
 }
 /* Host code: the launch runs the instantiation with the profile recorders (dcsim_replica_step<..., PP = true>). */
 static inline bool dcsim_profile_recorders(const dcsim_kparams_t* P) {
-  return P->pp != nullptr || P->occ != nullptr || P->tail != nullptr || P->jres != nullptr;
+  return P->pp != nullptr || P->occ != nullptr || P->tail != nullptr || P->jres != nullptr || P->cost != nullptr;
 }
 
 DCSIM_DEV bool dcsim_same_bits(double a, double b) { return dcsim_hi(a) == dcsim_hi(b) && dcsim_lo(a) == dcsim_lo(b); }
@@ -1557,6 +1560,70 @@ DCSIM_COLD void dcsim_pp_touch(const dcsim_kparams_t* P, char* blk, uint32_t r, 
   dcsim_pp_segment(P, w, r, now, p, pd);
 }
 
+/* ---- energy cost (opt-in: P->cost; layout and definitions in include/dcsim_b200.h) ---------------------------------
+ * The power profile's hook, per DC: the state that held over (TC_d, now] is still in DF_POWER[d] when its first write of
+ * a later instant comes, so the recorder hangs off those writes and the tail, with no per-event work.  Its working state
+ * is a row of DCSIM_COSTW_N doubles per replica and DC in HBM (zeroed by enable / reset); every instant in it is > 0
+ * once set, so 0.0 reads as "not yet".  The hourly energies accumulate in the replica's own HOUR_J columns. */
+enum {
+  DCSIM_COSTW_TC = 0, /* DC d's last change point: its energy is accounted up to here */
+  DCSIM_COSTW_LVL_S,  /* start of its open level (0: none opened yet) */
+  DCSIM_COSTW_LVL_P,  /* its power */
+  DCSIM_COSTW_N
+};
+
+DCSIM_DEV double* dcsim_cost_row(const dcsim_kparams_t* P, uint32_t r, int d, double t0) {
+  double* w = P->cost_work + ((uint64_t)r * P->spec.n_dc + d) * DCSIM_COSTW_N;
+  if (w[DCSIM_COSTW_TC] == 0.0) w[DCSIM_COSTW_TC] = t0;
+  return w;
+}
+
+/* The hour window k of an instant a >= 0: 3600 k <= a < 3600 (k + 1), decided on the exact products. */
+DCSIM_DEV double dcsim_cost_window(double a) {
+  double k = floor(a / 3600.0);
+  if (3600.0 * k > a) k -= 1.0;
+  else if (3600.0 * (k + 1.0) <= a) k += 1.0;
+  return k;
+}
+
+/* Level [s, e] of DC d at power p closes: cut at every hour boundary strictly inside it, each piece adding p * length to
+ * its hour of day, in time order (one writer per replica). */
+DCSIM_DEV void dcsim_cost_close(const dcsim_kparams_t* P, uint32_t r, int d, double s, double e, double p) {
+  const uint64_t n = P->n_replicas;
+  double* o = P->cost + (uint64_t)DCSIM_COST_HOUR_J(P->spec.n_dc, d, 0) * n + r;
+  double k = dcsim_cost_window(s), a = s;
+  for (;;) {
+    const double b = 3600.0 * (k + 1.0);
+    const bool cut = b < e;
+    o[(uint64_t)fmod(k, (double)DCSIM_HOURS) * n] += p * ((cut ? b : e) - a);
+    if (!cut) break;
+    a = b; k += 1.0;
+  }
+}
+
+/* DC d's power p held over (TC_d, now]: extend its open level or close it and open the next one at TC_d.  Nothing when
+ * the interval is empty. */
+DCSIM_DEV void dcsim_cost_segment(const dcsim_kparams_t* P, double* w, uint32_t r, int d, double now, double p) {
+  const double tc = w[DCSIM_COSTW_TC];
+  if (!(now > tc)) return;
+  if (w[DCSIM_COSTW_LVL_S] == 0.0) {
+    w[DCSIM_COSTW_LVL_S] = tc; w[DCSIM_COSTW_LVL_P] = p;
+  } else if (!dcsim_same_bits(p, w[DCSIM_COSTW_LVL_P])) {
+    dcsim_cost_close(P, r, d, w[DCSIM_COSTW_LVL_S], tc, w[DCSIM_COSTW_LVL_P]);
+    w[DCSIM_COSTW_LVL_S] = tc; w[DCSIM_COSTW_LVL_P] = p;
+  }
+  w[DCSIM_COSTW_TC] = now;
+}
+
+/* Lane 0, before a write of DF_POWER[d] at instant `now`: the state in it held over (TC_d, now].  Before the first
+ * processed event (DF_UTIL_BEGIN still 0.0) nothing accrues, so nothing is recorded. */
+DCSIM_COLD void dcsim_cost_touch(const dcsim_kparams_t* P, char* blk, uint32_t r, int d, double now) {
+  const struct { char* blk; } v = {blk};
+  const double t0 = DCF(v, DF_UTIL_BEGIN)[0];
+  if (t0 == 0.0) return;
+  dcsim_cost_segment(P, dcsim_cost_row(P, r, d, t0), r, d, now, DCF(v, DF_POWER)[d]);
+}
+
 /* Lane 0.  DC d's estimated power as SIM:168-179 computes it on every event: the running jobs' powers summed in
  * dict (= start) order from 0.0 — kept in DF_PSUM, see there — then the idle term. */
 DCSIM_DEV void dcsim_refresh_power(dcsim_ctx_t& c, int d) {
@@ -1564,6 +1631,7 @@ DCSIM_DEV void dcsim_refresh_power(dcsim_ctx_t& c, int d) {
   const int idle = cfg.total_gpus - DCI(c, DI_BUSY)[d];
   const double p_idle = (double)idle * (cfg.power_gating ? cfg.p_sleep : cfg.p_idle);
   if (c.pp) dcsim_pp_touch(c.P, c.blk, c.r, c.now);
+  if (c.cost) dcsim_cost_touch(c.P, c.blk, c.r, d, c.now);
   DCF(c, DF_POWER)[d] = DCF(c, DF_PSUM)[d] + p_idle;
 }
 
@@ -2563,6 +2631,40 @@ DCSIM_COLD void dcsim_pp_tail(const dcsim_kparams_t* P, char* blk, uint32_t r, d
   for (int d = 0; d < sp.n_dc; ++d) o[(uint64_t)(DCSIM_PP_FIELDS + d) * n] = w[DCSIM_PPW_DC_PEAK + d];
 }
 
+/* Lane 0, once, after the tail: every DC's last state up to the last event (`last`), then the tail interval with the
+ * tail's own power; closes the open levels and writes the replica's derived columns.  Nothing when no event was
+ * processed (`last` == 0): every column stays 0. */
+DCSIM_COLD void dcsim_cost_tail(const dcsim_kparams_t* P, char* blk, uint32_t r, double last) {
+  if (last == 0.0) return;
+  const struct { char* blk; } v = {blk};
+  const dcsim_spec_t& sp = P->spec;
+  const int nd = sp.n_dc;
+  const uint64_t n = P->n_replicas;
+  const double t0 = DCF(v, DF_UTIL_BEGIN)[0];
+  double* o = P->cost + r;
+  double tot_j = 0.0, tot_usd = 0.0, tot_g = 0.0;
+  for (int d = 0; d < nd; ++d) {
+    double* w = dcsim_cost_row(P, r, d, t0);
+    dcsim_cost_segment(P, w, r, d, last, DCF(v, DF_POWER)[d]);
+    dcsim_cost_segment(P, w, r, d, sp.end_time, dcsim_tail_power(sp.dc[d], DCI(v, DI_BUSY)[d], DCF(v, DF_CUR_FREQ)[d]));
+    if (w[DCSIM_COSTW_LVL_S] != 0.0) dcsim_cost_close(P, r, d, w[DCSIM_COSTW_LVL_S], w[DCSIM_COSTW_TC], w[DCSIM_COSTW_LVL_P]);
+    double ej = 0.0, usd = 0.0;
+    for (int h = 0; h < DCSIM_HOURS; ++h) {
+      const double e = o[(uint64_t)DCSIM_COST_HOUR_J(nd, d, h) * n];
+      ej += e;
+      usd += (e / 3.6e6) * sp.dc[d].price_kwh[h];
+    }
+    const double g = (ej / 3.6e6) * sp.dc[d].carbon_intensity;
+    o[(uint64_t)DCSIM_COST_ENERGY_J(nd, d) * n] = ej;
+    o[(uint64_t)DCSIM_COST_USD(nd, d) * n] = usd;
+    o[(uint64_t)DCSIM_COST_CARBON_G(nd, d) * n] = g;
+    tot_j += ej; tot_usd += usd; tot_g += g;
+  }
+  o[(uint64_t)DCSIM_COST_TOTAL_J(nd) * n] = tot_j;
+  o[(uint64_t)DCSIM_COST_TOTAL_USD(nd) * n] = tot_usd;
+  o[(uint64_t)DCSIM_COST_TOTAL_G(nd) * n] = tot_g;
+}
+
 /* Lane 0, once, after the tail: every DC's final state over (TC_d, end_time], then its open levels close at end_time;
  * writes PROFILE_S.  Nothing else when no event was processed (`last` == 0): the profile stays empty. */
 DCSIM_COLD void dcsim_occ_tail(const dcsim_kparams_t* P, char* blk, uint32_t r, double last) {
@@ -2712,6 +2814,7 @@ DCSIM_DEV uint32_t dcsim_replica_run(dcsim_ctx_t& c, bool live) {
     dcsim_replica_tail(c);
     if (c.lane == 0 && c.pp) dcsim_pp_tail(c.P, c.blk, c.r, c.now);
     if (c.lane == 0 && c.occ) dcsim_occ_tail(c.P, c.blk, c.r, c.now);
+    if (c.lane == 0 && c.cost) dcsim_cost_tail(c.P, c.blk, c.r, c.now);
     if (c.lane == 0) c.H->done = 1u;
     dcsim_warp_sync();
   }
@@ -2783,6 +2886,7 @@ DCSIM_DEV uint32_t dcsim_replica_step(const dcsim_kparams_t* P, uint64_t r, char
   c.occ = PP && !ghost && P->occ != nullptr;
   c.tail = PP && !ghost && P->tail != nullptr;
   c.jres = PP && !ghost && P->jres != nullptr;
+  c.cost = PP && !ghost && P->cost != nullptr;
   c.quiet = INPLACE && ghost;
   if (ghost) { /* a lane group without a replica (the batch's last warp): reads whatever is there, writes nothing to a
                   replica's state (staged modes: its own shared-memory slot takes the pop-min cache; in place: quiet) */

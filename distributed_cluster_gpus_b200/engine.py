@@ -441,6 +441,33 @@ class BatchedEngine:
         N.check(self._lib.dcsim_occupancy_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
                                                  C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
+    # -- energy cost and carbon (ensemble.energy_cost turns it into batch statistics) --------------------------------
+    def enable_energy_cost(self):
+        """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records each
+        DC's energy by hour of day, its cost under the DC's hourly tariff and its carbon (include/dcsim_b200.h
+        DCSIM_COST_*).  Runs the event-loop instantiation with the profile recorders compiled in."""
+        N.check(self._lib.dcsim_enable_energy_cost(self._h), self._h)
+        self._cost_on = True
+
+    @property
+    def energy_cost_enabled(self) -> bool:
+        return getattr(self, "_cost_on", False)
+
+    def energy_cost_rows(self) -> np.ndarray:
+        """[cost_cols(n_dc), n_replicas] float64: every replica's raw columns.  For tests and small batches."""
+        rows = np.empty((S.cost_cols(self.spec.n_dc), self.n_replicas), dtype=np.float64)
+        N.check(self._lib.dcsim_fetch_energy_cost(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
+        return rows
+
+    def energy_cost_moments_into(self, device_ptr: int):
+        """Pass 1 on the handle's stream: [4][cost_cols(n_dc)] float64 {n, sum, min, max} at ``device_ptr``."""
+        N.check(self._lib.dcsim_energy_cost_moments(self._h, C.c_void_p(device_ptr)), self._h)
+
+    def energy_cost_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 on the handle's stream over every column: sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        N.check(self._lib.dcsim_energy_cost_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
+                                                   C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+
     # -- per-run tail latency (ensemble.tail_latency turns it into batch statistics) ----------------------------------
     def enable_tail_latency(self, sla_s=None):
         """Opt-in, before the first advance of a batch (stays on across reset, cleared by it): every finished job's start
@@ -608,11 +635,11 @@ def _pp_key(power_profile, power_threshold):
 
 
 def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False,
-               occupancy=False, tail=None, job_resources=False):
+               occupancy=False, tail=None, job_resources=False, energy_cost=False):
     # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
             os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None),
-            bool(occupancy), tail, bool(job_resources and job_bin is not None))
+            bool(occupancy), tail, bool(job_resources and job_bin is not None), bool(energy_cost))
 
 
 def _tail_key(tail_latency, tail_sla_s):
@@ -628,17 +655,17 @@ def _drop_parked_batch_engine():
 
 def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
                    job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                   occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False):
+                   occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False, energy_cost=False):
     """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
     ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
     power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
     response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on;
     ``tail_latency``: with the per-run tail-latency recorder on, SLA ``tail_sla_s`` seconds (None: none);
-    ``job_resources``: with the job-resources recorder on (it implies the job ensemble).  A parked engine is only reused
-    by a caller that asks for the same recorders."""
+    ``job_resources``: with the job-resources recorder on (it implies the job ensemble); ``energy_cost``: with the
+    energy-cost recorder on.  A parked engine is only reused by a caller that asks for the same recorders."""
     job_bin = _job_bin(sp, job_ensemble or job_waits or job_resources, job_ensemble_bin)
     key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
-                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s), job_resources)
+                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s), job_resources, energy_cost)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -663,6 +690,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
             eng.enable_occupancy()
         if tail_latency:
             eng.enable_tail_latency(tail_sla_s)
+        if energy_cost:
+            eng.enable_energy_cost()
     except BaseException:
         eng.close()
         raise
@@ -679,7 +708,7 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
                                                         _pp_key(eng.power_profile_enabled, eng.power_threshold),
                                                         eng.job_waits_enabled, eng.occupancy_enabled,
                                                         _tail_key(eng.tail_latency_enabled, eng.tail_latency_sla),
-                                                        eng.job_resources_enabled)
+                                                        eng.job_resources_enabled, eng.energy_cost_enabled)
 
 
 def free_cached_engine():
@@ -729,7 +758,7 @@ class LoggedReplica:
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
                       max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
                       job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                      occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False):
+                      occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False, energy_cost=False):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
@@ -739,13 +768,13 @@ def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, d
     None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble);
     ``occupancy``: with the occupancy recorder on; ``tail_latency``: with the per-run tail-latency recorder on
     (``tail_sla_s``: its SLA [s], None = none), its slot buffer sized by each attempt's cap_arrivals; ``job_resources``:
-    with the job-resources recorder on (and the job ensemble)."""
+    with the job-resources recorder on (and the job ensemble); ``energy_cost``: with the energy-cost recorder on."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
         eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
                              job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy,
-                             tail_latency, tail_sla_s, job_resources)
+                             tail_latency, tail_sla_s, job_resources, energy_cost)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

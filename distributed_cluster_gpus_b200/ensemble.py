@@ -1366,3 +1366,123 @@ def tail_latency_from_jobs(jobs: Sequence[np.ndarray], status, n_dc: int, sla_s=
     """The numpy mirror end to end: per replica its created jobs (TAIL_JOB_DTYPE) and status word -> the per-run
     columns with np.quantile(..., method="inverted_cdf") -> batch statistics through host_passes."""
     return tail_latency_from_rows(tail_rows_from_jobs(jobs, status, n_dc, sla_s), status, sla_s, quantiles)
+
+
+# ---- energy cost and carbon ------------------------------------------------------------------------------------------
+COST_FIELDS = ("energy_j", "cost_usd", "carbon_g")    # per DC and for the cluster (DCSIM_COST_*)
+COST_CSV_HEADER = ["dc", "field", "carbon_g_per_kwh"] + PP_CSV_HEADER[2:]
+J_PER_KWH = 3.6e6
+
+
+def _cost_columns(n_dc: int):
+    """(field, dc, hour) of every stored column in the recorder's order; dc = -1: the cluster, hour = -1: none."""
+    cols = [("hour_j", d, h) for d in range(n_dc) for h in range(24)]
+    cols += [(f, d, -1) for f in COST_FIELDS for d in range(n_dc)]
+    return tuple(cols + [(f, -1, -1) for f in COST_FIELDS])
+
+
+@dataclass
+class EnergyCostResult:
+    """Batch statistics of the energy-cost recorder over the replicas with status 0.  ``n`` ... ``max`` and ``quantiles``
+    ([Q, columns]) cover ``columns`` = (field, dc, hour): the 24 hourly energies of each DC, energy, cost and carbon per
+    DC, then the cluster totals (dc = -1).  ``sum`` [columns]: the pooled sums over those replicas.  ``price_kwh``
+    [n_dc, 24] and ``carbon_intensity`` [n_dc] are the tables the columns were priced with."""
+    columns: Tuple[Tuple[str, int, int], ...]
+    n: np.ndarray
+    mean: np.ndarray
+    std: np.ndarray                                    # unbiased (ddof = 1); 0 for a single sample
+    min: np.ndarray
+    max: np.ndarray
+    q: Tuple[float, ...]
+    quantiles: np.ndarray
+    sum: np.ndarray
+    price_kwh: np.ndarray
+    carbon_intensity: np.ndarray
+
+    def column(self, field: str, dc: int = -1, hour: int = -1) -> int:
+        """Column of ``field`` (COST_FIELDS, or "hour_j" with an ``hour``) of DC ``dc`` (-1: the cluster)."""
+        return self.columns.index((field, dc, hour))
+
+    @property
+    def replicas(self) -> int:
+        return int(self.n[-1]) if len(self.n) else 0
+
+    def hourly(self, dc: int) -> dict:
+        """DC ``dc``'s 24 hourly energy bands over the replicas: {"mean", "std", "min", "max": [24], "quantiles":
+        [Q, 24]} [J], hour of day 0 .. 23."""
+        c = [self.column("hour_j", dc, h) for h in range(24)]
+        return {"mean": self.mean[c], "std": self.std[c], "min": self.min[c], "max": self.max[c],
+                "quantiles": self.quantiles[:, c]}
+
+    def pooled(self) -> dict:
+        """The pooled energy [kWh], cost [USD] and carbon [g] of every replica that counts, and the effective USD/kWh
+        (pooled cost over pooled kWh) and g/kWh, per DC (index) and for the cluster (key "cluster")."""
+        def one(dc):
+            kwh = float(self.sum[self.column("energy_j", dc)]) / J_PER_KWH
+            usd = float(self.sum[self.column("cost_usd", dc)])
+            g = float(self.sum[self.column("carbon_g", dc)])
+            return {"energy_kwh": kwh, "cost_usd": usd, "carbon_g": g,
+                    "usd_per_kwh": usd / kwh if kwh > 0 else float("nan"), "g_per_kwh": g / kwh if kwh > 0 else float("nan")}
+        out = {d: one(d) for d in range(len(self.carbon_intensity))}
+        out["cluster"] = one(-1)
+        out["replicas"] = self.replicas
+        return out
+
+    def to_csv(self, path: str, dc_names: Sequence[str]):
+        """Long format: dc,field,carbon_g_per_kwh,n,mean,std,min,p05,p25,p50,p75,p95,p99,max — per DC energy_j, cost_usd,
+        carbon_g and hour_j_00 .. hour_j_23 with the DC's carbon intensity (0 for a DC the carbon map leaves out), then
+        the cluster's energy_j, cost_usd and carbon_g (dc and carbon_g_per_kwh empty)."""
+        fmt = lambda x: repr(float(x))  # noqa: E731
+        D = len(self.carbon_intensity)
+        rows = [r for d in range(D) for r in [(d, (f, d, -1), f) for f in COST_FIELDS]
+                + [(d, ("hour_j", d, h), f"hour_j_{h:02d}") for h in range(24)]]
+        rows += [(-1, (f, -1, -1), f) for f in COST_FIELDS]
+        with open(path, "w", newline="") as fh:
+            w = csv.writer(fh)
+            w.writerow(COST_CSV_HEADER)
+            for d, key, name in rows:
+                c = self.columns.index(key)
+                head = [dc_names[d], name, fmt(self.carbon_intensity[d])] if d >= 0 else ["", name, ""]
+                w.writerow(head + [int(self.n[c]), fmt(self.mean[c]), fmt(self.std[c]), fmt(self.min[c])]
+                           + [fmt(self.quantiles[j, c]) for j in range(len(self.q))] + [fmt(self.max[c])])
+
+
+def cost_finalize(mom, m2, hist, n_dc: int, price_kwh, carbon_intensity, quantiles: Sequence[float] = PP_CSV_QUANTILES
+                  ) -> EnergyCostResult:
+    """All-reduced moments, m2 and histograms over the energy-cost columns -> statistics."""
+    cols = _cost_columns(n_dc)
+    mom = np.asarray(mom, dtype=np.float64)
+    st = column_stats(mom, np.asarray(m2), np.asarray(hist), np.zeros(len(cols), dtype=bool), quantiles)
+    return EnergyCostResult(columns=cols, **st.result_fields((len(cols),)), sum=mom[1].copy(),
+                            price_kwh=np.asarray(price_kwh, dtype=np.float64).reshape(n_dc, 24),
+                            carbon_intensity=np.asarray(carbon_intensity, dtype=np.float64).reshape(n_dc))
+
+
+def _cost_tables(sp):
+    return ([[sp.dc[d].price_kwh[h] for h in range(24)] for d in range(sp.n_dc)],
+            [sp.dc[d].carbon_intensity for d in range(sp.n_dc)])
+
+
+def energy_cost(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> EnergyCostResult:
+    """Statistics of the energy-cost recorder of ``engine`` (a finished BatchedEngine with enable_energy_cost()), over
+    all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
+    import torch
+    from . import spec as S
+    if not engine.energy_cost_enabled:
+        raise RuntimeError("energy cost not enabled (enable_energy_cost)")
+    dev = torch.device("cuda", engine.device)
+    n_dc = engine.spec.n_dc
+    passes = device_passes(dev, S.cost_cols(n_dc), engine.energy_cost_moments_into, engine.energy_cost_spread_into)
+    return cost_finalize(*passes, n_dc, *_cost_tables(engine.spec), quantiles)
+
+
+def energy_cost_from_rows(rows: np.ndarray, status, price_kwh, carbon_intensity,
+                          quantiles: Sequence[float] = PP_CSV_QUANTILES) -> EnergyCostResult:
+    """The same statistics from host columns [cost columns, R] (BatchedEngine.energy_cost_rows), the replicas' status
+    words and the tables ([n_dc, 24] USD/kWh, [n_dc] gCO2/kWh) through the numpy mirror of both passes.  All-reduced
+    over the ranks like energy_cost."""
+    rows = np.asarray(rows, dtype=np.float64)
+    n_dc = (rows.shape[0] - 3) // 27
+    ok = np.broadcast_to((np.asarray(status) == 0)[None, :], rows.shape)
+    passes = host_passes(rows, ok, np.zeros(rows.shape[0], dtype=bool))
+    return cost_finalize(*passes, n_dc, price_kwh, carbon_intensity, quantiles)

@@ -84,6 +84,10 @@ def parse_args(argv=None):
                    help="write batch statistics of every run's own exact p50 / p95 / p99 / p99.9 / max of service, "
                         "wait and response time per job type and DC, its finished and unfinished jobs, and whether its "
                         "p99 met --sla_p99_ms, to this file")
+    p.add_argument("--energy-cost-csv", type=str, default=None, metavar="PATH",
+                   help="write batch statistics of every DC's energy, electricity cost under its hourly tariff and "
+                        "carbon, the 24 hourly energy bands per DC, and the cluster totals over all replicas, to this "
+                        "file")
     p.add_argument("--power-profile-csv", type=str, default=None, metavar="PATH",
                    help="write batch statistics of every replica's cluster power over time — peak, time and energy over "
                         "--power-threshold, longest excursion, per-DC peaks — and the pooled power-duration curve's "
@@ -134,7 +138,7 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
         power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None,
         occupancy=args.occupancy_csv is not None, tail_latency=args.tail_latency_csv is not None,
-        job_resources=args.job_resources_csv is not None)
+        job_resources=args.job_resources_csv is not None, energy_cost=args.energy_cost_csv is not None)
     return sim
 
 
@@ -176,6 +180,7 @@ def main(argv=None):
     _add_occupancy(stats, sim.occupancy, sim)
     _add_tail_latency(stats, sim.tail_latency)
     _add_job_resources(stats, sim.job_resources, sim)
+    _add_energy_cost(stats, sim.energy_cost, sim)
     _report(args, stats)
     return sim
 
@@ -195,6 +200,8 @@ def _write_ensemble(args, sim):
         sim.tail_latency.to_csv(args.tail_latency_csv, [dc.name for dc in sim.dcs.values()])
     if args.job_resources_csv:
         sim.job_resources.to_csv(args.job_resources_csv, [dc.name for dc in sim.dcs.values()])
+    if args.energy_cost_csv:
+        sim.energy_cost.to_csv(args.energy_cost_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -233,6 +240,21 @@ def _add_tail_latency(stats, res):
     the mean / p05 / p50 / p95 over the runs of the per-run p99."""
     if res is not None:
         stats["tail_latency"] = res.pooled()
+
+
+def _add_energy_cost(stats, res, sim):
+    """For --summary-json: pooled energy [kWh], cost [USD], carbon [g] and the effective USD/kWh and g/kWh, per DC and
+    for the cluster, and the batch mean / min / max of each run's cluster cost and carbon."""
+    if res is None:
+        return
+    names = [dc.name for dc in sim.dcs.values()]
+    pooled = res.pooled()
+    out = {"replicas": pooled["replicas"], "cluster": pooled["cluster"],
+           "dc": {names[d]: dict(pooled[d], carbon_g_per_kwh=float(res.carbon_intensity[d])) for d in range(len(names))}}
+    for f in ("cost_usd", "carbon_g"):
+        c = res.column(f)
+        out[f"run_{f}"] = {"mean": float(res.mean[c]), "min": float(res.min[c]), "max": float(res.max[c])}
+    stats["energy_cost"] = out
 
 
 def _add_job_resources(stats, res, sim):
@@ -291,6 +313,8 @@ def _main_sharded(args, world, rank):
         raise SystemExit("--tail-latency-csv needs at least one replica per rank")
     if args.job_resources_csv and count == 0:
         raise SystemExit("--job-resources-csv needs at least one replica per rank")
+    if args.energy_cost_csv and count == 0:
+        raise SystemExit("--energy-cost-csv needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -329,6 +353,7 @@ def _main_sharded(args, world, rank):
         _add_occupancy(stats, sim.occupancy, sim)
         _add_tail_latency(stats, sim.tail_latency)
         _add_job_resources(stats, sim.job_resources, sim)
+        _add_energy_cost(stats, sim.energy_cost, sim)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -358,6 +383,9 @@ def _main_compare(args, world, rank):
     if args.job_resources_csv:
         raise SystemExit("--job-resources-csv is not available with --compare-algos (run each algo on its own for its "
                          "GPU, frequency and energy-per-job statistics)")
+    if args.energy_cost_csv:
+        raise SystemExit("--energy-cost-csv is not available with --compare-algos (run each algo on its own for its "
+                         "electricity cost and carbon)")
     if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
         raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
                          "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")

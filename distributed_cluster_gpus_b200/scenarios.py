@@ -20,14 +20,23 @@ SLOW_WAN = dict(capacity_gbps=1.0)
 
 def scenario(name, n_dc, gpus_per_dc, inf, trn, duration, freq_levels=None, algo="default_policy",
              policy="energy_aware", log_interval=5.0, power_cap=0.0, num_fixed_gpus=1, fixed_freq=None,
-             gpus_list=None, wan=None):
+             gpus_list=None, wan=None, energy_price=None):
     sc = {"name": name, "n_dc": n_dc, "gpus_per_dc": gpus_per_dc, "gpus_list": gpus_list,
           "freq_levels": list(freq_levels or FREQ8), "inf": dict(inf), "trn": dict(trn),
           "duration": float(duration), "algo": algo, "policy": policy, "log_interval": float(log_interval),
           "power_cap": float(power_cap), "num_fixed_gpus": int(num_fixed_gpus), "fixed_freq": fixed_freq}
     if wan is not None:   # only when given: every scenario without it keeps the reference's own WAN (and its fixture)
         sc["wan"] = {k: float(v) for k, v in wan.items()}
+    if energy_price is not None:  # a per-DC tariff {dc: {hour: USD/kWh}} in place of paper_config's; hours as strings (JSON)
+        sc["energy_price"] = {dc: {str(h): float(p) for h, p in hours.items()} for dc, hours in energy_price.items()}
     return sc
+
+
+def energy_price_of(sc):
+    """The tariff a scenario runs under: its own per-DC map (SIM:986-1005's {dc: {hour: price}} form) or paper_config's."""
+    if "energy_price" not in sc:
+        return _pc.build_energy_price()
+    return {dc: {int(h): float(p) for h, p in hours.items()} for dc, hours in sc["energy_price"].items()}
 
 
 # BASELINE.json configs, with the durations fixed once here (SURVEY.md §8(d) caveat iii)
@@ -95,7 +104,7 @@ def build_inputs(sc):
                                                        sc.get("wan"))
     return dict(ingresses=ingresses, dcs=dcs, graph=graph, arrival_inf=ArrivalConfig(**sc["inf"]),
                 arrival_train=ArrivalConfig(**sc["trn"]), coeffs_map=coeffs,
-                carbon_intensity=_pc.build_carbon_intensity(), energy_price=_pc.build_energy_price(),
+                carbon_intensity=_pc.build_carbon_intensity(), energy_price=energy_price_of(sc),
                 policy=_pc.build_policy(name=sc["policy"]))
 
 

@@ -62,7 +62,7 @@ class MultiIngressPaperSimulator:
                  cuda_stream: int = 0, keep_engine: bool = True, rng: str = "philox", cluster_ensemble: bool = False,
                  job_ensemble: bool = False, job_ensemble_bin: Optional[float] = None, power_profile: bool = False,
                  power_threshold: Optional[float] = None, job_waits: bool = False, occupancy: bool = False,
-                 tail_latency: bool = False, job_resources: bool = False):
+                 tail_latency: bool = False, job_resources: bool = False, energy_cost: bool = False):
         self.ingresses, self.dcs, self.graph = ingresses, dcs, graph
         self.arr_inf, self.arr_trn = arrival_inf, arrival_train
         self.router_policy = router_policy          # stored, never consulted — as in the reference (SIM:65)
@@ -124,6 +124,10 @@ class MultiIngressPaperSimulator:
         # whose p99 met sla_p99_ms, ensemble.TailLatencyResult
         self._want_tail_latency = bool(tail_latency)
         self.tail_latency = None
+        # energy_cost=True: after run(), statistics over all replicas (all ranks, as above) of every DC's energy by hour
+        # of day, its cost under the DC's hourly tariff and its carbon, ensemble.EnergyCostResult
+        self._want_energy_cost = bool(energy_cost)
+        self.energy_cost = None
         # job_resources=True: after run(), per finish window of job_ensemble_bin seconds and for the whole run, statistics
         # of every finished job's GPU count, frequency and predicted energy E_pred * size over all replicas (all ranks, as
         # above), the pooled (n, f) mix and energy-per-job quantiles, ensemble.JobResourcesResult.  It runs the job
@@ -184,7 +188,7 @@ class MultiIngressPaperSimulator:
                                           job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
                                           power_threshold=self._power_threshold, job_waits=self._want_job_waits,
                                           occupancy=self._want_occupancy, tail_latency=self._want_tail_latency,
-                                          job_resources=self._want_job_resources,
+                                          job_resources=self._want_job_resources, energy_cost=self._want_energy_cost,
                                           tail_sla_s=float(self.sla_p99_ms) / 1000.0)
         except BaseException:
             if companion is not None:
@@ -215,6 +219,9 @@ class MultiIngressPaperSimulator:
             if self._want_job_resources:
                 from ..ensemble import job_resources
                 self.job_resources = job_resources(eng)
+            if self._want_energy_cost:
+                from ..ensemble import energy_cost
+                self.energy_cost = energy_cost(eng)
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

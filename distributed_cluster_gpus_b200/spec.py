@@ -60,6 +60,42 @@ def tail_cols(n_dc: int) -> int:
     return 2 * (n_dc + 1) * TAIL_GROUP_FIELDS + 2 * len(TAIL_KINDS)
 
 
+# energy-cost columns (DCSIM_COST_*): HOUR_J per (dc, hour), then ENERGY_J, COST_USD and CARBON_G per DC, then the three
+# cluster totals
+COST_WORK_DOUBLES = 3  # the recorder's working row per replica and DC
+
+
+def cost_hour_j(n_dc: int, dc: int, hour: int) -> int:
+    return dc * HOURS + hour
+
+
+def cost_energy_j(n_dc: int, dc: int) -> int:
+    return HOURS * n_dc + dc
+
+
+def cost_usd(n_dc: int, dc: int) -> int:
+    return (HOURS + 1) * n_dc + dc
+
+
+def cost_carbon_g(n_dc: int, dc: int) -> int:
+    return (HOURS + 2) * n_dc + dc
+
+
+def cost_totals(n_dc: int):
+    """(TOTAL_J, TOTAL_USD, TOTAL_G) columns."""
+    base = (HOURS + 3) * n_dc
+    return base, base + 1, base + 2
+
+
+def cost_cols(n_dc: int) -> int:
+    return (HOURS + 3) * n_dc + 3
+
+
+def cost_bytes_per_replica(n_dc: int) -> int:
+    """Device bytes per replica of the energy-cost recorder: its columns and its working rows."""
+    return 8 * (cost_cols(n_dc) + COST_WORK_DOUBLES * n_dc)
+
+
 def tail_col(n_dc: int, jt: int, field: int, dc: int = -1) -> int:
     """Column of group (jt, dc) (dc = -1: all DCs) and field (TAIL_JOBS, TAIL_UNFINISHED or TAIL_STATS_BASE + kind * 5 +
     stat)."""

@@ -540,6 +540,48 @@ int dcsim_power_profile_moments(dcsim_t* h, double* dev_out);
 int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                                double* dev_m2_out, uint64_t* dev_hist_out);
 
+/* Energy cost and carbon: for EVERY replica and DC d, the energy d drew in each hour of the day, priced at d's hourly
+ * tariff (price_kwh[d][h], USD/kWh) and weighted by its carbon intensity (carbon_intensity[d], gCO2/kWh).
+ *   - P_d(t) is the step function d's energy integrates: over each inter-event interval (t_{k-1}, t_k] the estimate the
+ *     per-event accrual uses (SIM:168-179, 437) as it stood after event k-1; over the tail (t_last, end_time] the tail's
+ *     own power (instantaneous_power_w at current_freq, models.py:82-91).  It starts at the first processed event
+ *     (DCSIM_S_UTIL_BEGIN); a replica without one has an empty profile (every column 0).
+ *   - A LEVEL of DC d is a maximal run of positive-length intervals whose P_d are bitwise equal (the power profile's
+ *     rule, per DC).
+ *   - Hour windows are [3600 k, 3600 (k + 1)], boundaries exact doubles.  A level [s, e] is cut at every boundary
+ *     strictly inside it; a piece [a, b] lies in window k = floor(a / 3600), corrected so that 3600 k <= a < 3600 (k + 1)
+ *     holds for the exact products, and goes to hour of day h = k mod 24 (simulated time 0 is midnight, _current_hour).
+ *   - E[d][h] = sum of P * (b - a) over the pieces in hour h, in time order (levels of several days fold into one h).
+ * Per replica, columns:
+ *   HOUR_J[d][h]   E[d][h]                                             column DCSIM_COST_HOUR_J(n_dc, d, h)
+ *   ENERGY_J[d]    sum over h of E[d][h], in h order                   column DCSIM_COST_ENERGY_J(n_dc, d)
+ *   COST_USD[d]    sum over h of (E[d][h] / 3.6e6) * price_kwh[d][h], in h order (policy_paper._objective_score's)
+ *   CARBON_G[d]    (ENERGY_J[d] / 3.6e6) * carbon_intensity[d]
+ *   TOTAL_J, TOTAL_USD, TOTAL_G   the sums over d in DC order from 0.0
+ * ENERGY_J[d] is NOT DCSIM_SD_ENERGY_J bit for bit: the summary adds one product per event, this column one per level
+ * piece.  The two agree to a relative 1e-10 (the tests pin it).
+ * Device layout [DCSIM_COST_COLS(n_dc)][n_replicas] doubles, replica fastest, plus a working row of 3 doubles per replica
+ * and DC: (27 n_dc + 3) * 8 + 24 n_dc bytes per replica, 984 B at 4 DCs. */
+#define DCSIM_COST_HOUR_J(n_dc, d, h) ((d) * DCSIM_HOURS + (h))
+#define DCSIM_COST_ENERGY_J(n_dc, d) (DCSIM_HOURS * (n_dc) + (d))
+#define DCSIM_COST_USD(n_dc, d) ((DCSIM_HOURS + 1) * (n_dc) + (d))
+#define DCSIM_COST_CARBON_G(n_dc, d) ((DCSIM_HOURS + 2) * (n_dc) + (d))
+#define DCSIM_COST_TOTAL_J(n_dc) ((DCSIM_HOURS + 3) * (n_dc))
+#define DCSIM_COST_TOTAL_USD(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 1)
+#define DCSIM_COST_TOTAL_G(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 2)
+#define DCSIM_COST_COLS(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 3)
+/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  DCSIM_E_STATE after the
+ * first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the rows
+ * and their working state do not fit. */
+int dcsim_enable_energy_cost(dcsim_t* h);
+/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
+int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes);
+/* The two passes over every column and the replicas with status 0: the contract of dcsim_ensemble_moments / _spread
+ * (no integer columns).  Both on the handle's stream, with device pointers. */
+int dcsim_energy_cost_moments(dcsim_t* h, double* dev_out);
+int dcsim_energy_cost_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                             double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Occupancy: for EVERY replica and DC d, how long the queues were and how full the DC was over time.  Step functions over
  * [t0, end_time]: Qi(t) = len(q_inf), Qt(t) = len(q_train), Q = Qi + Qt, N(t) = running jobs, B(t) = busy GPUs.
  *   - t0 is the first processed event (DCSIM_S_UTIL_BEGIN); a replica without one has an empty profile (every field 0).

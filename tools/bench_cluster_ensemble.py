@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy / tail / resources, the job-log
-ensemble / the power profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder / the per-run
-tail-latency recorder / the job-resources recorder on top of the job ensemble) at bench size: the event loop with the recorder off and on, the two reduction kernels, the recorder's bytes per
+"""Cost of the cluster-log ensemble (or, with --recorder job / power / waits / occupancy / tail / resources / cost, the
+job-log ensemble / the power profile / the waiting-time recorder on top of the job ensemble / the occupancy recorder / the
+per-run tail-latency recorder / the job-resources recorder on top of the job ensemble / the energy-cost recorder) at bench size: the event loop with the recorder off and on, the two reduction kernels, the recorder's bytes per
 replica.  One JSON line on stdout; writes nothing else.
 
-    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy|tail|resources] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
+    python tools/bench_cluster_ensemble.py [--recorder cluster|job|power|waits|occupancy|tail|resources|cost] [--replicas 65536] [--scenario cfg3_4x64_sinusoid_120s]
                                            [--rounds 3]
 
 Each batch runs on a fresh engine (two bench-size batches do not fit beside each other), the arms alternate
@@ -30,7 +30,7 @@ def main():
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail", "resources"], default="cluster")
+    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail", "resources", "cost"], default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -59,6 +59,8 @@ def main():
             e.enable_occupancy()
         elif arm == "on" and args.recorder == "tail":
             e.enable_tail_latency(0.5)
+        elif arm == "on" and args.recorder == "cost":
+            e.enable_energy_cost()
         elif arm == "on":
             e.enable_cluster_ensemble()
         return e
@@ -85,6 +87,11 @@ def main():
             cols = (S.OCC_FIELDS + 2 * S.OCC_BINS) * sp.n_dc
             moments_into, spread_into = on.occupancy_moments_into, on.occupancy_spread_into
             rows, recorder_bytes = cols + 1, (cols + 1) * 8 + sp.n_dc * 11 * 8   # columns + working rows (DCSIM_OCCW_N)
+        elif args.recorder == "cost":
+            cols = S.cost_cols(sp.n_dc)
+            moments_into, spread_into = on.energy_cost_moments_into, on.energy_cost_spread_into
+            rows, recorder_bytes = cols, S.cost_bytes_per_replica(sp.n_dc)   # columns + working rows (3 doubles per DC)
+            stats = EN.energy_cost(on).pooled()
         elif args.recorder == "tail":
             cols = S.tail_cols(sp.n_dc)
             moments_into, spread_into = on.tail_latency_moments_into, on.tail_latency_spread_into
@@ -158,6 +165,7 @@ def main():
                       "moments_ms": moments_ms, "spread_ms": spread_ms,
                       **({"waits": stats} if args.recorder == "waits" else {}),
                       **({"resources": stats} if args.recorder == "resources" else {}),
+                      **({"cost": stats} if args.recorder == "cost" else {}),
                       **({"selection_ms": first_moments_ms - moments_ms, "tail": stats} if args.recorder == "tail" else {})}),
           flush=True)
 
