@@ -57,6 +57,13 @@ def latency_quantiles(hist_row, qs=(0.5, 0.9, 0.99)):
 
 RNG_KINDS = {"philox": 0, "mt19937": 1}
 
+# The opt-in batch recorders, in the order their statistics are computed.  Each name is the keyword that turns the
+# recorder on (acquire_engine, run_to_completion, MultiIngressPaperSimulator), the simulator's result attribute and the
+# ensemble function that computes it.  Every one of those functions all-reduces under torch.distributed, so every rank
+# calls them in this order.
+RECORDERS = ("cluster_ensemble", "job_ensemble", "power_profile", "job_waits", "occupancy", "tail_latency",
+             "job_resources", "energy_cost")
+
 
 class RecorderOverflow(RuntimeError):
     """A recorder (0 trace, 1 job log, 2 cluster log, 3 cluster-log ensemble) saw more rows (ensemble: log ticks) than its
@@ -624,27 +631,39 @@ _CACHED = {"key": None, "engine": None}
 _CACHED_LOGGED = {"key": None, "engine": None}   # the one-replica companion engine of LoggedReplica
 
 
-def _job_bin(sp, job_ensemble, job_ensemble_bin):
-    """The job-log ensemble's resolved window width, None when it is off."""
-    return float(job_ensemble_bin or sp.log_interval) if job_ensemble else None
+def _recorders(sp, cluster_ensemble=False, job_ensemble=False, job_ensemble_bin=None, power_profile=False,
+               power_threshold=None, job_waits=False, occupancy=False, tail_latency=False, tail_sla_s=None,
+               job_resources=False, energy_cost=False):
+    """The recorder keywords of acquire_engine -> the BatchedEngine.enable_* calls (name, arguments) that turn those
+    recorders on, in the order they are made: the job ensemble, at its resolved window width, before the waits and
+    job-resources recorders that live in its cells (either one implies it)."""
+    job = job_ensemble or job_waits or job_resources
+    calls = (("enable_cluster_ensemble", cluster_ensemble, ()),
+             ("enable_job_ensemble", job, (float(job_ensemble_bin or sp.log_interval),)),
+             ("enable_job_waits", job_waits, ()),
+             ("enable_job_resources", job_resources, ()),
+             ("enable_power_profile", power_profile, (power_threshold,)),
+             ("enable_occupancy", occupancy, ()),
+             ("enable_tail_latency", tail_latency, (tail_sla_s,)),
+             ("enable_energy_cost", energy_cost, ()))
+    return tuple((name, args) for name, on, args in calls if on)
 
 
-def _pp_key(power_profile, power_threshold):
-    """The power profile's threshold as the engine cache sees it: None when the profile is off, +inf for no threshold."""
-    return (float("inf") if power_threshold is None else float(power_threshold)) if power_profile else None
+def _engine_recorders(eng):
+    """The recorder keywords of acquire_engine that ``eng`` runs with."""
+    return dict(cluster_ensemble=eng.cluster_ensemble_capacity > 0, job_ensemble=eng.job_ensemble_bin is not None,
+                job_ensemble_bin=eng.job_ensemble_bin, power_profile=eng.power_profile_enabled,
+                power_threshold=eng.power_threshold, job_waits=eng.job_waits_enabled, occupancy=eng.occupancy_enabled,
+                tail_latency=eng.tail_latency_enabled, tail_sla_s=eng.tail_latency_sla,
+                job_resources=eng.job_resources_enabled, energy_cost=eng.energy_cost_enabled)
 
 
-def _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble=False, job_bin=None, pp=None, job_waits=False,
-               occupancy=False, tail=None, job_resources=False, energy_cost=False):
-    # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused
+def _cache_key(sp, n_replicas, device, cuda_stream, recorders):
+    # the launch overrides are read when a handle sizes its launch: a parked engine sized under others is not reused.
+    # A threshold or SLA of None is +inf, as in the library.
     return (sp.to_bytes(), int(n_replicas), int(device), int(cuda_stream), os.environ.get("DCSIM_RECORDS", ""),
-            os.environ.get("DCSIM_GROUP", ""), bool(cluster_ensemble), job_bin, pp, bool(job_waits and job_bin is not None),
-            bool(occupancy), tail, bool(job_resources and job_bin is not None), bool(energy_cost))
-
-
-def _tail_key(tail_latency, tail_sla_s):
-    """The tail-latency recorder's SLA as the engine cache sees it: None when the recorder is off, +inf for no SLA."""
-    return (float("inf") if tail_sla_s is None else float(tail_sla_s)) if tail_latency else None
+            os.environ.get("DCSIM_GROUP", ""),
+            tuple((name, tuple(float("inf") if a is None else float(a) for a in args)) for name, args in recorders))
 
 
 def _drop_parked_batch_engine():
@@ -653,19 +672,16 @@ def _drop_parked_batch_engine():
     _CACHED["engine"], _CACHED["key"] = None, None
 
 
-def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, cluster_ensemble=False,
-                   job_ensemble=False, job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                   occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False, energy_cost=False):
-    """A fresh batch; ``cluster_ensemble``: with the cluster-log ensemble recorder on; ``job_ensemble``: with the job-log
-    ensemble recorder on, windows of ``job_ensemble_bin`` seconds (None: log_interval); ``power_profile``: with the
-    power-profile recorder on, threshold ``power_threshold`` watts (None: none); ``job_waits``: with the waiting /
-    response-time recorder on (it implies the job ensemble); ``occupancy``: with the occupancy recorder on;
-    ``tail_latency``: with the per-run tail-latency recorder on, SLA ``tail_sla_s`` seconds (None: none);
-    ``job_resources``: with the job-resources recorder on (it implies the job ensemble); ``energy_cost``: with the
-    energy-cost recorder on.  A parked engine is only reused by a caller that asks for the same recorders."""
-    job_bin = _job_bin(sp, job_ensemble or job_waits or job_resources, job_ensemble_bin)
-    key = _cache_key(sp, n_replicas, device, cuda_stream, cluster_ensemble, job_bin, _pp_key(power_profile, power_threshold),
-                     job_waits, occupancy, _tail_key(tail_latency, tail_sla_s), job_resources, energy_cost)
+def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0, **recorders):
+    """A fresh batch with the recorders of ``recorders`` on (all off by default): ``cluster_ensemble``: the cluster-log
+    ensemble; ``job_ensemble``: the job-log ensemble, windows of ``job_ensemble_bin`` seconds (None: log_interval);
+    ``power_profile``: the power profile, threshold ``power_threshold`` watts (None: none); ``job_waits``: the waiting /
+    response-time recorder (it implies the job ensemble); ``occupancy``: the occupancy recorder; ``tail_latency``: the
+    per-run tail-latency recorder, SLA ``tail_sla_s`` seconds (None: none); ``job_resources``: the job-resources recorder
+    (it implies the job ensemble); ``energy_cost``: the energy-cost recorder.  A parked engine is only reused by a caller
+    that asks for the same recorders."""
+    calls = _recorders(sp, **recorders)
+    key = _cache_key(sp, n_replicas, device, cuda_stream, calls)
     if _CACHED["engine"] is not None and _CACHED["key"] == key:
         eng, _CACHED["engine"], _CACHED["key"] = _CACHED["engine"], None, None
         eng.reset(base_seed, first_replica_id)   # fresh batch: recorders may be re-targeted again
@@ -676,22 +692,8 @@ def acquire_engine(sp, n_replicas, base_seed, first_replica_id=0, device=0, cuda
     _drop_parked_batch_engine()   # (tens of GB: gone before the new batch allocates; the one-replica companion stays)
     eng = BatchedEngine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream)
     try:
-        if cluster_ensemble:
-            eng.enable_cluster_ensemble()
-        if job_bin is not None:
-            eng.enable_job_ensemble(job_bin)
-        if job_waits:
-            eng.enable_job_waits()
-        if job_resources:
-            eng.enable_job_resources()
-        if power_profile:
-            eng.enable_power_profile(power_threshold)
-        if occupancy:
-            eng.enable_occupancy()
-        if tail_latency:
-            eng.enable_tail_latency(tail_sla_s)
-        if energy_cost:
-            eng.enable_energy_cost()
+        for name, args in calls:
+            getattr(eng, name)(*args)
     except BaseException:
         eng.close()
         raise
@@ -703,12 +705,8 @@ def release_engine(eng, sp, device=0, cuda_stream=0):
     parked companion of LoggedReplica is a separate slot and is left alone (closing and re-creating it would cost
     every run() its allocations)."""
     _drop_parked_batch_engine()
-    _CACHED["engine"], _CACHED["key"] = eng, _cache_key(sp, eng.n_replicas, device, cuda_stream, eng.cluster_ensemble_capacity > 0,
-                                                        eng.job_ensemble_bin,
-                                                        _pp_key(eng.power_profile_enabled, eng.power_threshold),
-                                                        eng.job_waits_enabled, eng.occupancy_enabled,
-                                                        _tail_key(eng.tail_latency_enabled, eng.tail_latency_sla),
-                                                        eng.job_resources_enabled, eng.energy_cost_enabled)
+    _CACHED["engine"] = eng
+    _CACHED["key"] = _cache_key(sp, eng.n_replicas, device, cuda_stream, _recorders(sp, **_engine_recorders(eng)))
 
 
 def free_cached_engine():
@@ -756,25 +754,17 @@ class LoggedReplica:
 
 
 def run_to_completion(spec_factory, n_replicas, base_seed, first_replica_id=0, device=0, cuda_stream=0,
-                      max_retries=3, configure=None, while_running=None, cluster_ensemble=False, job_ensemble=False,
-                      job_ensemble_bin=None, power_profile=False, power_threshold=None, job_waits=False,
-                      occupancy=False, tail_latency=False, tail_sla_s=None, job_resources=False, energy_cost=False):
+                      max_retries=3, configure=None, while_running=None, **recorders):
     """Runs all replicas to end_time.  A replica that overflowed a capacity is never trusted: the whole batch
     is re-run with that capacity raised (``spec_factory(caps)`` rebuilds the blob).  Returns (engine, summary);
     hand the engine back with release_engine() (reuse) or close().  ``while_running()`` is called once, after the
     kernels of the first attempt were launched and before the host waits for them (host work that can overlap).
-    ``cluster_ensemble`` / ``job_ensemble``: every attempt runs with that ensemble recorder on (``job_ensemble_bin``: its
-    window width, None = log_interval); ``power_profile``: with the power-profile recorder on (``power_threshold`` [W],
-    None = no threshold); ``job_waits``: with the waiting / response-time recorder on (and the job ensemble);
-    ``occupancy``: with the occupancy recorder on; ``tail_latency``: with the per-run tail-latency recorder on
-    (``tail_sla_s``: its SLA [s], None = none), its slot buffer sized by each attempt's cap_arrivals; ``job_resources``:
-    with the job-resources recorder on (and the job ensemble); ``energy_cost``: with the energy-cost recorder on."""
+    ``recorders``: the recorder keywords of acquire_engine; every attempt runs with those recorders on (the tail-latency
+    slot buffer sized by each attempt's cap_arrivals)."""
     caps = {}
     for attempt in range(max_retries + 1):
         sp = spec_factory(dict(caps))
-        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, cluster_ensemble,
-                             job_ensemble, job_ensemble_bin, power_profile, power_threshold, job_waits, occupancy,
-                             tail_latency, tail_sla_s, job_resources, energy_cost)
+        eng = acquire_engine(sp, n_replicas, base_seed, first_replica_id, device, cuda_stream, **recorders)
         if configure:
             configure(eng)
         eng.advance(0, sync=False)

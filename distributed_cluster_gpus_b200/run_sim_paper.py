@@ -18,6 +18,26 @@ from .simcore.validators import validate_gpus
 
 ALGOS = ["default_policy", "cap_uniform", "cap_greedy", "joint_nf", "bandit", "carbon_cost", "eco_route", "chsac_af",
          "debug"]
+# every batch recorder (engine.RECORDERS, in its order) -> the dest of the --X-csv flag that turns it on and names its
+# file
+RECORDER_CSV = {"cluster_ensemble": "ensemble_csv", "job_ensemble": "job_ensemble_csv",
+                "power_profile": "power_profile_csv", "job_waits": "job_waits_csv", "occupancy": "occupancy_csv",
+                "tail_latency": "tail_latency_csv", "job_resources": "job_resources_csv", "energy_cost": "energy_cost_csv"}
+_ENSEMBLES_REFUSED = ("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
+                      "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")
+# why --compare-algos refuses a recorder's flag (the power profile's also refuses --power-threshold), in the order the
+# flags are checked
+_COMPARE_REFUSALS = {
+    "power_profile": "--power-profile-csv / --power-threshold are not available with --compare-algos (run each algo on "
+                     "its own)",
+    "occupancy": "--occupancy-csv is not available with --compare-algos (run each algo on its own for its occupancy)",
+    "tail_latency": "--tail-latency-csv is not available with --compare-algos (run each algo on its own for its per-run "
+                    "tail latency)",
+    "job_resources": "--job-resources-csv is not available with --compare-algos (run each algo on its own for its GPU, "
+                     "frequency and energy-per-job statistics)",
+    "energy_cost": "--energy-cost-csv is not available with --compare-algos (run each algo on its own for its electricity "
+                   "cost and carbon)",
+    "cluster_ensemble": _ENSEMBLES_REFUSED, "job_ensemble": _ENSEMBLES_REFUSED, "job_waits": _ENSEMBLES_REFUSED}
 
 
 def parse_args(argv=None):
@@ -134,11 +154,8 @@ def build_simulator(args, replicas=None, first_replica_id=0, device=None, write_
         fixed_freq=args.fixed_freq, logger=get_logger(log_dir=out_dir),
         replicas=args.replicas if replicas is None else replicas, first_replica_id=first_replica_id,
         device=args.device if device is None else device, write_logs=write_logs, rng=args.rng,
-        cluster_ensemble=args.ensemble_csv is not None, job_ensemble=args.job_ensemble_csv is not None,
-        job_ensemble_bin=args.job_ensemble_bin, power_profile=args.power_profile_csv is not None,
-        power_threshold=power_threshold(args), job_waits=args.job_waits_csv is not None,
-        occupancy=args.occupancy_csv is not None, tail_latency=args.tail_latency_csv is not None,
-        job_resources=args.job_resources_csv is not None, energy_cost=args.energy_cost_csv is not None)
+        job_ensemble_bin=args.job_ensemble_bin, power_threshold=power_threshold(args),
+        **{name: getattr(args, dest) is not None for name, dest in RECORDER_CSV.items()})
     return sim
 
 
@@ -175,33 +192,25 @@ def main(argv=None):
     _write_ensemble(args, sim)
     stats = batch_statistics(sim.summary)
     _add_latency_quantiles(stats, sim.latency_histogram)
+    _add_recorders(stats, sim)
+    _report(args, stats)
+    return sim
+
+
+def _write_ensemble(args, sim):
+    for name, dest in RECORDER_CSV.items():
+        if getattr(args, dest):
+            getattr(sim, name).to_csv(getattr(args, dest), [dc.name for dc in sim.dcs.values()])
+
+
+def _add_recorders(stats, sim):
+    """The batch recorders' figures for --summary-json, each only when its recorder ran."""
     _add_power_profile(stats, sim.power_profile)
     _add_job_waits(stats, sim.job_waits)
     _add_occupancy(stats, sim.occupancy, sim)
     _add_tail_latency(stats, sim.tail_latency)
     _add_job_resources(stats, sim.job_resources, sim)
     _add_energy_cost(stats, sim.energy_cost, sim)
-    _report(args, stats)
-    return sim
-
-
-def _write_ensemble(args, sim):
-    if args.ensemble_csv:
-        sim.cluster_ensemble.to_csv(args.ensemble_csv, [dc.name for dc in sim.dcs.values()])
-    if args.job_ensemble_csv:
-        sim.job_ensemble.to_csv(args.job_ensemble_csv, [dc.name for dc in sim.dcs.values()])
-    if args.power_profile_csv:
-        sim.power_profile.to_csv(args.power_profile_csv, [dc.name for dc in sim.dcs.values()])
-    if args.job_waits_csv:
-        sim.job_waits.to_csv(args.job_waits_csv, [dc.name for dc in sim.dcs.values()])
-    if args.occupancy_csv:
-        sim.occupancy.to_csv(args.occupancy_csv, [dc.name for dc in sim.dcs.values()])
-    if args.tail_latency_csv:
-        sim.tail_latency.to_csv(args.tail_latency_csv, [dc.name for dc in sim.dcs.values()])
-    if args.job_resources_csv:
-        sim.job_resources.to_csv(args.job_resources_csv, [dc.name for dc in sim.dcs.values()])
-    if args.energy_cost_csv:
-        sim.energy_cost.to_csv(args.energy_cost_csv, [dc.name for dc in sim.dcs.values()])
 
 
 def _add_power_profile(stats, res):
@@ -299,22 +308,9 @@ def _main_sharded(args, world, rank):
         else:
             dist.init_process_group(backend)
     first, count = sharding.shard(args.replicas, rank, world)
-    if args.ensemble_csv and count == 0:
-        raise SystemExit("--ensemble-csv needs at least one replica per rank")
-    if args.job_ensemble_csv and count == 0:
-        raise SystemExit("--job-ensemble-csv needs at least one replica per rank")
-    if args.power_profile_csv and count == 0:
-        raise SystemExit("--power-profile-csv needs at least one replica per rank")
-    if args.job_waits_csv and count == 0:
-        raise SystemExit("--job-waits-csv needs at least one replica per rank")
-    if args.occupancy_csv and count == 0:
-        raise SystemExit("--occupancy-csv needs at least one replica per rank")
-    if args.tail_latency_csv and count == 0:
-        raise SystemExit("--tail-latency-csv needs at least one replica per rank")
-    if args.job_resources_csv and count == 0:
-        raise SystemExit("--job-resources-csv needs at least one replica per rank")
-    if args.energy_cost_csv and count == 0:
-        raise SystemExit("--energy-cost-csv needs at least one replica per rank")
+    for dest in RECORDER_CSV.values():
+        if getattr(args, dest) and count == 0:
+            raise SystemExit(f"--{dest.replace('_', '-')} needs at least one replica per rank")
     sim = build_simulator(args, replicas=max(count, 1), first_replica_id=first, device=local, write_logs=(rank == 0))
     sim.run()                                                   # (the ensemble's all-reduces run inside, on every rank)
     if rank == 0:
@@ -348,12 +344,7 @@ def _main_sharded(args, world, rank):
                  "mean_latency_s_mean": stats["mean_latency_s_mean"], "mean_latency_s_ci95": ci(stats["mean_latency_s_var"]),
                  "mean_latency_s_p05_p50_p95": [float(q) for q in np.percentile(cols[1][keep], [5, 50, 95])]}
         _add_latency_quantiles(stats, hist.cpu().numpy().astype(np.uint64))
-        _add_power_profile(stats, sim.power_profile)
-        _add_job_waits(stats, sim.job_waits)
-        _add_occupancy(stats, sim.occupancy, sim)
-        _add_tail_latency(stats, sim.tail_latency)
-        _add_job_resources(stats, sim.job_resources, sim)
-        _add_energy_cost(stats, sim.energy_cost, sim)
+        _add_recorders(stats, sim)
         _report(args, stats)
     dist.barrier()
     dist.destroy_process_group()
@@ -371,24 +362,9 @@ def _main_compare(args, world, rank):
     unknown = [a for a in algos if a not in ALGOS]
     if unknown:
         raise SystemExit(f"--compare-algos: unknown algo(s) {unknown}; choose from {ALGOS}")
-    if args.power_profile_csv or args.power_threshold is not None:
-        raise SystemExit("--power-profile-csv / --power-threshold are not available with --compare-algos (run each algo "
-                         "on its own)")
-    if args.occupancy_csv:
-        raise SystemExit("--occupancy-csv is not available with --compare-algos (run each algo on its own for its "
-                         "occupancy)")
-    if args.tail_latency_csv:
-        raise SystemExit("--tail-latency-csv is not available with --compare-algos (run each algo on its own for its "
-                         "per-run tail latency)")
-    if args.job_resources_csv:
-        raise SystemExit("--job-resources-csv is not available with --compare-algos (run each algo on its own for its "
-                         "GPU, frequency and energy-per-job statistics)")
-    if args.energy_cost_csv:
-        raise SystemExit("--energy-cost-csv is not available with --compare-algos (run each algo on its own for its "
-                         "electricity cost and carbon)")
-    if args.ensemble_csv or args.job_ensemble_csv or args.job_waits_csv:
-        raise SystemExit("--ensemble-csv / --job-ensemble-csv / --job-waits-csv are not available with --compare-algos "
-                         "(run each algo on its own for its cluster-log and job-log ensembles and its waiting times)")
+    for name, why in _COMPARE_REFUSALS.items():
+        if getattr(args, RECORDER_CSV[name]) or name == "power_profile" and args.power_threshold is not None:
+            raise SystemExit(why)
     dist = None
     first, count, device = 0, args.replicas, args.device
     if world > 1:

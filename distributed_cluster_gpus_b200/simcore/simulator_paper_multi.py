@@ -17,7 +17,7 @@ from typing import Dict, Optional, Tuple, Union
 import numpy as np
 
 from .. import spec as S
-from ..engine import RNG_KINDS, LoggedReplica, RecorderOverflow, release_engine, run_to_completion
+from ..engine import RECORDERS, RNG_KINDS, LoggedReplica, RecorderOverflow, release_engine, run_to_completion
 from .arrivals import ArrivalConfig
 from .models import DataCenter
 from .network import Graph, Ingress
@@ -96,44 +96,33 @@ class MultiIngressPaperSimulator:
         self.summary: Optional[np.ndarray] = None
         self.latency_histogram: Optional[np.ndarray] = None
         self.launch_info: Optional[dict] = None
-        # cluster_ensemble=True: after run(), per-tick statistics of every DC's cluster-log columns over all replicas (of
-        # all ranks when torch.distributed runs: every rank's run() takes part in the all-reduces), ensemble.EnsembleResult
-        self._want_ensemble = bool(cluster_ensemble)
-        self.cluster_ensemble = None
-        # job_ensemble=True: after run(), per finish window of job_ensemble_bin seconds (None: log_interval) and for the
-        # whole run, statistics of every DC's job counts and mean latencies over all replicas (all ranks, as above),
-        # ensemble.JobEnsembleResult
-        self._want_job_ensemble, self._job_ensemble_bin = bool(job_ensemble), job_ensemble_bin
-        self.job_ensemble = None
-        # power_profile=True: after run(), batch statistics of every replica's cluster power step function — peak, time
-        # and energy over power_threshold watts (None: no threshold), per-DC peaks and the pooled power-duration curve
-        # (all ranks, as above), ensemble.PowerProfileResult
-        self._want_power_profile, self._power_threshold = bool(power_profile), power_threshold
-        self.power_profile = None
-        # job_waits=True: after run(), per finish window of job_ensemble_bin seconds and for the whole run, statistics of
-        # every job's wait (start - xfer_done) and response time (finish - arrival) over all replicas (all ranks, as
-        # above), ensemble.JobWaitsResult.  It runs the job ensemble's recorder too (its windows and job counts)
-        self._want_job_waits = bool(job_waits)
-        self.job_waits = None
-        # occupancy=True: after run(), statistics of every DC's time-weighted queue lengths, running jobs and busy GPUs
-        # between events over all replicas (all ranks, as above), ensemble.OccupancyResult
-        self._want_occupancy = bool(occupancy)
-        self.occupancy = None
-        # tail_latency=True: after run(), statistics over all replicas (all ranks, as above) of every run's own exact
-        # p50 / p95 / p99 / p99.9 / max of service, wait and response time per job type and DC, and the share of runs
-        # whose p99 met sla_p99_ms, ensemble.TailLatencyResult
-        self._want_tail_latency = bool(tail_latency)
-        self.tail_latency = None
-        # energy_cost=True: after run(), statistics over all replicas (all ranks, as above) of every DC's energy by hour
-        # of day, its cost under the DC's hourly tariff and its carbon, ensemble.EnergyCostResult
-        self._want_energy_cost = bool(energy_cost)
-        self.energy_cost = None
-        # job_resources=True: after run(), per finish window of job_ensemble_bin seconds and for the whole run, statistics
-        # of every finished job's GPU count, frequency and predicted energy E_pred * size over all replicas (all ranks, as
-        # above), the pooled (n, f) mix and energy-per-job quantiles, ensemble.JobResourcesResult.  It runs the job
-        # ensemble's recorder too (its windows and job counts)
-        self._want_job_resources = bool(job_resources)
-        self.job_resources = None
+        # The batch recorders (engine.RECORDERS), each off unless asked for.  After run(), the attribute of the same name
+        # holds its statistics over all replicas (of all ranks when torch.distributed runs: every rank's run() takes part
+        # in the all-reduces), None when it is off:
+        #   cluster_ensemble  per-tick statistics of every DC's cluster-log columns, ensemble.EnsembleResult
+        #   job_ensemble      per finish window of job_ensemble_bin seconds (None: log_interval) and for the whole run,
+        #                     every DC's job counts and mean latencies, ensemble.JobEnsembleResult
+        #   power_profile     the cluster power step function: peak, time and energy over power_threshold watts (None: no
+        #                     threshold), per-DC peaks and the pooled power-duration curve, ensemble.PowerProfileResult
+        #   job_waits         per finish window and for the whole run, every job's wait (start - xfer_done) and response
+        #                     time (finish - arrival), ensemble.JobWaitsResult
+        #   occupancy         every DC's time-weighted queue lengths, running jobs and busy GPUs between events,
+        #                     ensemble.OccupancyResult
+        #   tail_latency      every run's own exact p50 / p95 / p99 / p99.9 / max of service, wait and response time per
+        #                     job type and DC, and the share of runs whose p99 met sla_p99_ms, ensemble.TailLatencyResult
+        #   job_resources     per finish window and for the whole run, every finished job's GPU count, frequency and
+        #                     predicted energy E_pred * size, the pooled (n, f) mix and energy-per-job quantiles,
+        #                     ensemble.JobResourcesResult
+        #   energy_cost       every DC's energy by hour of day, its cost under the DC's hourly tariff and its carbon,
+        #                     ensemble.EnergyCostResult
+        # job_waits and job_resources run the job ensemble's recorder too (its windows and job counts).
+        self._recorders = dict(cluster_ensemble=bool(cluster_ensemble), job_ensemble=bool(job_ensemble),
+                               job_ensemble_bin=job_ensemble_bin, power_profile=bool(power_profile),
+                               power_threshold=power_threshold, job_waits=bool(job_waits), occupancy=bool(occupancy),
+                               tail_latency=bool(tail_latency), job_resources=bool(job_resources),
+                               energy_cost=bool(energy_cost))
+        for name in RECORDERS:
+            setattr(self, name, None)
         self._spec = self._flatten({})              # validates now, like the reference's constructor would fail now
 
     # ------------------------------------------------------------------------------------------------
@@ -184,12 +173,7 @@ class MultiIngressPaperSimulator:
         try:
             eng, summ = run_to_completion(self._flatten, self.replicas, self.rng_seed, self.first_replica_id, self.device,
                                           self.cuda_stream, configure=configure, while_running=while_running,
-                                          cluster_ensemble=self._want_ensemble, job_ensemble=self._want_job_ensemble,
-                                          job_ensemble_bin=self._job_ensemble_bin, power_profile=self._want_power_profile,
-                                          power_threshold=self._power_threshold, job_waits=self._want_job_waits,
-                                          occupancy=self._want_occupancy, tail_latency=self._want_tail_latency,
-                                          job_resources=self._want_job_resources, energy_cost=self._want_energy_cost,
-                                          tail_sla_s=float(self.sla_p99_ms) / 1000.0)
+                                          tail_sla_s=float(self.sla_p99_ms) / 1000.0, **self._recorders)
         except BaseException:
             if companion is not None:
                 companion.release(keep=False)
@@ -198,30 +182,11 @@ class MultiIngressPaperSimulator:
             self.summary = summ
             self.latency_histogram = eng.latency_histogram()     # [2, 128] job-latency counts of the whole batch
             self.launch_info = eng.launch_info()
-            if self._want_ensemble:
-                from ..ensemble import cluster_ensemble
-                self.cluster_ensemble = cluster_ensemble(eng)
-            if self._want_job_ensemble:
-                from ..ensemble import job_ensemble
-                self.job_ensemble = job_ensemble(eng)
-            if self._want_power_profile:
-                from ..ensemble import power_profile
-                self.power_profile = power_profile(eng, summary=summ)
-            if self._want_job_waits:
-                from ..ensemble import job_waits
-                self.job_waits = job_waits(eng)
-            if self._want_occupancy:
-                from ..ensemble import occupancy
-                self.occupancy = occupancy(eng)
-            if self._want_tail_latency:
-                from ..ensemble import tail_latency
-                self.tail_latency = tail_latency(eng)
-            if self._want_job_resources:
-                from ..ensemble import job_resources
-                self.job_resources = job_resources(eng)
-            if self._want_energy_cost:
-                from ..ensemble import energy_cost
-                self.energy_cost = energy_cost(eng)
+            from .. import ensemble
+            for name in RECORDERS:
+                if self._recorders[name]:
+                    compute = getattr(ensemble, name)
+                    setattr(self, name, compute(eng, summary=summ) if name == "power_profile" else compute(eng))
             self._store_replica0(summ[0])
             if in_batch_log:
                 try:

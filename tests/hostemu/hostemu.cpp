@@ -57,6 +57,7 @@ struct hostemu_out_t {
   double* tail;                      /* [n][cap_arr][2], set to NaN here */
   double* tail_cols;                 /* [DCSIM_TAIL_COLS(n_dc)][n] (with tail) */
   double tail_sla;
+  double* cost;                      /* [DCSIM_COST_COLS(n_dc)][n] */
   /* what the pre-pass and the merge leave: arr_* [n][cap_arr], ml_* [n][2 * cap_arr], arr_hdr [n]; entries they did not
    * write hold 0xee bytes */
   double* arr_t;
@@ -105,6 +106,10 @@ uint64_t hostemu_jens_windows(const void* spec_blob, double bin_s) {
 double hostemu_pp_range(const void* spec_blob) { return dcsim_pp_range((const dcsim_spec_t*)spec_blob); }
 /* the GPU-count rows of the job-resources mix (the last one takes g >= G) */
 uint32_t hostemu_jres_g(const void* spec_blob) { return (uint32_t)DCSIM_JRES_G(((const dcsim_spec_t*)spec_blob)->max_gpus_per_job); }
+/* the energy-cost recorder's hour window of an instant (dcsim_cost_window), and the hour the handlers use
+ * (dcsim_current_hour) */
+double hostemu_energy_cost_window(double t) { return dcsim_cost_window(t); }
+int hostemu_current_hour(double t) { return dcsim_current_hour(t); }
 
 /* dcsim_arrival_inputs_equal: 1 equal, 0 not (the first differing field's name into `field`, `field_bytes` long), -1 on
  * a malformed blob. */
@@ -153,6 +158,10 @@ long long hostemu_run_batch(const void* spec_lists, const void* spec_run, size_t
     P->occ_work = (double*)calloc(n_replicas * (size_t)P->spec.n_dc * DCSIM_OCCW_N, sizeof(double));
   }
   P->tail = o->tail; P->tail_cols = o->tail_cols; P->tail_sla = o->tail_sla;
+  if (o->cost) {
+    P->cost = o->cost;
+    P->cost_work = (double*)calloc(n_replicas * (size_t)P->spec.n_dc * DCSIM_COSTW_N, sizeof(double));
+  }
   dcsim_derive_kparams(P);
 
   /* the pre-pass and the merge: the owner's spec and the layout it implies (dcsim_prepare) */
@@ -240,7 +249,7 @@ long long hostemu_run_batch(const void* spec_lists, const void* spec_run, size_t
   if (o->arr_hdr) memcpy(o->arr_hdr, P->arr_hdr, n_replicas * sizeof(dcsim_arrhdr_t));
   free(P->arr_t); free(P->arr_raw); free(P->arr_meta); free(P->arr_pred); free(P->arr_tx); free(P->arr_fin);
   free(P->ml_t); free(P->ml_aux); free(P->ml_meta); free(P->arr_hdr); free(P->mt_state);
-  free(P->pp_work); free(P->occ_work); free(P);
+  free(P->pp_work); free(P->occ_work); free(P->cost_work); free(P);
   return total;
 }
 

@@ -28,7 +28,7 @@ class Out(C.Structure):
                 ("counts", _vp), ("layout", _vp), ("lat_hist", _vp), ("ens", _vp),
                 ("jens", _vp), ("jens_hist", _vp), ("jens_bin", _f64), ("jwait", _vp), ("jwait_hist", _vp),
                 ("jres", _vp), ("jres_mix", _vp), ("jres_hist", _vp), ("pp", _vp), ("pp_threshold", _f64),
-                ("occ", _vp), ("tail", _vp), ("tail_cols", _vp), ("tail_sla", _f64),
+                ("occ", _vp), ("tail", _vp), ("tail_cols", _vp), ("tail_sla", _f64), ("cost", _vp),
                 ("arr_t", _vp), ("arr_raw", _vp), ("arr_meta", _vp), ("arr_pred", _vp), ("arr_tx", _vp),
                 ("ml_t", _vp), ("ml_aux", _vp), ("ml_meta", _vp), ("arr_hdr", _vp), ("lists_only", C.c_int32)]
 
@@ -48,6 +48,10 @@ def _bind(path):
         getattr(L, name).argtypes = [_vp]
     L.hostemu_jens_windows.restype = C.c_uint64
     L.hostemu_jens_windows.argtypes = [_vp, _f64]
+    L.hostemu_energy_cost_window.restype = _f64
+    L.hostemu_energy_cost_window.argtypes = [_f64]
+    L.hostemu_current_hour.restype = C.c_int
+    L.hostemu_current_hour.argtypes = [_f64]
     L.hostemu_compatible.restype = C.c_int
     L.hostemu_compatible.argtypes = [_vp, C.c_size_t, _vp, C.c_size_t, C.c_char_p, C.c_size_t]
     L.hostemu_run_batch.restype = C.c_longlong
@@ -108,6 +112,16 @@ def jres_g(spec_bytes):
     return int(lib().hostemu_jres_g(spec_bytes))
 
 
+def cost_window(t):
+    """The energy-cost recorder's hour window k of instant t: 3600 k <= t < 3600 (k + 1) (dcsim_cost_window)."""
+    return float(lib().hostemu_energy_cost_window(float(t)))
+
+
+def current_hour(t):
+    """The hour of day the handlers use at instant t (dcsim_current_hour, SIM:982-984)."""
+    return int(lib().hostemu_current_hour(float(t)))
+
+
 def occ_rows(n_dc):
     return 1 + S.OCC_FIELDS * n_dc + 2 * S.OCC_BINS * n_dc
 
@@ -124,7 +138,8 @@ def compatible(spec_a: bytes, spec_b: bytes):
 def run_batch(spec_bytes, n_replicas, seed0, chunk_events=0, trace_cap=0, rec_replica=-1, job_dtype=None,
               jobs_cap=0, cluster_dtype=None, cluster_cap=0, rng_kind=0, perturbed=False, smallring=False, uniform=False,
               variant=None, run_spec=None, lat_hist=True, ens_cap=0, jens_bin=None, jwait=False, jres=False, pp=False,
-              pp_threshold=float("inf"), occ=False, tail=False, tail_sla=None, prepass=False, lists_only=False):
+              pp_threshold=float("inf"), occ=False, tail=False, tail_sla=None, cost=False, prepass=False,
+              lists_only=False):
     """n replicas from keys seed0, seed0 + 1, ...: the pre-pass and the merge under `spec_bytes`, then the event loop of
     `run_spec` (default: the same spec; else a spec whose arrival inputs equal it) on those lists, in launches of
     `chunk_events` events (0: to the end).  The batch latency histogram is on unless lat_hist=False ("lat_hist"
@@ -138,6 +153,7 @@ def run_batch(spec_bytes, n_replicas, seed0, chunk_events=0, trace_cap=0, rec_re
       pp=True         "pp" [PP_FIELDS + n_dc + PP_BINS, n] over `pp_threshold`
       occ=True        "occ" [occ_rows(n_dc), n]
       tail=True       "tail" [n, cap_arr, 2], "tail_cols" [tail_cols(n_dc), n] under `tail_sla` (None: none)
+      cost=True       "cost" [cost_cols(n_dc), n]
 
     plus trace / jobs / cluster of `rec_replica`.  prepass=True adds what the pre-pass and the merge left ("arr_t",
     "arr_raw" (the job sizes), "arr_meta", "arr_pred", "arr_tx": [n, cap_arr]; "ml_t", "ml_aux", "ml_meta":
@@ -185,6 +201,8 @@ def run_batch(spec_bytes, n_replicas, seed0, chunk_events=0, trace_cap=0, rec_re
     if tail:
         out("tail", (n_replicas, cap, 2))
         out("tail_cols", (S.tail_cols(n_dc), n_replicas))
+    if cost:
+        out("cost", (S.cost_cols(n_dc), n_replicas))
     if prepass or lists_only:
         for name in ("arr_t", "arr_raw", "arr_tx"):
             out(name, (n_replicas, cap))

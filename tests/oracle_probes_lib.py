@@ -1,5 +1,5 @@
 """TEST-ONLY ctypes access to the probes of the stepped C oracle (tests/oracle_jobs/oracle_probes.c): per-job instants,
-the per-arrival record, the occupancy checkers, every created job and the power profile."""
+the per-arrival record, the occupancy checkers, every created job, the power profile and the energy cost."""
 import ctypes as C
 import os
 import subprocess
@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 _DIR = os.path.join(_HERE, "oracle_jobs")
 _SO = os.path.join(_DIR, "_build", "liboracle_probes.so")
 _SRCS = tuple(os.path.join(_DIR, f) for f in ("oracle_probes.c", "oracle_jobs.c", "oracle_lists.c", "oracle_occ.c",
-                                              "oracle_tail.c", "oracle_power.c", "build.sh")) + (
+                                              "oracle_tail.c", "oracle_power.c", "oracle_cost.c", "build.sh")) + (
     os.path.join(_HERE, "..", "oracle", "dcsim_oracle.c"), os.path.join(_HERE, "..", "include", "dcsim_b200.h"))
 JOB_ROW_DTYPE = np.dtype([("jid", "<u4"), ("dc", "<i4"), ("jtype", "<i4"), ("at_xfer", "<i4"), ("arrival", "<f8"),
                           ("xfer_done", "<f8"), ("start", "<f8"), ("finish", "<f8")])
@@ -35,7 +35,7 @@ def lib():
         L.dcoracle_set_test_time_quantum.argtypes = [C.c_double]
         for name, extra in (("oraclejobs_run", [C.c_uint32]), ("oraclelists_run", [C.c_uint32, vp]),
                             ("oracleocc_occupancy", []), ("oracleocc_reached", [C.c_uint32]),
-                            ("oracletail_run", [C.c_uint32])):
+                            ("oracletail_run", [C.c_uint32]), ("oraclecost_run", [])):
             getattr(L, name).restype = C.c_longlong
             getattr(L, name).argtypes = [vp, C.c_size_t, u64, C.c_int, vp] + extra
         L.oraclepower_profile.restype = C.c_longlong
@@ -100,6 +100,15 @@ def oracle_power_profile(spec_bytes, seed, threshold, rng_kind=0, hi=None):
     if n == -2:
         raise AssertionError("the oracle's DCs accrued energy at different instants")
     if n < 0:
+        raise ValueError("the oracle rejected the spec blob")
+    return row
+
+
+def oracle_energy_cost(spec_bytes, seed, rng_kind=0):
+    """One replica's energy-cost column [cost_cols(n_dc)] from the oracle stepped one event at a time."""
+    n_dc = S.Spec.from_buffer_copy(spec_bytes).n_dc
+    row = np.zeros(S.cost_cols(n_dc))
+    if lib().oraclecost_run(spec_bytes, len(spec_bytes), seed & (2**64 - 1), rng_kind, row.ctypes.data) < 0:
         raise ValueError("the oracle rejected the spec blob")
     return row
 

@@ -12,8 +12,8 @@ import sys
 import numpy as np
 import pytest
 
-import hostemu_cost_lib as H
-import oracle_cost_lib as OP
+import hostemu_lib as H
+import oracle_probes_lib as OP
 from conftest import GOLDEN_DIR, ROOT
 from distributed_cluster_gpus_b200 import ensemble as E
 from distributed_cluster_gpus_b200 import scenarios as SC

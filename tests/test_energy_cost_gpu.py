@@ -9,7 +9,7 @@ import json
 import numpy as np
 import pytest
 
-import hostemu_cost_lib as H
+import hostemu_lib as H
 import test_recorder_corpus as RC
 from conftest import has_cuda
 from distributed_cluster_gpus_b200 import ensemble as E, scenarios as SC, spec as S
