@@ -21,21 +21,16 @@ EXPORTS = (
     "dcsim_summary_device_ptr", "dcsim_reduce_summary", "dcsim_enable_latency_histogram", "dcsim_fetch_latency_histogram", "dcsim_fetch_trace", "dcsim_fetch_job_log",
     "dcsim_fetch_cluster_log", "dcsim_launch_info", "dcsim_last_error", "dcsim_destroy", "dcsim_set_rng",
     "dcsim_recorder_counts", "dcsim_allreduce_summary", "dcsim_fetch_summary_host",
+    "dcsim_stat_columns", "dcsim_stat_moments", "dcsim_stat_spread",
     "dcsim_enable_cluster_ensemble", "dcsim_cluster_ensemble_capacity", "dcsim_fetch_cluster_ensemble",
-    "dcsim_ensemble_moments", "dcsim_ensemble_spread",
-    "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_job_ensemble_moments",
-    "dcsim_job_ensemble_spread", "dcsim_fetch_dc_latency_histogram",
+    "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_fetch_dc_latency_histogram",
     "dcsim_arrivals_compatible", "dcsim_create_shared", "dcsim_paired_moments", "dcsim_paired_spread",
-    "dcsim_enable_power_profile", "dcsim_power_profile_range", "dcsim_fetch_power_profile", "dcsim_power_profile_moments",
-    "dcsim_power_profile_spread",
-    "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_job_waits_moments", "dcsim_job_waits_spread",
-    "dcsim_fetch_dc_wait_histogram",
-    "dcsim_enable_job_resources", "dcsim_fetch_job_resources", "dcsim_job_resources_moments", "dcsim_job_resources_spread",
-    "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy", "dcsim_occupancy_moments",
-    "dcsim_occupancy_spread",
-    "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs", "dcsim_tail_latency_moments",
-    "dcsim_tail_latency_spread",
-    "dcsim_enable_energy_cost", "dcsim_fetch_energy_cost", "dcsim_energy_cost_moments", "dcsim_energy_cost_spread",
+    "dcsim_enable_power_profile", "dcsim_power_profile_range", "dcsim_fetch_power_profile",
+    "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_fetch_dc_wait_histogram",
+    "dcsim_enable_job_resources", "dcsim_fetch_job_resources",
+    "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy",
+    "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs",
+    "dcsim_enable_energy_cost", "dcsim_fetch_energy_cost",
 )
 
 _lib = None
@@ -105,6 +100,13 @@ def load():
     if hasattr(L, "dcsim_recorder_counts"):
         L.dcsim_recorder_counts.restype = i32
         L.dcsim_recorder_counts.argtypes = [vp, C.POINTER(u32 * 3)]
+    if hasattr(L, "dcsim_stat_columns"):
+        L.dcsim_stat_columns.restype = i32
+        L.dcsim_stat_columns.argtypes = [vp, i32, C.POINTER(u64), C.POINTER(u64)]
+        L.dcsim_stat_moments.restype = i32
+        L.dcsim_stat_moments.argtypes = [vp, i32, vp]
+        L.dcsim_stat_spread.restype = i32
+        L.dcsim_stat_spread.argtypes = [vp, i32, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_cluster_ensemble"):
         L.dcsim_enable_cluster_ensemble.restype = i32
         L.dcsim_enable_cluster_ensemble.argtypes = [vp, u32]
@@ -112,10 +114,6 @@ def load():
         L.dcsim_cluster_ensemble_capacity.argtypes = [vp, C.POINTER(u32)]
         L.dcsim_fetch_cluster_ensemble.restype = i32
         L.dcsim_fetch_cluster_ensemble.argtypes = [vp, vp, C.c_size_t]
-        L.dcsim_ensemble_moments.restype = i32
-        L.dcsim_ensemble_moments.argtypes = [vp, vp]
-        L.dcsim_ensemble_spread.restype = i32
-        L.dcsim_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_job_ensemble"):
         L.dcsim_enable_job_ensemble.restype = i32
         L.dcsim_enable_job_ensemble.argtypes = [vp, C.c_double]
@@ -123,10 +121,6 @@ def load():
         L.dcsim_job_ensemble_windows.argtypes = [vp, C.POINTER(u32)]
         L.dcsim_fetch_job_ensemble.restype = i32
         L.dcsim_fetch_job_ensemble.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
-        L.dcsim_job_ensemble_moments.restype = i32
-        L.dcsim_job_ensemble_moments.argtypes = [vp, vp]
-        L.dcsim_job_ensemble_spread.restype = i32
-        L.dcsim_job_ensemble_spread.argtypes = [vp, vp, vp, vp, vp, vp]
         L.dcsim_fetch_dc_latency_histogram.restype = i32
         L.dcsim_fetch_dc_latency_histogram.argtypes = [vp, vp, C.c_size_t]
     if hasattr(L, "dcsim_create_shared"):
@@ -143,10 +137,6 @@ def load():
         L.dcsim_enable_job_waits.argtypes = [vp]
         L.dcsim_fetch_job_waits.restype = i32
         L.dcsim_fetch_job_waits.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
-        L.dcsim_job_waits_moments.restype = i32
-        L.dcsim_job_waits_moments.argtypes = [vp, vp]
-        L.dcsim_job_waits_spread.restype = i32
-        L.dcsim_job_waits_spread.argtypes = [vp, vp, vp, vp, vp, vp]
         L.dcsim_fetch_dc_wait_histogram.restype = i32
         L.dcsim_fetch_dc_wait_histogram.argtypes = [vp, vp, C.c_size_t]
     if hasattr(L, "dcsim_enable_job_resources"):
@@ -154,10 +144,6 @@ def load():
         L.dcsim_enable_job_resources.argtypes = [vp]
         L.dcsim_fetch_job_resources.restype = i32
         L.dcsim_fetch_job_resources.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t]
-        L.dcsim_job_resources_moments.restype = i32
-        L.dcsim_job_resources_moments.argtypes = [vp, vp]
-        L.dcsim_job_resources_spread.restype = i32
-        L.dcsim_job_resources_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_occupancy"):
         L.dcsim_enable_occupancy.restype = i32
         L.dcsim_enable_occupancy.argtypes = [vp]
@@ -165,10 +151,6 @@ def load():
         L.dcsim_occupancy_bin_widths.argtypes = [vp, vp]
         L.dcsim_fetch_occupancy.restype = i32
         L.dcsim_fetch_occupancy.argtypes = [vp, vp, C.c_size_t]
-        L.dcsim_occupancy_moments.restype = i32
-        L.dcsim_occupancy_moments.argtypes = [vp, vp]
-        L.dcsim_occupancy_spread.restype = i32
-        L.dcsim_occupancy_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_tail_latency"):
         L.dcsim_enable_tail_latency.restype = i32
         L.dcsim_enable_tail_latency.argtypes = [vp, C.c_double]
@@ -176,10 +158,6 @@ def load():
         L.dcsim_fetch_tail_latency.argtypes = [vp, vp, C.c_size_t]
         L.dcsim_fetch_tail_jobs.restype = i32
         L.dcsim_fetch_tail_jobs.argtypes = [vp, u64, u64, vp, C.c_size_t]
-        L.dcsim_tail_latency_moments.restype = i32
-        L.dcsim_tail_latency_moments.argtypes = [vp, vp]
-        L.dcsim_tail_latency_spread.restype = i32
-        L.dcsim_tail_latency_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_power_profile"):
         L.dcsim_enable_power_profile.restype = i32
         L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]
@@ -187,19 +165,11 @@ def load():
         L.dcsim_power_profile_range.argtypes = [vp, C.POINTER(C.c_double)]
         L.dcsim_fetch_power_profile.restype = i32
         L.dcsim_fetch_power_profile.argtypes = [vp, vp, C.c_size_t]
-        L.dcsim_power_profile_moments.restype = i32
-        L.dcsim_power_profile_moments.argtypes = [vp, vp]
-        L.dcsim_power_profile_spread.restype = i32
-        L.dcsim_power_profile_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     if hasattr(L, "dcsim_enable_energy_cost"):
         L.dcsim_enable_energy_cost.restype = i32
         L.dcsim_enable_energy_cost.argtypes = [vp]
         L.dcsim_fetch_energy_cost.restype = i32
         L.dcsim_fetch_energy_cost.argtypes = [vp, vp, C.c_size_t]
-        L.dcsim_energy_cost_moments.restype = i32
-        L.dcsim_energy_cost_moments.argtypes = [vp, vp]
-        L.dcsim_energy_cost_spread.restype = i32
-        L.dcsim_energy_cost_spread.argtypes = [vp, vp, vp, vp, vp, vp]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

@@ -1473,25 +1473,6 @@ int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
-int dcsim_ensemble_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = ens_counts(h);
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  return ens_moments(h, src, h->n_replicas, (uint64_t)h->ens_cap * cols_per_tick, dev_out);
-}
-
-int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
-                          uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = ens_counts(h);
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_cluster_src src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, h->spec.n_dc};
-  return ens_spread(h, src, h->n_replicas, (uint64_t)h->ens_cap * cols_per_tick, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
-}
-
 static int pair_check(dcsim_t* base, const double* dev_variant_summary, uint64_t n) {
   if (!base || !dev_variant_summary) return DCSIM_E_INVALID;
   if (n != base->n_replicas)
@@ -1568,26 +1549,6 @@ int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32
   return DCSIM_OK;
 }
 
-int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_job_src src{h->d_jens, h->d_status, h->n_replicas, cells};
-  return ens_moments(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells, dev_out);
-}
-
-int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                              double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_job_src src{h->d_jens, h->d_status, h->n_replicas, cells};
-  return ens_spread(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JENS_FIELDS * cells, dev_mean, dev_lo, dev_hi,
-                    dev_m2_out, dev_hist_out);
-}
-
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   if (!h || !out) return DCSIM_E_INVALID;
   const uint32_t row_len = 2u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
@@ -1629,26 +1590,6 @@ int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t*
   if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jwait_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
-}
-
-int dcsim_job_waits_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_wait_src src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells};
-  return ens_moments(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JWAIT_FIELDS * cells, dev_out);
-}
-
-int dcsim_job_waits_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                           double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  const dcsim_ens_wait_src src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells};
-  return ens_spread(h, src, h->n_replicas, (h->jens_windows + 1) * DCSIM_JWAIT_FIELDS * cells, dev_mean, dev_lo, dev_hi,
-                    dev_m2_out, dev_hist_out);
 }
 
 int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
@@ -1698,29 +1639,6 @@ int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint3
   return DCSIM_OK;
 }
 
-static dcsim_ens_res_src jres_src(const dcsim_t* h) {
-  const uint32_t cells = 2u * (uint32_t)h->spec.n_dc;
-  return dcsim_ens_res_src{h->d_jres, h->d_jens, h->d_jres_cnt, h->d_status, h->n_replicas, cells,
-                           (h->jens_windows + 1) * DCSIM_JRES_FIELDS * cells};
-}
-
-int dcsim_job_resources_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_res_src src = jres_src(h);
-  return ens_moments(h, src, h->n_replicas, src.win_cols + jres_mix_cols(h) + jres_hist_cols(h), dev_out);
-}
-
-int dcsim_job_resources_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                               double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_res_src src = jres_src(h);
-  return ens_spread(h, src, h->n_replicas, src.win_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out); /* the counts need no spread */
-}
-
 int dcsim_enable_power_profile(dcsim_t* h, double threshold_w) {
   if (!h) return DCSIM_E_INVALID;
   if (!(threshold_w >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_power_profile: the threshold must be >= 0 (+inf: none)%s%lld");
@@ -1757,24 +1675,6 @@ int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
-int dcsim_power_profile_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_pp_src src{h->d_pp, h->d_status, h->n_replicas};
-  return ens_moments(h, src, h->n_replicas, pp_cols(h), dev_out);
-}
-
-int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                               double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_pp_src src{h->d_pp, h->d_status, h->n_replicas};
-  const uint64_t n_cols = (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc); /* the bins need no spread */
-  return ens_spread(h, src, h->n_replicas, n_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
-}
-
 int dcsim_enable_energy_cost(dcsim_t* h) {
   if (!h) return DCSIM_E_INVALID;
   if (h->member) return set_err(h, DCSIM_E_STATE, "enable_energy_cost on a member of a shared group%s%lld");
@@ -1801,23 +1701,6 @@ int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes) {
   CUDA_TRY(h, cudaMemcpyAsync(out, h->d_cost, cost_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
-}
-
-int dcsim_energy_cost_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_cost_src src{h->d_cost, h->d_status, h->n_replicas};
-  return ens_moments(h, src, h->n_replicas, cost_cols(h), dev_out);
-}
-
-int dcsim_energy_cost_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                             double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_cost_src src{h->d_cost, h->d_status, h->n_replicas};
-  return ens_spread(h, src, h->n_replicas, cost_cols(h), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
 int dcsim_enable_tail_latency(dcsim_t* h, double sla_s) {
@@ -1881,27 +1764,6 @@ int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* ou
   return DCSIM_OK;
 }
 
-int dcsim_tail_latency_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  int rc = tail_ready(h);
-  if (rc == DCSIM_OK) rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t group_cols = 2u * (uint32_t)(h->spec.n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
-  const dcsim_ens_tail_src src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols};
-  return ens_moments(h, src, h->n_replicas, DCSIM_TAIL_COLS(h->spec.n_dc), dev_out);
-}
-
-int dcsim_tail_latency_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                              double* dev_m2_out, uint64_t* dev_hist_out) {
-  if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  int rc = tail_ready(h);
-  if (rc == DCSIM_OK) rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
-  if (rc != DCSIM_OK) return rc;
-  const uint32_t group_cols = 2u * (uint32_t)(h->spec.n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
-  const dcsim_ens_tail_src src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols};
-  return ens_spread(h, src, h->n_replicas, DCSIM_TAIL_COLS(h->spec.n_dc), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
-}
-
 int dcsim_enable_occupancy(dcsim_t* h) {
   if (!h) return DCSIM_E_INVALID;
   if (h->member) return set_err(h, DCSIM_E_STATE, "enable_occupancy on a member of a shared group%s%lld");
@@ -1936,21 +1798,85 @@ int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
-int dcsim_occupancy_moments(dcsim_t* h, double* dev_out) {
-  if (!h || !dev_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_occ_src src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)h->spec.n_dc};
-  return ens_moments(h, src, h->n_replicas, occ_cols(h), dev_out);
+extern "C++" {
+/* The batch recorder `stat` (DCSIM_STAT_*) as the two passes see it: f(src, columns, spread_columns) with its column
+ * source and column counts for the handle's current state.  With `ready`, the recorder's precondition runs first: it
+ * fails when the recorder is off or the batch has not advanced, and queues what the source reads (the tick counts, the
+ * status words, the tail selection) on the stream ahead of the pass.  Without it this is host arithmetic only. */
+template <class F>
+static int with_stat(dcsim_t* h, int stat, bool ready, F&& f) {
+  const int n_dc = h->spec.n_dc;
+  const uint32_t cells = 2u * (uint32_t)n_dc;
+  const uint64_t rows = (h->d_jens ? h->jens_windows : 0) + 1; /* the job ensemble's windows, then the whole run */
+  int rc = DCSIM_OK;
+  switch (stat) {
+    case DCSIM_STAT_CLUSTER_ENSEMBLE: {
+      if (ready && (rc = ens_counts(h)) != DCSIM_OK) return rc;
+      const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)n_dc;
+      const uint64_t cols = (uint64_t)(h->d_ens ? h->ens_cap : 0u) * cols_per_tick;
+      return f(dcsim_ens_cluster_src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, n_dc}, cols, cols);
+    }
+    case DCSIM_STAT_JOB_ENSEMBLE: {
+      if (ready && (rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble")) != DCSIM_OK) return rc;
+      const uint64_t cols = rows * DCSIM_JENS_FIELDS * cells;
+      return f(dcsim_ens_job_src{h->d_jens, h->d_status, h->n_replicas, cells}, cols, cols);
+    }
+    case DCSIM_STAT_POWER_PROFILE:
+      if (ready && (rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile")) != DCSIM_OK) return rc;
+      return f(dcsim_ens_pp_src{h->d_pp, h->d_status, h->n_replicas}, pp_cols(h), (uint64_t)(DCSIM_PP_FIELDS + n_dc));
+    case DCSIM_STAT_JOB_WAITS: {
+      if (ready && (rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits")) != DCSIM_OK) return rc;
+      const uint64_t cols = rows * DCSIM_JWAIT_FIELDS * cells;
+      return f(dcsim_ens_wait_src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells}, cols, cols);
+    }
+    case DCSIM_STAT_OCCUPANCY:
+      if (ready && (rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy")) != DCSIM_OK) return rc;
+      return f(dcsim_ens_occ_src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)n_dc},
+               occ_cols(h), occ_stat_cols(h));
+    case DCSIM_STAT_TAIL_LATENCY: {
+      if (ready && ((rc = tail_ready(h)) != DCSIM_OK ||
+                    (rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency")) != DCSIM_OK)) return rc;
+      const uint32_t group_cols = 2u * (uint32_t)(n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
+      const uint64_t cols = DCSIM_TAIL_COLS(n_dc);
+      return f(dcsim_ens_tail_src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols}, cols, cols);
+    }
+    case DCSIM_STAT_JOB_RESOURCES: {
+      if (ready && (rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources")) != DCSIM_OK) return rc;
+      const uint64_t win_cols = rows * DCSIM_JRES_FIELDS * cells; /* the counts after them need no spread */
+      return f(dcsim_ens_res_src{h->d_jres, h->d_jens, h->d_jres_cnt, h->d_status, h->n_replicas, cells, win_cols},
+               win_cols + jres_mix_cols(h) + jres_hist_cols(h), win_cols);
+    }
+    case DCSIM_STAT_ENERGY_COST:
+      if (ready && (rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost")) != DCSIM_OK) return rc;
+      return f(dcsim_ens_cost_src{h->d_cost, h->d_status, h->n_replicas}, cost_cols(h), cost_cols(h));
+    default:
+      return set_err(h, DCSIM_E_INVALID, "unknown statistic %s%lld (DCSIM_STAT_*)", "", (long long)stat);
+  }
+}
+} /* extern "C++" */
+
+int dcsim_stat_columns(dcsim_t* h, int stat, uint64_t* columns_out, uint64_t* spread_columns_out) {
+  if (!h || !columns_out || !spread_columns_out) return DCSIM_E_INVALID;
+  return with_stat(h, stat, false, [&](const auto&, uint64_t cols, uint64_t spread_cols) {
+    *columns_out = cols;
+    *spread_columns_out = spread_cols;
+    return DCSIM_OK;
+  });
 }
 
-int dcsim_occupancy_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                           double* dev_m2_out, uint64_t* dev_hist_out) {
+int dcsim_stat_moments(dcsim_t* h, int stat, double* dev_out) {
+  if (!h || !dev_out) return DCSIM_E_INVALID;
+  return with_stat(h, stat, true, [&](const auto& src, uint64_t cols, uint64_t) {
+    return ens_moments(h, src, h->n_replicas, cols, dev_out);
+  });
+}
+
+int dcsim_stat_spread(dcsim_t* h, int stat, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                      double* dev_m2_out, uint64_t* dev_hist_out) {
   if (!h || !dev_mean || !dev_lo || !dev_hi || !dev_m2_out || !dev_hist_out) return DCSIM_E_INVALID;
-  const int rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
-  if (rc != DCSIM_OK) return rc;
-  const dcsim_ens_occ_src src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)h->spec.n_dc};
-  return ens_spread(h, src, h->n_replicas, occ_stat_cols(h), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out); /* the bins need no spread */
+  return with_stat(h, stat, true, [&](const auto& src, uint64_t, uint64_t spread_cols) {
+    return ens_spread(h, src, h->n_replicas, spread_cols, dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
+  });
 }
 
 int dcsim_recorder_counts(dcsim_t* h, uint32_t* out3) {

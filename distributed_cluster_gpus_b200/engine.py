@@ -232,15 +232,6 @@ class BatchedEngine:
         self._ens_check(self._lib.dcsim_fetch_cluster_ensemble(self._h, C.c_void_p(out.ctypes.data), out.nbytes))
         return out
 
-    def ensemble_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][capacity * FIELDS * n_dc] float64 {n, sum, min, max} at ``device_ptr``."""
-        self._ens_check(self._lib.dcsim_ensemble_moments(self._h, C.c_void_p(device_ptr)))
-
-    def ensemble_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        self._ens_check(self._lib.dcsim_ensemble_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                        C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)))
-
     # -- job-log ensemble (ensemble.job_ensemble turns it into per-window statistics) --------------------------------
     def enable_job_ensemble(self, bin_s=None):
         """Opt-in, before the first advance of a batch (stays on across reset): every replica sums its finished jobs and
@@ -276,15 +267,6 @@ class BatchedEngine:
                                                    C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
         return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
 
-    def job_ensemble_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][(W + 1) * 3 * n_dc * 2] float64 {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_job_ensemble_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def job_ensemble_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_job_ensemble_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                    C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
-
     def dc_latency_histogram(self) -> np.ndarray:
         """[n_dc, 2, LAT_BINS] uint64: job-latency counts per DC and job type over the replicas with status 0."""
         out = np.zeros((self.spec.n_dc, 2, LAT_BINS), dtype=np.uint64)
@@ -313,15 +295,6 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_job_waits(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
                                                 C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
         return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
-
-    def job_waits_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][(W + 1) * 3 * n_dc * 2] float64 {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_job_waits_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def job_waits_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_job_waits_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                 C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
     def dc_wait_histogram(self) -> np.ndarray:
         """[n_dc, 2 kinds (wait, response), 2, LAT_BINS] uint64 over the replicas with status 0."""
@@ -357,17 +330,6 @@ class BatchedEngine:
                                                     C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
         return rows, mix[:, :, :-1].reshape(n_dc, 2, G, MAX_FREQ, n), np.ascontiguousarray(mix[:, :, -1]), hist
 
-    def job_resources_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][(W + 1) * 6 * n_dc * 2 + n_dc * 2 * (G * MAX_FREQ + 1 + JRES_EBINS)] float64
-        {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_job_resources_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def job_resources_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream, over the (W + 1) * 6 * n_dc * 2 windowed columns: per column sum
-        (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_job_resources_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                     C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
-
     # -- power profile (ensemble.power_profile turns it into batch statistics) ----------------------------------------
     def enable_power_profile(self, threshold=None):
         """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records its
@@ -400,16 +362,6 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_power_profile(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
         return rows
 
-    def power_profile_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][PP_FIELDS + n_dc + PP_BINS] float64 {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_power_profile_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def power_profile_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream over the first PP_FIELDS + n_dc columns: sum (x - mean)^2 and an ENS_BINS
-        histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_power_profile_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                     C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
-
     # -- occupancy (ensemble.occupancy turns it into batch statistics) ------------------------------------------------
     def enable_occupancy(self):
         """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records, per
@@ -437,17 +389,6 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_occupancy(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
         return rows
 
-    def occupancy_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][OCC_FIELDS * n_dc + 2 * OCC_BINS * n_dc] float64 {n, sum, min, max} at
-        ``device_ptr``."""
-        N.check(self._lib.dcsim_occupancy_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def occupancy_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream over the first OCC_FIELDS * n_dc columns: sum (x - mean)^2 and an ENS_BINS
-        histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_occupancy_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                 C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
-
     # -- energy cost and carbon (ensemble.energy_cost turns it into batch statistics) --------------------------------
     def enable_energy_cost(self):
         """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records each
@@ -465,15 +406,6 @@ class BatchedEngine:
         rows = np.empty((S.cost_cols(self.spec.n_dc), self.n_replicas), dtype=np.float64)
         N.check(self._lib.dcsim_fetch_energy_cost(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
         return rows
-
-    def energy_cost_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][cost_cols(n_dc)] float64 {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_energy_cost_moments(self._h, C.c_void_p(device_ptr)), self._h)
-
-    def energy_cost_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream over every column: sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_energy_cost_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                   C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
 
     # -- per-run tail latency (ensemble.tail_latency turns it into batch statistics) ----------------------------------
     def enable_tail_latency(self, sla_s=None):
@@ -512,14 +444,25 @@ class BatchedEngine:
                 self._h)
         return out
 
-    def tail_latency_moments_into(self, device_ptr: int):
-        """Pass 1 on the handle's stream: [4][S.tail_cols(n_dc)] float64 {n, sum, min, max} at ``device_ptr``."""
-        N.check(self._lib.dcsim_tail_latency_moments(self._h, C.c_void_p(device_ptr)), self._h)
+    # -- the two passes of every recorder's statistic (ensemble.py) -------------------------------------------------
+    def stat_columns(self, name: str):
+        """(columns, spread_columns) of recorder ``name`` (one of RECORDERS) as the library reduces them: pass 1 writes
+        [4][columns], pass 2 covers the first spread_columns.  Host arithmetic, whether or not the recorder is on."""
+        cols, spread = C.c_uint64(0), C.c_uint64(0)
+        N.check(self._lib.dcsim_stat_columns(self._h, RECORDERS.index(name), C.byref(cols), C.byref(spread)), self._h)
+        return int(cols.value), int(spread.value)
 
-    def tail_latency_spread_into(self, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
-        """Pass 2 on the handle's stream: per column sum (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
-        N.check(self._lib.dcsim_tail_latency_spread(self._h, C.c_void_p(mean_ptr), C.c_void_p(lo_ptr), C.c_void_p(hi_ptr),
-                                                    C.c_void_p(m2_ptr), C.c_void_p(hist_ptr)), self._h)
+    def stat_moments_into(self, name: str, device_ptr: int):
+        """Pass 1 of recorder ``name`` on the handle's stream: [4][columns] float64 {n, sum, min, max} at
+        ``device_ptr``."""
+        self._ens_check(self._lib.dcsim_stat_moments(self._h, RECORDERS.index(name), C.c_void_p(device_ptr)))
+
+    def stat_spread_into(self, name: str, mean_ptr: int, lo_ptr: int, hi_ptr: int, m2_ptr: int, hist_ptr: int):
+        """Pass 2 of recorder ``name`` on the handle's stream, over its first spread_columns: per column sum
+        (x - mean)^2 and an ENS_BINS histogram over [lo, hi]."""
+        self._ens_check(self._lib.dcsim_stat_spread(self._h, RECORDERS.index(name), C.c_void_p(mean_ptr),
+                                                    C.c_void_p(lo_ptr), C.c_void_p(hi_ptr), C.c_void_p(m2_ptr),
+                                                    C.c_void_p(hist_ptr)))
 
     # -- paired reductions (compare.py) ------------------------------------------------------------------------------
     def paired_moments_into(self, variant_summary_ptr: int, device_ptr: int):

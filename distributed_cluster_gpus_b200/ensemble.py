@@ -21,6 +21,7 @@ Waiting and response times (``BatchedEngine.enable_job_waits``, ``job_waits``) u
 ``WAIT_FIELDS``.
 """
 import csv
+import functools
 import math
 from dataclasses import dataclass
 from typing import Sequence, Tuple
@@ -284,6 +285,14 @@ def device_passes(dev, cols: int, moments_into, spread_into, stat_cols: int = No
     return two_passes(moments, spread)
 
 
+def _recorder_passes(engine, name: str):
+    """device_passes over recorder ``name`` (engine.RECORDERS) of ``engine``, on the columns the library reduces."""
+    import torch
+    cols, spread_cols = engine.stat_columns(name)
+    return device_passes(torch.device("cuda", engine.device), cols, functools.partial(engine.stat_moments_into, name),
+                         functools.partial(engine.stat_spread_into, name), spread_cols)
+
+
 def host_passes(x: np.ndarray, ok: np.ndarray, integral: np.ndarray, stat_cols: int = None):
     """two_passes through the numpy mirror of the kernels over the columns x [columns, R] (ok [columns, R]: the values
     that count), the spread over the first ``stat_cols`` columns (None: all of them), ``integral`` [stat_cols] the
@@ -303,10 +312,7 @@ def cluster_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> 
     """Statistics of the cluster-log ensemble of ``engine`` (a finished BatchedEngine with enable_cluster_ensemble()),
     over all ranks when torch.distributed runs with world > 1 (every rank calls this).  Raises RecorderOverflow if a
     replica recorded more ticks than the capacity."""
-    import torch
-    dev = torch.device("cuda", engine.device)
-    cols = engine.cluster_ensemble_capacity * len(FIELDS) * engine.spec.n_dc
-    passes = device_passes(dev, cols, engine.ensemble_moments_into, engine.ensemble_spread_into)
+    passes = _recorder_passes(engine, "cluster_ensemble")
     return finalize(*passes, engine.spec.n_dc, engine.spec.log_interval, quantiles)
 
 
@@ -452,8 +458,7 @@ def job_ensemble(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobE
     import torch
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
-    cols = (engine.job_ensemble_windows + 1) * len(JOB_FIELDS) * n_dc * 2
-    passes = device_passes(dev, cols, engine.job_ensemble_moments_into, engine.job_ensemble_spread_into)
+    passes = _recorder_passes(engine, "job_ensemble")
     lat_hist = _allreduce_sum(torch.from_numpy(engine.dc_latency_histogram().astype(np.int64)).to(dev))
     return job_finalize(*passes, lat_hist, n_dc, engine.job_ensemble_bin, engine.spec.end_time, quantiles)
 
@@ -617,8 +622,7 @@ def job_waits(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobWait
         raise RuntimeError("job waits not enabled (enable_job_waits)")
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
-    cols = (engine.job_ensemble_windows + 1) * len(WAIT_FIELDS) * n_dc * 2
-    passes = device_passes(dev, cols, engine.job_waits_moments_into, engine.job_waits_spread_into)
+    passes = _recorder_passes(engine, "job_waits")
     wait_hist = _allreduce_sum(torch.from_numpy(engine.dc_wait_histogram().astype(np.int64)).to(dev))
     return waits_finalize(*passes, wait_hist, n_dc, engine.job_ensemble_bin, engine.spec.end_time, quantiles)
 
@@ -835,17 +839,13 @@ def res_finalize(mom, m2, hist, n_dc: int, G: int, levels, bin_s: float, end_tim
 def job_resources(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobResourcesResult:
     """Statistics of the job-resources recorder of ``engine`` (a finished BatchedEngine with enable_job_resources()),
     over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    import torch
     from .engine import jres_mix_g
     if not engine.job_resources_enabled:
         raise RuntimeError("job resources not enabled (enable_job_resources)")
-    dev = torch.device("cuda", engine.device)
     sp = engine.spec
-    G = jres_mix_g(sp.max_gpus_per_job)
-    win = (engine.job_ensemble_windows + 1) * len(RES_FIELDS) * sp.n_dc * 2
-    cols = win + sp.n_dc * 2 * (G * RES_MAX_FREQ + 1 + RES_EBINS)
-    passes = device_passes(dev, cols, engine.job_resources_moments_into, engine.job_resources_spread_into, stat_cols=win)
-    return res_finalize(*passes, sp.n_dc, G, _res_levels(sp), engine.job_ensemble_bin, sp.end_time, quantiles)
+    passes = _recorder_passes(engine, "job_resources")
+    return res_finalize(*passes, sp.n_dc, jres_mix_g(sp.max_gpus_per_job), _res_levels(sp), engine.job_ensemble_bin,
+                        sp.end_time, quantiles)
 
 
 def job_resources_from_rows(rows: np.ndarray, mix: np.ndarray, off_level: np.ndarray, hist: np.ndarray, jobs: np.ndarray,
@@ -1001,8 +1001,7 @@ def power_profile(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES, summary
         raise RuntimeError("power profile not enabled (enable_power_profile)")
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
-    passes = device_passes(dev, len(PP_FIELDS) + n_dc + PP_BINS, engine.power_profile_moments_into,
-                           engine.power_profile_spread_into, stat_cols=len(PP_FIELDS) + n_dc)
+    passes = _recorder_passes(engine, "power_profile")
     energy = _pooled_energy(engine.summary() if summary is None else summary, dev)
     thr = engine.power_threshold
     return pp_finalize(*passes, n_dc, engine.power_profile_range(), float("inf") if thr is None else thr, energy, quantiles)
@@ -1154,15 +1153,10 @@ def occ_finalize(mom, m2, hist, n_dc: int, widths, quantiles: Sequence[float] = 
 def occupancy(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> OccupancyResult:
     """Statistics of the occupancy recorder of ``engine`` (a finished BatchedEngine with enable_occupancy()), over all
     ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    import torch
     if not engine.occupancy_enabled:
         raise RuntimeError("occupancy not enabled (enable_occupancy)")
-    dev = torch.device("cuda", engine.device)
-    n_dc = engine.spec.n_dc
-    stat = len(OCC_STATS) * n_dc
-    passes = device_passes(dev, stat + 2 * OCC_BINS * n_dc, engine.occupancy_moments_into, engine.occupancy_spread_into,
-                           stat_cols=stat)
-    return occ_finalize(*passes, n_dc, engine.occupancy_bin_widths(), quantiles)
+    passes = _recorder_passes(engine, "occupancy")
+    return occ_finalize(*passes, engine.spec.n_dc, engine.occupancy_bin_widths(), quantiles)
 
 
 def occupancy_from_rows(rows: np.ndarray, summary: np.ndarray, widths, quantiles: Sequence[float] = PP_CSV_QUANTILES
@@ -1338,15 +1332,11 @@ def tail_finalize(mom, m2, hist, n_dc: int, sla_s: float, quantiles: Sequence[fl
 def tail_latency(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> TailLatencyResult:
     """Statistics of the per-run tail-latency columns of ``engine`` (a finished BatchedEngine with
     enable_tail_latency()), over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    import torch
-    from . import spec as S
     if not engine.tail_latency_enabled:
         raise RuntimeError("tail latency not enabled (enable_tail_latency)")
-    dev = torch.device("cuda", engine.device)
-    n_dc = engine.spec.n_dc
-    passes = device_passes(dev, S.tail_cols(n_dc), engine.tail_latency_moments_into, engine.tail_latency_spread_into)
+    passes = _recorder_passes(engine, "tail_latency")
     sla = engine.tail_latency_sla
-    return tail_finalize(*passes, n_dc, math.inf if sla is None else sla, quantiles)
+    return tail_finalize(*passes, engine.spec.n_dc, math.inf if sla is None else sla, quantiles)
 
 
 def tail_latency_from_rows(rows: np.ndarray, status, sla_s=None, quantiles: Sequence[float] = PP_CSV_QUANTILES
@@ -1466,14 +1456,10 @@ def _cost_tables(sp):
 def energy_cost(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> EnergyCostResult:
     """Statistics of the energy-cost recorder of ``engine`` (a finished BatchedEngine with enable_energy_cost()), over
     all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    import torch
-    from . import spec as S
     if not engine.energy_cost_enabled:
         raise RuntimeError("energy cost not enabled (enable_energy_cost)")
-    dev = torch.device("cuda", engine.device)
-    n_dc = engine.spec.n_dc
-    passes = device_passes(dev, S.cost_cols(n_dc), engine.energy_cost_moments_into, engine.energy_cost_spread_into)
-    return cost_finalize(*passes, n_dc, *_cost_tables(engine.spec), quantiles)
+    passes = _recorder_passes(engine, "energy_cost")
+    return cost_finalize(*passes, engine.spec.n_dc, *_cost_tables(engine.spec), quantiles)
 
 
 def energy_cost_from_rows(rows: np.ndarray, status, price_kwh, carbon_intensity,

@@ -322,6 +322,40 @@ int dcsim_allreduce_summary(dcsim_t* h, void* nccl_comm, double* out);
 int dcsim_enable_latency_histogram(dcsim_t* h);
 int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
+/* ---- batch-wide statistics of the opt-in batch recorders below ------------------------------------------------------
+ * Each recorder's statistic is a set of columns, each column one value per replica (the recorder's block gives its
+ * columns, which replicas count in them and which columns are integers).  Two passes reduce them on the handle's
+ * stream, with device pointers:
+ *   dcsim_stat_moments  dev_out = [4][columns] doubles {n, sum, min, max} over the replicas that count in each column
+ *                       (an empty column: 0, 0, +inf, -inf).  The caller all-reduces rows 0-1 (sum), 2 (min), 3 (max).
+ *   dcsim_stat_spread   given the global per-column mean, lo (min) and hi (max), over the first spread_columns columns:
+ *                       dev_m2_out[column] = sum (x - mean)^2 and dev_hist_out[column][DCSIM_ENS_BINS] counts over
+ *                       [lo, hi].  Integer columns use unit bins centred on the integers lo, lo+1, ... when
+ *                       hi - lo + 1 <= DCSIM_ENS_BINS, else integer width ceil((hi - lo + 1) / BINS); the others
+ *                       width (hi - lo) / BINS, bin = min(BINS - 1, floor((x - lo) / width)) (all in bin 0 when
+ *                       hi == lo).  The caller all-reduces both (sum).
+ * Both sum in a fixed order (a function of the replica count only): bit-identical run to run.  Each first runs the
+ * recorder's own checks: DCSIM_E_STATE when it is not enabled or the batch has not advanced.  dcsim_stat_columns gives
+ * (columns, spread_columns) for the handle's current state: host arithmetic only, for any valid id whether or not the
+ * recorder is on.  An id outside [0, DCSIM_STATS) is DCSIM_E_INVALID.  The ids follow the order in which a sharded run
+ * computes the statistics (each one all-reduces). */
+enum {
+  DCSIM_STAT_CLUSTER_ENSEMBLE = 0,
+  DCSIM_STAT_JOB_ENSEMBLE,
+  DCSIM_STAT_POWER_PROFILE,
+  DCSIM_STAT_JOB_WAITS,
+  DCSIM_STAT_OCCUPANCY,
+  DCSIM_STAT_TAIL_LATENCY,
+  DCSIM_STAT_JOB_RESOURCES,
+  DCSIM_STAT_ENERGY_COST,
+  DCSIM_STATS
+};
+#define DCSIM_ENS_BINS 1024
+int dcsim_stat_columns(dcsim_t* h, int stat, uint64_t* columns_out, uint64_t* spread_columns_out);
+int dcsim_stat_moments(dcsim_t* h, int stat, double* dev_out);
+int dcsim_stat_spread(dcsim_t* h, int stat, const double* dev_mean, const double* dev_lo, const double* dev_hi,
+                      double* dev_m2_out, uint64_t* dev_hist_out);
+
 /* Cluster-log ensemble: at every log tick, for EVERY replica, the values the replica's cluster_log.csv row of each DC
  * would hold (simulator_paper_multi.py write_csv_logs), unrounded.  Device layout [tick][field][dc][replica] doubles,
  * replica fastest (the reductions read it coalesced).  Tick k is the k-th processed log event (instant: the chain
@@ -342,7 +376,6 @@ enum {
   DCSIM_ENS_ENERGY_J = 10,   /* unrounded (the CSV shows energy_kJ) */
   DCSIM_ENS_FIELDS = 11
 };
-#define DCSIM_ENS_BINS 1024
 /* Opt-in (before the first advance of a batch; stays on across dcsim_reset, like the latency histogram).  max_ticks = 0:
  * the exact number of log ticks of the spec (the t += log_interval chain replayed against the loop's t > end_time
  * cut-off).  DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the buffer does not fit. */
@@ -352,18 +385,9 @@ int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out);
 /* Copies the first min(capacity, out_bytes / row bytes) ticks of the raw values, [tick][field][dc][replica] doubles,
  * to host memory (synchronises).  Ticks a replica did not reach read as NaN.  For tests and small batches. */
 int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes);
-/* Pass 1, per column (tick, field, dc) over the replicas that recorded the tick: dev_out = [4][capacity * FIELDS * n_dc]
- * doubles {n, sum, min, max} (an empty column: 0, 0, +inf, -inf).  The caller all-reduces rows 0-1 (sum), 2 (min), 3
- * (max).  Fixed summation order (a function of the replica count only): bit-identical run to run.  Synchronises once to
- * check the capacity. */
-int dcsim_ensemble_moments(dcsim_t* h, double* dev_out);
-/* Pass 2, given the global per-column mean, lo (min) and hi (max): dev_m2_out[column] = sum (x - mean)^2 (fixed order)
- * and dev_hist_out[column][DCSIM_ENS_BINS] counts over [lo, hi].  Integer fields (busy, run_*, q_*) use unit bins
- * centred on the integers lo, lo+1, ... when hi - lo + 1 <= DCSIM_ENS_BINS, else integer width ceil((hi - lo + 1) / BINS);
- * the others width (hi - lo) / BINS, bin = min(BINS - 1, floor((x - lo) / width)) (all in bin 0 when hi == lo).  The
- * caller all-reduces both (sum). */
-int dcsim_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi, double* dev_m2_out,
-                          uint64_t* dev_hist_out);
+/* DCSIM_STAT_CLUSTER_ENSEMBLE: columns (tick, field, dc), capacity * FIELDS * n_dc of them (0 when not enabled), each
+ * over the replicas that recorded the tick; the spread covers every column.  Integer fields: busy, run_*, q_*.  Both
+ * passes synchronise once to check the capacity. */
 
 /* Job-log ensemble: for EVERY replica, what its job_log.csv rows (simulator_paper_multi.py:820) add up to per finish
  * window, DC and job type.  Window k of W = max(1, ceil(end_time / bin_s)) covers [k * bin_s, (k + 1) * bin_s); a job
@@ -392,12 +416,8 @@ int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out);
  * `hist` [n_replicas][n_dc][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than its array is
  * DCSIM_E_INVALID.  For tests and small batches. */
 int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
-/* Pass 1, per column (row, field, dc, jtype) over the valid replicas: dev_out = [4][(W + 1) * JENS_FIELDS * n_dc * 2]
- * doubles {n, sum, min, max}, the same contract as dcsim_ensemble_moments.  Pass 2: as dcsim_ensemble_spread; JOBS is
- * the integer field (unit bins when its range allows).  Both run on the handle's stream, with device pointers. */
-int dcsim_job_ensemble_moments(dcsim_t* h, double* dev_out);
-int dcsim_job_ensemble_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                              double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_JOB_ENSEMBLE: columns (row, field, dc, jtype), (W + 1) * JENS_FIELDS * n_dc * 2 of them (W = 0 when not
+ * enabled), over the valid replicas; the spread covers every column.  JOBS is the integer field. */
 /* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
 int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
 
@@ -431,11 +451,9 @@ int dcsim_enable_job_waits(dcsim_t* h);
  * [n_replicas] doubles, `hist` [n_replicas][n_dc][2][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than
  * its array is DCSIM_E_INVALID. */
 int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
-/* The two passes over the columns (row, field, dc, jtype), [4][(W + 1) * DCSIM_JWAIT_FIELDS * n_dc * 2]: the contract
- * of dcsim_job_ensemble_moments / _spread; WAITED is the integer field. */
-int dcsim_job_waits_moments(dcsim_t* h, double* dev_out);
-int dcsim_job_waits_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                           double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_JOB_WAITS: columns (row, field, dc, jtype), (W + 1) * DCSIM_JWAIT_FIELDS * n_dc * 2 of them (W = 0 when
+ * the job ensemble is off), over the valid replicas as described above; the spread covers every column.  WAITED is the
+ * integer field. */
 /* The per-DC wait and response histograms summed over the valid replicas: `out` [n_dc][2 kinds][2][DCSIM_LAT_BINS] u64
  * (synchronises). */
 int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
@@ -487,13 +505,9 @@ int dcsim_enable_job_resources(dcsim_t* h);
  * Any may be NULL; a buffer smaller than its array is DCSIM_E_INVALID. */
 int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* mix, size_t mix_bytes, uint32_t* hist,
                               size_t hist_bytes);
-/* Pass 1 over every column, (W + 1) * DCSIM_JRES_FIELDS * n_dc * 2 windowed, then n_dc * 2 * (MIX_COLS(G) + EBINS)
- * counts: dev_out = [4][columns] {n, sum, min, max}; the count columns' sums are the pooled mix and energy histogram.
- * Pass 2 over the windowed columns only: the contract of dcsim_job_ensemble_spread, GPU_SUM the integer field.  Replicas with
- * status 0 count.  Both on the handle's stream, with device pointers. */
-int dcsim_job_resources_moments(dcsim_t* h, double* dev_out);
-int dcsim_job_resources_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                               double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_JOB_RESOURCES: (W + 1) * DCSIM_JRES_FIELDS * n_dc * 2 windowed columns (W = 0 when the job ensemble is
+ * off), then n_dc * 2 * (MIX_COLS(G) + EBINS) count columns, over the replicas with status 0; the count columns' sums
+ * are the pooled mix and energy histogram.  The spread covers the windowed columns only, GPU_SUM the integer field. */
 
 /* Power profile: for EVERY replica, the cluster power P(t) its total energy integrates, as a step function, and what a
  * site is sized by — peak, time and energy over a threshold, a time-weighted power histogram.
@@ -531,14 +545,10 @@ int dcsim_enable_power_profile(dcsim_t* h, double threshold_w);
 int dcsim_power_profile_range(dcsim_t* h, double* hi_out);
 /* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
 int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes);
-/* Pass 1 over every column (the fields, DC_PEAK_W, the bins) and the replicas with status 0: dev_out =
- * [4][DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS] {n, sum, min, max}; the bins' sums are the pooled power-duration curve.
- * Pass 2 over the first DCSIM_PP_FIELDS + n_dc columns only (the bins need no spread): m2 and histograms, the contract
- * of dcsim_ensemble_spread; EXCURSIONS and OUT_OF_RANGE are the integer columns.  Both on the handle's stream, with
- * device pointers. */
-int dcsim_power_profile_moments(dcsim_t* h, double* dev_out);
-int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                               double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_POWER_PROFILE: every stored column (the fields, DC_PEAK_W, the bins), DCSIM_PP_FIELDS + n_dc +
+ * DCSIM_PP_BINS of them, over the replicas with status 0; the bins' sums are the pooled power-duration curve.  The
+ * spread covers the first DCSIM_PP_FIELDS + n_dc columns only (the bins need none); EXCURSIONS and OUT_OF_RANGE are the
+ * integer columns. */
 
 /* Energy cost and carbon: for EVERY replica and DC d, the energy d drew in each hour of the day, priced at d's hourly
  * tariff (price_kwh[d][h], USD/kWh) and weighted by its carbon intensity (carbon_intensity[d], gCO2/kWh).
@@ -576,11 +586,8 @@ int dcsim_power_profile_spread(dcsim_t* h, const double* dev_mean, const double*
 int dcsim_enable_energy_cost(dcsim_t* h);
 /* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
 int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes);
-/* The two passes over every column and the replicas with status 0: the contract of dcsim_ensemble_moments / _spread
- * (no integer columns).  Both on the handle's stream, with device pointers. */
-int dcsim_energy_cost_moments(dcsim_t* h, double* dev_out);
-int dcsim_energy_cost_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                             double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_ENERGY_COST: the DCSIM_COST_COLS(n_dc) stored columns, over the replicas with status 0; the spread covers
+ * every column.  No integer columns. */
 
 /* Occupancy: for EVERY replica and DC d, how long the queues were and how full the DC was over time.  Step functions over
  * [t0, end_time]: Qi(t) = len(q_inf), Qt(t) = len(q_train), Q = Qi + Qt, N(t) = running jobs, B(t) = busy GPUs.
@@ -614,16 +621,11 @@ int dcsim_enable_occupancy(dcsim_t* h);
 int dcsim_occupancy_bin_widths(dcsim_t* h, int32_t* w_out);
 /* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
 int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes);
-/* Columns: first DCSIM_OCC_FIELDS * n_dc statistics (field, dc), field-major, per replica Q_INF_AREA / PROFILE_S,
- * Q_TRN_AREA / PROFILE_S, RUN_AREA / PROFILE_S, Q_INF_MAX, Q_TRN_MAX, QUEUED_S / PROFILE_S, SATURATED_S / PROFILE_S,
- * IDLE_S / PROFILE_S; then the 2 * DCSIM_OCC_BINS * n_dc bins as stored.  A replica counts when its status is 0 and
- * PROFILE_S > 0.  Pass 1 over every column: dev_out = [4][columns] {n, sum, min, max}; the bins' sums are the pooled
- * time-weighted distributions of queue length and busy GPUs.  Pass 2 over the statistics columns only: m2 and
- * histograms, the contract of dcsim_ensemble_spread; Q_INF_MAX and Q_TRN_MAX are the integer columns.  Both on the
- * handle's stream, with device pointers. */
-int dcsim_occupancy_moments(dcsim_t* h, double* dev_out);
-int dcsim_occupancy_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                           double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_OCCUPANCY: first DCSIM_OCC_FIELDS * n_dc statistics (field, dc), field-major, per replica Q_INF_AREA /
+ * PROFILE_S, Q_TRN_AREA / PROFILE_S, RUN_AREA / PROFILE_S, Q_INF_MAX, Q_TRN_MAX, QUEUED_S / PROFILE_S, SATURATED_S /
+ * PROFILE_S, IDLE_S / PROFILE_S; then the 2 * DCSIM_OCC_BINS * n_dc bins as stored.  A replica counts when its status
+ * is 0 and PROFILE_S > 0.  The bins' sums are the pooled time-weighted distributions of queue length and busy GPUs.
+ * The spread covers the statistics columns only; Q_INF_MAX and Q_TRN_MAX are the integer columns. */
 
 /* Per-run tail latency: for EVERY replica, exact order statistics of its own finished jobs.  For a job that finished
  * (status 0 replica) with arrival instant arr (the ingress arrival, simulator_paper_multi.py:539-540), xfer_done instant
@@ -660,25 +662,22 @@ enum {
  * (with the byte count in dcsim_last_error) when the buffers do not fit. */
 int dcsim_enable_tail_latency(dcsim_t* h, double sla_s);
 /* The columns to host memory, [DCSIM_TAIL_COLS(n_dc)][n_replicas] doubles (synchronises).  The columns are made from
- * the slot buffer by one selection pass on the handle's stream, run by the first of this call, _moments or _spread
- * after the batch is done (every later advance or reset makes them stale); DCSIM_E_STATE while a replica is still
- * running.  A smaller buffer is DCSIM_E_INVALID. */
+ * the slot buffer by one selection pass on the handle's stream, run by the first of this call, dcsim_stat_moments or
+ * dcsim_stat_spread after the batch is done (every later advance or reset makes them stale); DCSIM_E_STATE while a
+ * replica is still running.  A smaller buffer is DCSIM_E_INVALID. */
 int dcsim_fetch_tail_latency(dcsim_t* h, double* out, size_t out_bytes);
 /* The raw slot buffer of local replicas [first, first + count): [count][cap_arrivals][2] doubles, (start, finish) of
  * arrival slot jid - 1 (synchronises).  A range, because a large batch's buffer takes tens of GB. */
 int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* out, size_t out_bytes);
-/* The two passes over the DCSIM_TAIL_COLS(n_dc) columns: the contract of dcsim_ensemble_moments / _spread.  A replica
- * counts in a column when its status is 0 and the value is not NaN.  JOBS, UNFINISHED and SLA_MET are integer columns. */
-int dcsim_tail_latency_moments(dcsim_t* h, double* dev_out);
-int dcsim_tail_latency_spread(dcsim_t* h, const double* dev_mean, const double* dev_lo, const double* dev_hi,
-                              double* dev_m2_out, uint64_t* dev_hist_out);
+/* DCSIM_STAT_TAIL_LATENCY: the DCSIM_TAIL_COLS(n_dc) columns; the spread covers every column.  A replica counts in a
+ * column when its status is 0 and the value is not NaN.  JOBS, UNFINISHED and SLA_MET are integer columns. */
 
 /* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant
  * batch with the same keys (a member's dcsim_summary_device_ptr or a copy of it: [n][DCSIM_SUMMARY_K] doubles on the
  * base's device).  Replica r counts in a column when both rows have status 0 and the metric is defined in both (a
  * per-job or latency metric needs a finished job of that kind).  n_cols = (DCSIM_PAIR_DC_ENERGY_J + n_dc) *
- * DCSIM_PAIR_FIELDS.  The same two passes and contract as dcsim_ensemble_moments / _spread, on the base's stream; n
- * must be the base's replica count.  JOBS_*, UNFINISHED and their differences, and LOWER / HIGHER, are integer columns
+ * DCSIM_PAIR_FIELDS.  The same two passes and contract as dcsim_stat_moments / _spread, on the base's stream; n must
+ * be the base's replica count.  JOBS_*, UNFINISHED and their differences, and LOWER / HIGHER, are integer columns
  * (unit bins when their range allows). */
 enum {
   DCSIM_PAIR_ENERGY_J = 0,         /* total energy [J] */

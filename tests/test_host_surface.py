@@ -29,6 +29,15 @@ def test_library_loads_and_exports_every_declared_symbol():
     assert lib.dcsim_summary_k() == S.SUMMARY_K == 88
 
 
+def test_statistic_ids_follow_the_recorder_order():
+    """engine.stat_* pass RECORDERS.index(name) as the library's DCSIM_STAT_* id."""
+    from distributed_cluster_gpus_b200.engine import RECORDERS
+    header = open(os.path.join(ROOT, "include", "dcsim_b200.h")).read()
+    block = re.search(r"enum \{\s*(DCSIM_STAT_CLUSTER_ENSEMBLE = 0,.*?)\};", header, re.S).group(1)
+    assert block.rstrip().endswith("DCSIM_STATS")
+    assert [i.lower() for i in re.findall(r"DCSIM_STAT_([A-Z_]+)", block)] == list(RECORDERS)
+
+
 def test_create_rejects_bad_arguments_without_a_gpu():
     lib = _native.load()
     h = C.c_void_p()

@@ -24,13 +24,17 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
+# --recorder -> the recorder's name in engine.RECORDERS
+RECORDERS = {"cluster": "cluster_ensemble", "job": "job_ensemble", "power": "power_profile", "waits": "job_waits",
+             "occupancy": "occupancy", "tail": "tail_latency", "resources": "job_resources", "cost": "energy_cost"}
+
 
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--replicas", type=int, default=65536)
     ap.add_argument("--scenario", default="cfg3_4x64_sinusoid_120s")
     ap.add_argument("--rounds", type=int, default=3)
-    ap.add_argument("--recorder", choices=["cluster", "job", "power", "waits", "occupancy", "tail", "resources", "cost"], default="cluster")
+    ap.add_argument("--recorder", choices=list(RECORDERS), default="cluster")
     args = ap.parse_args()
 
     import torch
@@ -79,27 +83,19 @@ def main():
     try:
         on.advance(0)
         events = float(on.summary()[:, S.S_EVENTS].sum())
+        recorder = RECORDERS[args.recorder]
+        cols, spread_cols = on.stat_columns(recorder)
         if args.recorder == "power":
-            cols = S.PP_FIELDS + sp.n_dc + S.PP_BINS
-            moments_into, spread_into = on.power_profile_moments_into, on.power_profile_spread_into
             rows, recorder_bytes = cols, cols * 8 + 20 * 8      # columns + the working row (DCSIM_PPW_N doubles)
         elif args.recorder == "occupancy":
-            cols = (S.OCC_FIELDS + 2 * S.OCC_BINS) * sp.n_dc
-            moments_into, spread_into = on.occupancy_moments_into, on.occupancy_spread_into
             rows, recorder_bytes = cols + 1, (cols + 1) * 8 + sp.n_dc * 11 * 8   # columns + working rows (DCSIM_OCCW_N)
         elif args.recorder == "cost":
-            cols = S.cost_cols(sp.n_dc)
-            moments_into, spread_into = on.energy_cost_moments_into, on.energy_cost_spread_into
             rows, recorder_bytes = cols, S.cost_bytes_per_replica(sp.n_dc)   # columns + working rows (3 doubles per DC)
             stats = EN.energy_cost(on).pooled()
         elif args.recorder == "tail":
-            cols = S.tail_cols(sp.n_dc)
-            moments_into, spread_into = on.tail_latency_moments_into, on.tail_latency_spread_into
             cap = sp.cap_arrivals if sp.cap_arrivals > 0 else 16384
             rows, recorder_bytes = cols, cols * 8 + cap * 16     # columns + the slot buffer (16 B per arrival slot)
         elif args.recorder == "waits":
-            cols = (on.job_ensemble_windows + 1) * len(EN.WAIT_FIELDS) * sp.n_dc * 2
-            moments_into, spread_into = on.job_waits_moments_into, on.job_waits_spread_into
             rows, recorder_bytes = on.job_ensemble_windows + 1, ((on.job_ensemble_windows + 1) * 3 * sp.n_dc * 2 * 8
                                                                  + sp.n_dc * 2 * 2 * EN.LAT_BINS * 4)
             summ = on.summary()
@@ -110,37 +106,29 @@ def main():
                 stats[name]["mean_service_s"] = float(lat / fin) if fin else float("nan")
         elif args.recorder == "resources":
             win = on.job_ensemble_windows + 1
-            G = min(max(sp.max_gpus_per_job, 1), 32)
-            counts = sp.n_dc * 2 * (G * EN.RES_MAX_FREQ + 1 + EN.RES_EBINS)
-            cols = win * len(EN.RES_FIELDS) * sp.n_dc * 2 + counts
-            moments_into, spread_into = on.job_resources_moments_into, on.job_resources_spread_into
-            rows, recorder_bytes = win, win * 3 * sp.n_dc * 2 * 8 + counts * 4
+            rows, recorder_bytes = win, win * 3 * sp.n_dc * 2 * 8 + (cols - spread_cols) * 4   # sums + u32 counts
             stats = EN.job_resources(on).pooled()
         elif args.recorder == "job":
-            cols = (on.job_ensemble_windows + 1) * len(EN.JOB_FIELDS) * sp.n_dc * 2
-            moments_into, spread_into = on.job_ensemble_moments_into, on.job_ensemble_spread_into
             rows, recorder_bytes = on.job_ensemble_windows + 1, ((on.job_ensemble_windows + 1) * 2 * sp.n_dc * 2 * 8
                                                                  + sp.n_dc * 2 * EN.LAT_BINS * 4)
         else:
-            cols = on.cluster_ensemble_capacity * len(EN.FIELDS) * sp.n_dc
-            moments_into, spread_into = on.ensemble_moments_into, on.ensemble_spread_into
             rows, recorder_bytes = on.cluster_ensemble_capacity, cols * 8
         mom = torch.zeros((4, cols), dtype=torch.float64, device="cuda")
-        m2 = torch.zeros(cols, dtype=torch.float64, device="cuda")
-        hist = torch.zeros((cols, EN.BINS), dtype=torch.int64, device="cuda")
+        m2 = torch.zeros(spread_cols, dtype=torch.float64, device="cuda")
+        hist = torch.zeros((spread_cols, EN.BINS), dtype=torch.int64, device="cuda")
         ev = [torch.cuda.Event(enable_timing=True) for _ in range(4)]
         first_moments_ms = None
         for _ in range(2):
             torch.cuda.synchronize()
             ev[0].record(stream)
-            moments_into(mom.data_ptr())
+            on.stat_moments_into(recorder, mom.data_ptr())
             ev[1].record(stream)
             cnt = mom[0]
             mean = torch.where(cnt > 0, mom[1] / cnt.clamp(min=1.0), torch.zeros_like(cnt)).contiguous()
             lo, hi = mom[2].contiguous(), mom[3].contiguous()
             torch.cuda.synchronize()
             ev[2].record(stream)
-            spread_into(mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
+            on.stat_spread_into(recorder, mean.data_ptr(), lo.data_ptr(), hi.data_ptr(), m2.data_ptr(), hist.data_ptr())
             ev[3].record(stream)
             torch.cuda.synchronize()
             first_moments_ms = ev[0].elapsed_time(ev[1]) if first_moments_ms is None else first_moments_ms
