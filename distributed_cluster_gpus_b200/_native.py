@@ -22,15 +22,9 @@ EXPORTS = (
     "dcsim_fetch_cluster_log", "dcsim_launch_info", "dcsim_last_error", "dcsim_destroy", "dcsim_set_rng",
     "dcsim_recorder_counts", "dcsim_allreduce_summary", "dcsim_fetch_summary_host",
     "dcsim_stat_columns", "dcsim_stat_moments", "dcsim_stat_spread",
-    "dcsim_enable_cluster_ensemble", "dcsim_cluster_ensemble_capacity", "dcsim_fetch_cluster_ensemble",
-    "dcsim_enable_job_ensemble", "dcsim_job_ensemble_windows", "dcsim_fetch_job_ensemble", "dcsim_fetch_dc_latency_histogram",
+    "dcsim_recorder_enable", "dcsim_recorder_state", "dcsim_recorder_fetch", "dcsim_recorder_histogram",
     "dcsim_arrivals_compatible", "dcsim_create_shared", "dcsim_paired_moments", "dcsim_paired_spread",
-    "dcsim_enable_power_profile", "dcsim_power_profile_range", "dcsim_fetch_power_profile",
-    "dcsim_enable_job_waits", "dcsim_fetch_job_waits", "dcsim_fetch_dc_wait_histogram",
-    "dcsim_enable_job_resources", "dcsim_fetch_job_resources",
-    "dcsim_enable_occupancy", "dcsim_occupancy_bin_widths", "dcsim_fetch_occupancy",
-    "dcsim_enable_tail_latency", "dcsim_fetch_tail_latency", "dcsim_fetch_tail_jobs",
-    "dcsim_enable_energy_cost", "dcsim_fetch_energy_cost",
+    "dcsim_power_profile_range", "dcsim_occupancy_bin_widths", "dcsim_fetch_tail_jobs",
 )
 
 _lib = None
@@ -107,22 +101,21 @@ def load():
         L.dcsim_stat_moments.argtypes = [vp, i32, vp]
         L.dcsim_stat_spread.restype = i32
         L.dcsim_stat_spread.argtypes = [vp, i32, vp, vp, vp, vp, vp]
-    if hasattr(L, "dcsim_enable_cluster_ensemble"):
-        L.dcsim_enable_cluster_ensemble.restype = i32
-        L.dcsim_enable_cluster_ensemble.argtypes = [vp, u32]
-        L.dcsim_cluster_ensemble_capacity.restype = i32
-        L.dcsim_cluster_ensemble_capacity.argtypes = [vp, C.POINTER(u32)]
-        L.dcsim_fetch_cluster_ensemble.restype = i32
-        L.dcsim_fetch_cluster_ensemble.argtypes = [vp, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_job_ensemble"):
-        L.dcsim_enable_job_ensemble.restype = i32
-        L.dcsim_enable_job_ensemble.argtypes = [vp, C.c_double]
-        L.dcsim_job_ensemble_windows.restype = i32
-        L.dcsim_job_ensemble_windows.argtypes = [vp, C.POINTER(u32)]
-        L.dcsim_fetch_job_ensemble.restype = i32
-        L.dcsim_fetch_job_ensemble.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
-        L.dcsim_fetch_dc_latency_histogram.restype = i32
-        L.dcsim_fetch_dc_latency_histogram.argtypes = [vp, vp, C.c_size_t]
+    if hasattr(L, "dcsim_recorder_enable"):
+        L.dcsim_recorder_enable.restype = i32
+        L.dcsim_recorder_enable.argtypes = [vp, i32, C.c_double]
+        L.dcsim_recorder_state.restype = i32
+        L.dcsim_recorder_state.argtypes = [vp, i32, C.POINTER(S.RecorderState)]
+        L.dcsim_recorder_fetch.restype = i32
+        L.dcsim_recorder_fetch.argtypes = [vp, i32, i32, vp, C.c_size_t]
+        L.dcsim_recorder_histogram.restype = i32
+        L.dcsim_recorder_histogram.argtypes = [vp, i32, vp, C.c_size_t]
+        L.dcsim_power_profile_range.restype = i32
+        L.dcsim_power_profile_range.argtypes = [vp, C.POINTER(C.c_double)]
+        L.dcsim_occupancy_bin_widths.restype = i32
+        L.dcsim_occupancy_bin_widths.argtypes = [vp, vp]
+        L.dcsim_fetch_tail_jobs.restype = i32
+        L.dcsim_fetch_tail_jobs.argtypes = [vp, u64, u64, vp, C.c_size_t]
     if hasattr(L, "dcsim_create_shared"):
         L.dcsim_arrivals_compatible.restype = i32
         L.dcsim_arrivals_compatible.argtypes = [vp, C.c_size_t, vp, C.c_size_t, C.POINTER(i32)]
@@ -132,44 +125,6 @@ def load():
         L.dcsim_paired_moments.argtypes = [vp, vp, u64, vp]
         L.dcsim_paired_spread.restype = i32
         L.dcsim_paired_spread.argtypes = [vp, vp, u64, vp, vp, vp, vp, vp]
-    if hasattr(L, "dcsim_enable_job_waits"):
-        L.dcsim_enable_job_waits.restype = i32
-        L.dcsim_enable_job_waits.argtypes = [vp]
-        L.dcsim_fetch_job_waits.restype = i32
-        L.dcsim_fetch_job_waits.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t]
-        L.dcsim_fetch_dc_wait_histogram.restype = i32
-        L.dcsim_fetch_dc_wait_histogram.argtypes = [vp, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_job_resources"):
-        L.dcsim_enable_job_resources.restype = i32
-        L.dcsim_enable_job_resources.argtypes = [vp]
-        L.dcsim_fetch_job_resources.restype = i32
-        L.dcsim_fetch_job_resources.argtypes = [vp, vp, C.c_size_t, vp, C.c_size_t, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_occupancy"):
-        L.dcsim_enable_occupancy.restype = i32
-        L.dcsim_enable_occupancy.argtypes = [vp]
-        L.dcsim_occupancy_bin_widths.restype = i32
-        L.dcsim_occupancy_bin_widths.argtypes = [vp, vp]
-        L.dcsim_fetch_occupancy.restype = i32
-        L.dcsim_fetch_occupancy.argtypes = [vp, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_tail_latency"):
-        L.dcsim_enable_tail_latency.restype = i32
-        L.dcsim_enable_tail_latency.argtypes = [vp, C.c_double]
-        L.dcsim_fetch_tail_latency.restype = i32
-        L.dcsim_fetch_tail_latency.argtypes = [vp, vp, C.c_size_t]
-        L.dcsim_fetch_tail_jobs.restype = i32
-        L.dcsim_fetch_tail_jobs.argtypes = [vp, u64, u64, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_power_profile"):
-        L.dcsim_enable_power_profile.restype = i32
-        L.dcsim_enable_power_profile.argtypes = [vp, C.c_double]
-        L.dcsim_power_profile_range.restype = i32
-        L.dcsim_power_profile_range.argtypes = [vp, C.POINTER(C.c_double)]
-        L.dcsim_fetch_power_profile.restype = i32
-        L.dcsim_fetch_power_profile.argtypes = [vp, vp, C.c_size_t]
-    if hasattr(L, "dcsim_enable_energy_cost"):
-        L.dcsim_enable_energy_cost.restype = i32
-        L.dcsim_enable_energy_cost.argtypes = [vp]
-        L.dcsim_fetch_energy_cost.restype = i32
-        L.dcsim_fetch_energy_cost.argtypes = [vp, vp, C.c_size_t]
     L.dcsim_launch_info.restype = i32
     L.dcsim_launch_info.argtypes = [vp, C.POINTER(S.LaunchInfo)]
     L.dcsim_last_error.restype = C.c_char_p

@@ -564,6 +564,15 @@ static void group_release(dcsim_group* g) {
   delete g;
 }
 
+/* An opt-in batch recorder of a handle: its device buffers (d[0] != NULL: enabled), its resolved argument (bin_s,
+ * threshold_w or sla_s; 0 for the others) and its rows (cluster ensemble: the tick capacity; job ensemble, job waits,
+ * job resources: W + 1; the others: 1).  All zero while it is off. */
+struct dcsim_slot {
+  void* d[2];
+  double arg;
+  uint64_t rows;
+};
+
 struct dcsim {
   dcsim_spec_t spec;
   dcsim_layout_t L;
@@ -591,41 +600,22 @@ struct dcsim {
   int launches;
   int mode; /* DCSIM_MODE_* of the advance kernel for this handle's layout */
   uint32_t* d_hist;
-  double* d_ens;       /* [ens_cap][DCSIM_ENS_FIELDS][n_dc][n_replicas] cluster-log ensemble (opt-in) */
-  uint32_t* d_ens_nlog; /* [n_replicas] ticks each replica recorded, + 1 word: the largest DCSIM_S_EV_LOG */
-  uint32_t ens_cap;
-  double* d_jens;          /* [jens_windows + 1][DCSIM_JENS_STORED][n_dc][2][n_replicas] job-log ensemble (opt-in) */
-  uint32_t* d_jens_hist;   /* [n_replicas][n_dc][2][DCSIM_LAT_BINS] its per-DC latency histograms */
-  unsigned long long* d_jens_hist_out; /* [n_dc][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_latency_histogram */
-  double jens_bin;
-  uint64_t jens_windows;
-  double* d_pp;            /* [DCSIM_PP_FIELDS + n_dc + DCSIM_PP_BINS][n_replicas] power profile (opt-in) */
-  double* d_pp_work;       /* [n_replicas][DCSIM_PPW_N] its working state */
-  double pp_threshold;
-  double* d_occ;           /* [1 + DCSIM_OCC_FIELDS * n_dc + 2 * DCSIM_OCC_BINS * n_dc][n_replicas] occupancy (opt-in) */
-  double* d_occ_work;      /* [n_replicas][n_dc][DCSIM_OCCW_N] its working state */
-  double* d_tail;          /* [n_replicas][cap_arr][2] per-run tail latency: (start, finish) per arrival slot (opt-in) */
-  double* d_tail_cols;     /* [DCSIM_TAIL_COLS(n_dc)][n_replicas] its columns */
-  double tail_sla;
-  int tail_fresh;          /* 1: the columns were selected from this batch's finished slots */
-  double* d_jwait;         /* [jens_windows + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] waiting / response times (opt-in) */
-  uint32_t* d_jwait_hist;  /* [n_replicas][n_dc][2 kinds][2][DCSIM_LAT_BINS] their per-DC histograms */
-  unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of dcsim_fetch_dc_wait_histogram */
-  double* d_jres;          /* [jens_windows + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas] job resources (opt-in) */
-  uint32_t* d_jres_cnt;    /* [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] mix, then [n_dc][2][DCSIM_JRES_EBINS][n_replicas]
-                              energy bins */
-  double* d_cost;          /* [DCSIM_COST_COLS(n_dc)][n_replicas] energy cost and carbon (opt-in) */
-  double* d_cost_work;     /* [n_replicas][n_dc][DCSIM_COSTW_N] its working state */
-  uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the job ensemble and power profile
-                         reductions, refreshed on the stream ahead of every one of them (status_words) */
+  dcsim_slot rec[DCSIM_STATS]; /* the opt-in batch recorders, by DCSIM_STAT_* (their buffers: recorder_table) */
+  int tail_fresh;          /* 1: the tail columns were selected from this batch's finished slots */
+  uint32_t* d_ens_nlog; /* [n_replicas] ticks each cluster-ensemble replica recorded, + 1 word: the largest DCSIM_S_EV_LOG */
+  unsigned long long* d_jens_hist_out;  /* [n_dc][2][DCSIM_LAT_BINS]: scratch of the job ensemble's histogram */
+  unsigned long long* d_jwait_hist_out; /* [n_dc][2][2][DCSIM_LAT_BINS]: scratch of the job waits' histogram */
+  uint32_t* d_status; /* [n_replicas] status words (+ 1 word: their maximum) of the recorder reductions, refreshed on
+                         the stream ahead of every one of them (status_words) */
   unsigned long long events_seen;
   char err[512];
 };
 
 static thread_local char g_create_err[512] = "";
 
-static size_t ens_bytes(const dcsim_t* h, uint32_t ticks) {
-  return (size_t)ticks * DCSIM_ENS_FIELDS * (size_t)h->spec.n_dc * (size_t)h->n_replicas * sizeof(double);
+/* The byte sizes of the recorders' buffers (recorder_table): a whole buffer, or one row of those sized by rows. */
+static size_t ens_tick_bytes(const dcsim_t* h) { /* one tick of the cluster-log ensemble */
+  return (size_t)DCSIM_ENS_FIELDS * (size_t)h->spec.n_dc * (size_t)h->n_replicas * sizeof(double);
 }
 
 static size_t jens_row_bytes(const dcsim_t* h) { /* one row (window) of the job-log ensemble */
@@ -647,9 +637,9 @@ static uint64_t jres_mix_cols(const dcsim_t* h) { /* per replica */
   return 2ull * (uint64_t)h->spec.n_dc * (uint64_t)DCSIM_JRES_MIX_COLS(DCSIM_JRES_G(h->spec.max_gpus_per_job));
 }
 static uint64_t jres_hist_cols(const dcsim_t* h) { return 2ull * (uint64_t)h->spec.n_dc * DCSIM_JRES_EBINS; }
-static size_t jres_cnt_bytes(const dcsim_t* h) {
-  return (size_t)(jres_mix_cols(h) + jres_hist_cols(h)) * (size_t)h->n_replicas * sizeof(uint32_t);
-}
+static size_t jres_mix_bytes(const dcsim_t* h) { return (size_t)jres_mix_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t); }
+static size_t jres_ebin_bytes(const dcsim_t* h) { return (size_t)jres_hist_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t); }
+static size_t jres_cnt_bytes(const dcsim_t* h) { return jres_mix_bytes(h) + jres_ebin_bytes(h); }
 
 static uint64_t pp_cols(const dcsim_t* h) { return (uint64_t)(DCSIM_PP_FIELDS + h->spec.n_dc + DCSIM_PP_BINS); }
 static size_t pp_bytes(const dcsim_t* h) { return (size_t)pp_cols(h) * (size_t)h->n_replicas * sizeof(double); }
@@ -687,24 +677,101 @@ static int set_err(dcsim_t* h, int code, const char* fmt, const char* a = "", lo
                      "CUDA error: %s (line %lld)", cudaGetErrorString(e_), (long long)__LINE__); \
   } while (0)
 
-/* The device buffers of an opt-in recorder: *a and, when b is given, *b — both or neither.  Running out of device memory
- * is DCSIM_E_NOMEM with `need` bytes in the message `nomem_fmt`, and clears the sticky error: the handle stays usable. */
-static int recorder_alloc(dcsim_t* h, void** a, size_t a_bytes, void** b, size_t b_bytes, const char* nomem_fmt, long long need) {
-  cudaError_t e = cudaMalloc(a, a_bytes);
-  if (e != cudaSuccess) *a = NULL;
-  else if (b && (e = cudaMalloc(b, b_bytes)) != cudaSuccess) { cudaFree(*a); *a = NULL; *b = NULL; }
-  if (e == cudaSuccess) return DCSIM_OK;
-  if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
-  cudaGetLastError();
-  return set_err(h, DCSIM_E_NOMEM, nomem_fmt, "", need);
+/* ---- the opt-in batch recorders: what each one does differently, by DCSIM_STAT_* ------------------------------------
+ * Enabling one (dcsim_recorder_enable) checks, in this order: its argument, that the job ensemble is on (needs_jens),
+ * that the handle is not a group member (unless member_ok), and — unless a re-targeting recorder is asked for the target
+ * it has — that the batch has not advanced.  A re-targeting recorder (the two ensembles: their rows depend on the
+ * argument) frees its buffers and those of the recorders that need it, then allocates anew; the others keep theirs and
+ * only take the new argument.  Every buffer is filled with its `fill` byte on enable and on dcsim_reset (-1: left as it
+ * is).  A fetch (dcsim_recorder_fetch) copies the recorder's parts, each one a buffer or the next `bytes` of it. */
+enum { ARG_NONE, ARG_TICKS, ARG_BIN, ARG_LIMIT }; /* max_ticks; bin_s (finite, >= 0); threshold_w / sla_s (>= 0, +inf: none) */
+typedef size_t (*rec_bytes_fn)(const dcsim_t*);
+struct rec_buf { rec_bytes_fn bytes; bool per_row; int fill; };
+struct rec_part { int buf; rec_bytes_fn bytes; /* NULL: the whole buffer */ };
+struct rec_desc {
+  const char* name;
+  int arg;
+  const char* arg_name;
+  rec_buf buf[2];      /* bytes == NULL: no second buffer */
+  rec_part part[3];
+  int parts;
+  bool retarget, needs_jens, member_ok;
+  const char* nomem_hint;
+  int (*ready)(dcsim_t*); /* the read precondition beyond recorder_ready (NULL: none) */
+};
+
+static int ens_counts(dcsim_t* h);
+static int tail_ready(dcsim_t* h);
+
+static const char* const FEWER = "run fewer replicas";
+static const char* const WIDER = "a wider bin_s or fewer replicas";
+static const rec_desc recorder_table[DCSIM_STATS] = {
+  /* DCSIM_STAT_CLUSTER_ENSEMBLE: [ticks][FIELDS][n_dc][n] rows, NaN until recorded */
+  {"cluster ensemble", ARG_TICKS, "max_ticks", {{ens_tick_bytes, true, 0xff}, {}}, {{0, NULL}}, 1,
+   true, false, true, FEWER, ens_counts},
+  /* DCSIM_STAT_JOB_ENSEMBLE: rows, per-replica latency histograms */
+  {"job ensemble", ARG_BIN, "bin_s", {{jens_row_bytes, true, 0}, {jens_hist_bytes, false, 0}}, {{0, NULL}, {1, NULL}}, 2,
+   true, false, true, WIDER, NULL},
+  /* DCSIM_STAT_POWER_PROFILE: columns, working state */
+  {"power profile", ARG_LIMIT, "threshold_w", {{pp_bytes, false, 0}, {pp_work_bytes, false, 0}}, {{0, NULL}}, 1,
+   false, false, false, FEWER, NULL},
+  /* DCSIM_STAT_JOB_WAITS: rows, per-replica wait and response histograms */
+  {"job waits", ARG_NONE, NULL, {{jwait_row_bytes, true, 0}, {jwait_hist_bytes, false, 0}}, {{0, NULL}, {1, NULL}}, 2,
+   false, true, false, WIDER, NULL},
+  /* DCSIM_STAT_OCCUPANCY: columns, working state */
+  {"occupancy", ARG_NONE, NULL, {{occ_bytes, false, 0}, {occ_work_bytes, false, 0}}, {{0, NULL}}, 1,
+   false, false, false, FEWER, NULL},
+  /* DCSIM_STAT_TAIL_LATENCY: the slot buffer (NaN: not finished), the columns the selection pass writes; a fetch copies
+   * the columns (dcsim_fetch_tail_jobs reads the slots by replica range) */
+  {"tail latency", ARG_LIMIT, "sla_s", {{tail_slot_bytes, false, 0xff}, {tail_cols_bytes, false, -1}}, {{1, NULL}}, 1,
+   false, false, false, FEWER, tail_ready},
+  /* DCSIM_STAT_JOB_RESOURCES: rows, then the counts: the mix, then the energy bins */
+  {"job resources", ARG_NONE, NULL, {{jres_row_bytes, true, 0}, {jres_cnt_bytes, false, 0}},
+   {{0, NULL}, {1, jres_mix_bytes}, {1, jres_ebin_bytes}}, 3, false, true, false, WIDER, NULL},
+  /* DCSIM_STAT_ENERGY_COST: columns, working state */
+  {"energy cost", ARG_NONE, NULL, {{cost_bytes, false, 0}, {cost_work_bytes, false, 0}}, {{0, NULL}}, 1,
+   false, false, false, FEWER, NULL},
+};
+
+static size_t rec_buf_bytes(const dcsim_t* h, int stat, int k) {
+  const rec_buf& b = recorder_table[stat].buf[k];
+  return (b.per_row ? (size_t)h->rec[stat].rows : 1) * b.bytes(h);
 }
 
-/* A read of an opt-in recorder (`rec`; NULL: not enabled) needs it enabled and the batch advanced. */
-static int recorder_ready(dcsim_t* h, const void* rec, const char* what, const char* enable_fn) {
-  if (!rec) { snprintf(h->err, sizeof(h->err), "%s not enabled (%s)", what, enable_fn); return DCSIM_E_STATE; }
-  if (!h->launches) { snprintf(h->err, sizeof(h->err), "%s read before the first advance", what); return DCSIM_E_STATE; }
+static int check_stat(dcsim_t* h, int stat) {
+  if (stat >= 0 && stat < DCSIM_STATS) return DCSIM_OK;
+  return set_err(h, DCSIM_E_INVALID, "unknown statistic %s%lld (DCSIM_STAT_*)", "", (long long)stat);
+}
+
+/* A read of recorder `stat` needs it enabled and the batch advanced. */
+static int recorder_ready(dcsim_t* h, int stat) {
+  const char* name = recorder_table[stat].name;
+  if (!h->rec[stat].d[0]) { snprintf(h->err, sizeof(h->err), "%s not enabled (dcsim_recorder_enable)", name); return DCSIM_E_STATE; }
+  if (!h->launches) { snprintf(h->err, sizeof(h->err), "%s read before the first advance", name); return DCSIM_E_STATE; }
   CUDA_TRY(h, cudaSetDevice(h->device));
   return DCSIM_OK;
+}
+
+/* ... then the recorder's own read precondition (the tick counts, the tail selection), on the stream ahead of the read:
+ * what its fetches and its reductions run first. */
+static int recorder_read(dcsim_t* h, int stat) {
+  const int rc = recorder_ready(h, stat);
+  return rc != DCSIM_OK || !recorder_table[stat].ready ? rc : recorder_table[stat].ready(h);
+}
+
+/* The buffers of recorder `stat`, when it is on, filled with their fill bytes on the stream. */
+static int recorder_fill(dcsim_t* h, int stat) {
+  for (int k = 0; k < 2 && h->rec[stat].d[k]; ++k) {
+    const int fill = recorder_table[stat].buf[k].fill;
+    if (fill >= 0) CUDA_TRY(h, cudaMemsetAsync(h->rec[stat].d[k], fill, rec_buf_bytes(h, stat, k), h->g->stream));
+  }
+  return DCSIM_OK;
+}
+
+static void recorder_free(dcsim_t* h, int stat) {
+  cudaFree(h->rec[stat].d[0]);
+  cudaFree(h->rec[stat].d[1]);
+  h->rec[stat] = dcsim_slot{};
 }
 
 /* Column `field` of every replica's summary row into out[0, n_replicas), their maximum into out[n_replicas]. */
@@ -717,11 +784,13 @@ static int summary_counts(dcsim_t* h, int field, uint32_t* out) {
   return DCSIM_OK;
 }
 
-/* Before a reduction over the job ensemble or the power profile (`rec`, checked as by recorder_ready): every replica's
- * status word into d_status, on the stream, where the reduction that reads it follows. */
-static int status_words(dcsim_t* h, const void* rec, const char* what, const char* enable_fn) {
-  const int rc = recorder_ready(h, rec, what, enable_fn);
-  return rc != DCSIM_OK ? rc : summary_counts(h, DCSIM_S_STATUS, h->d_status);
+/* Before a reduction over recorder `stat` (after recorder_read): every replica's status word into d_status, on
+ * the stream, where the reduction that reads it follows.  The cluster ensemble's columns count by the tick counts
+ * instead. */
+static int status_words(dcsim_t* h, int stat) {
+  const int rc = recorder_read(h, stat);
+  if (rc != DCSIM_OK || stat == DCSIM_STAT_CLUSTER_ENSEMBLE) return rc;
+  return summary_counts(h, DCSIM_S_STATUS, h->d_status);
 }
 
 /* Sums the per-replica histogram rows hist[n_replicas][row_len] (without the replicas whose `status` word is not 0, when
@@ -892,7 +961,8 @@ static cudaError_t size_launch(dcsim_t* h) {
  * re-lays the state block out. */
 static int relayout(dcsim_t* h, int job_log) {
   dcsim_layout_t L;
-  dcsim_make_layout(&h->spec, &L, dcsim_job_fields(job_log, h->d_jwait, h->d_tail, h->d_jres));
+  dcsim_make_layout(&h->spec, &L, dcsim_job_fields(job_log, h->rec[DCSIM_STAT_JOB_WAITS].d[0], h->rec[DCSIM_STAT_TAIL_LATENCY].d[0],
+                                                       h->rec[DCSIM_STAT_JOB_RESOURCES].d[0]));
   if (L.lean == h->L.lean) return DCSIM_OK;
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   h->L = L;
@@ -1071,33 +1141,11 @@ int dcsim_reset(dcsim_t* h, uint64_t base_seed, uint64_t first_replica_id) {
   CUDA_TRY(h, cudaMemsetAsync(h->d_state, 0, (size_t)h->n_replicas * (size_t)h->L.total_bytes, h->g->stream));
   CUDA_TRY(h, cudaMemsetAsync(h->d_counts, 0, 4 * sizeof(uint32_t), h->g->stream));
   if (h->d_hist) CUDA_TRY(h, cudaMemsetAsync(h->d_hist, 0, (size_t)h->n_replicas * 2 * DCSIM_LAT_BINS * sizeof(uint32_t), h->g->stream));
-  if (h->d_ens) CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, ens_bytes(h, h->ens_cap), h->g->stream)); /* NaN: not recorded */
-  if (h->d_jens) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, (h->jens_windows + 1) * jens_row_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
+  for (int s = 0; s < DCSIM_STATS; ++s) {
+    const int rc = recorder_fill(h, s);
+    if (rc != DCSIM_OK) return rc;
   }
-  if (h->d_pp) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
-  }
-  if (h->d_occ) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_occ, 0, occ_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_occ_work, 0, occ_work_bytes(h), h->g->stream));
-  }
-  if (h->d_cost) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_cost, 0, cost_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_cost_work, 0, cost_work_bytes(h), h->g->stream));
-  }
-  if (h->d_jwait) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, (h->jens_windows + 1) * jwait_row_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
-  }
-  if (h->d_tail) CUDA_TRY(h, cudaMemsetAsync(h->d_tail, 0xff, tail_slot_bytes(h), h->g->stream)); /* NaN: not finished */
   h->tail_fresh = 0;
-  if (h->d_jres) {
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jres, 0, (h->jens_windows + 1) * jres_row_bytes(h), h->g->stream));
-    CUDA_TRY(h, cudaMemsetAsync(h->d_jres_cnt, 0, jres_cnt_bytes(h), h->g->stream));
-  }
   if (!h->member) { /* new keys: the group's lists are redrawn by its next prepare / advance */
     h->g->seed0 = base_seed + first_replica_id;
     h->g->arrivals_ready = 0;
@@ -1173,15 +1221,19 @@ static void fill_kparams(const dcsim_t* h, dcsim_kparams_t* P, uint64_t max_even
   P->max_transfer = h->g->max_transfer;
   P->lat_hist = h->d_hist;
   P->mt_state = h->g->d_mt;
-  P->ens = h->d_ens; P->ens_cap = h->ens_cap;
-  P->jens = h->d_jens; P->jens_hist = h->d_jens_hist; P->jens_bin = h->jens_bin; P->jens_windows = h->jens_windows;
-  P->tail = h->d_tail; P->tail_cols = h->d_tail_cols; P->tail_sla = h->tail_sla;
-  P->pp = h->d_pp; P->pp_work = h->d_pp_work; P->pp_threshold = h->pp_threshold;
-  P->jwait = h->d_jwait; P->jwait_hist = h->d_jwait_hist;
-  P->occ = h->d_occ; P->occ_work = h->d_occ_work;
-  P->cost = h->d_cost; P->cost_work = h->d_cost_work;
-  P->jres = h->d_jres; P->jres_mix = h->d_jres_cnt;
-  P->jres_hist = h->d_jres ? h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas : NULL;
+  const dcsim_slot* R = h->rec;
+  const dcsim_slot &ens = R[DCSIM_STAT_CLUSTER_ENSEMBLE], &jens = R[DCSIM_STAT_JOB_ENSEMBLE], &jres = R[DCSIM_STAT_JOB_RESOURCES];
+  P->ens = (double*)ens.d[0]; P->ens_cap = (uint32_t)ens.rows;
+  P->jens = (double*)jens.d[0]; P->jens_hist = (uint32_t*)jens.d[1]; P->jens_bin = jens.arg; P->jens_windows = jens.rows ? jens.rows - 1 : 0;
+  P->tail = (double*)R[DCSIM_STAT_TAIL_LATENCY].d[0]; P->tail_cols = (double*)R[DCSIM_STAT_TAIL_LATENCY].d[1];
+  P->tail_sla = R[DCSIM_STAT_TAIL_LATENCY].arg;
+  P->pp = (double*)R[DCSIM_STAT_POWER_PROFILE].d[0]; P->pp_work = (double*)R[DCSIM_STAT_POWER_PROFILE].d[1];
+  P->pp_threshold = R[DCSIM_STAT_POWER_PROFILE].arg;
+  P->jwait = (double*)R[DCSIM_STAT_JOB_WAITS].d[0]; P->jwait_hist = (uint32_t*)R[DCSIM_STAT_JOB_WAITS].d[1];
+  P->occ = (double*)R[DCSIM_STAT_OCCUPANCY].d[0]; P->occ_work = (double*)R[DCSIM_STAT_OCCUPANCY].d[1];
+  P->cost = (double*)R[DCSIM_STAT_ENERGY_COST].d[0]; P->cost_work = (double*)R[DCSIM_STAT_ENERGY_COST].d[1];
+  P->jres = (double*)jres.d[0]; P->jres_mix = (uint32_t*)jres.d[1];
+  P->jres_hist = jres.d[0] ? (uint32_t*)jres.d[1] + jres_mix_cols(h) * h->n_replicas : NULL;
   dcsim_derive_kparams(P);
 }
 
@@ -1421,57 +1473,39 @@ int dcsim_fetch_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
   return DCSIM_OK;
 }
 
-int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks) {
-  if (!h) return DCSIM_E_INVALID;
-  const uint32_t ticks = max_ticks ? max_ticks : dcsim_ens_ticks(&h->spec);
-  if (h->d_ens && h->ens_cap == ticks) return DCSIM_OK;
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_cluster_ensemble must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  if (h->d_ens) { cudaFree(h->d_ens); h->d_ens = NULL; h->ens_cap = 0; }
-  if (!h->d_ens_nlog) CUDA_TRY(h, cudaMalloc(&h->d_ens_nlog, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  const size_t bytes = ens_bytes(h, ticks);
-  const int rc = recorder_alloc(h, (void**)&h->d_ens, bytes ? bytes : sizeof(double), NULL, 0,
-                                "enable_cluster_ensemble: %s%lld bytes of device memory do not fit (run fewer replicas)", (long long)bytes);
-  if (rc != DCSIM_OK) return rc;
-  h->ens_cap = ticks;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_ens, 0xff, bytes, h->g->stream)); /* NaN: not recorded */
-  return DCSIM_OK;
-}
-
-int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out) {
-  if (!h || !ticks_out) return DCSIM_E_INVALID;
-  *ticks_out = h->d_ens ? h->ens_cap : 0u;
-  return DCSIM_OK;
-}
-
-/* Every replica's recorded tick count into d_ens_nlog; fails when one of them went past the capacity (synchronises). */
+extern "C++" {
+/* The cluster ensemble's read precondition: every replica's recorded tick count into d_ens_nlog; fails when one of them
+ * went past the capacity (synchronises). */
 static int ens_counts(dcsim_t* h) {
-  int rc = recorder_ready(h, h->d_ens, "cluster ensemble", "dcsim_enable_cluster_ensemble");
-  if (rc == DCSIM_OK) rc = summary_counts(h, DCSIM_S_EV_LOG, h->d_ens_nlog);
+  const int rc = summary_counts(h, DCSIM_S_EV_LOG, h->d_ens_nlog);
   if (rc != DCSIM_OK) return rc;
   uint32_t most = 0u;
   CUDA_TRY(h, cudaMemcpyAsync(&most, h->d_ens_nlog + h->n_replicas, sizeof(most), cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  if (most > h->ens_cap) {
-    snprintf(h->err, sizeof(h->err), "cluster ensemble overflow: a replica recorded %u log ticks, capacity %u", most, h->ens_cap);
+  const uint32_t cap = (uint32_t)h->rec[DCSIM_STAT_CLUSTER_ENSEMBLE].rows;
+  if (most > cap) {
+    snprintf(h->err, sizeof(h->err), "cluster ensemble overflow: a replica recorded %u log ticks, capacity %u", most, cap);
     return DCSIM_E_STATE;
   }
   return DCSIM_OK;
 }
 
-int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes) {
-  if (!h || !out) return DCSIM_E_INVALID;
-  const int rc = ens_counts(h);
-  if (rc != DCSIM_OK) return rc;
-  const size_t tick_bytes = ens_bytes(h, 1);
-  size_t ticks = out_bytes / tick_bytes;
-  if (ticks > h->ens_cap) ticks = h->ens_cap;
-  if (ticks) {
-    CUDA_TRY(h, cudaMemcpyAsync(out, h->d_ens, ticks * tick_bytes, cudaMemcpyDeviceToHost, h->g->stream));
-    CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  }
+/* The tail recorder's read precondition: the columns of the finished batch, selected once per batch on the stream. */
+static int tail_ready(dcsim_t* h) {
+  if (h->tail_fresh) return DCSIM_OK;
+  int done = 0, rc;
+  if ((rc = dcsim_all_done(h, &done)) != DCSIM_OK) return rc;
+  if (!done) return set_err(h, DCSIM_E_STATE, "tail latency read while replicas are still running (advance to the end first)%s%lld");
+  dcsim_kparams_t P;
+  fill_kparams(h, &P, 0);
+  const uint64_t per_sm = 8; /* 256 threads and 18 KB each: 8 CTAs fit an SM */
+  const uint64_t grid = h->n_replicas < per_sm * (uint64_t)h->sm_count ? h->n_replicas : per_sm * (uint64_t)h->sm_count;
+  dcsim_tail_select_kernel<<<(int)grid, DCSIM_TAIL_THREADS, 0, h->g->stream>>>(P);
+  CUDA_TRY(h, cudaGetLastError());
+  h->tail_fresh = 1;
   return DCSIM_OK;
 }
+} /* extern "C++" */
 
 static int pair_check(dcsim_t* base, const double* dev_variant_summary, uint64_t n) {
   if (!base || !dev_variant_summary) return DCSIM_E_INVALID;
@@ -1501,160 +1535,155 @@ int dcsim_paired_spread(dcsim_t* base, const double* dev_variant_summary, uint64
   return ens_spread(base, src, n, pair_cols(base), dev_mean, dev_lo, dev_hi, dev_m2_out, dev_hist_out);
 }
 
-int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s) {
+extern "C++" {
+static int enable_err(dcsim_t* h, int code, int stat, const char* a, const char* b = "") {
+  snprintf(h->err, sizeof(h->err), "enable %s: %s%s", recorder_table[stat].name, a, b);
+  return code;
+}
+
+/* The histogram scratch of recorder `stat` (NULL: it has no histogram), and the length of one replica's row of the
+ * per-replica histograms, its second buffer [n_replicas][row_len] u32. */
+static unsigned long long** hist_scratch(dcsim_t* h, int stat) {
+  return stat == DCSIM_STAT_JOB_ENSEMBLE ? &h->d_jens_hist_out : (stat == DCSIM_STAT_JOB_WAITS ? &h->d_jwait_hist_out : NULL);
+}
+static uint32_t hist_row_len(const dcsim_t* h, int stat) {
+  return (uint32_t)(recorder_table[stat].buf[1].bytes(h) / ((size_t)h->n_replicas * sizeof(uint32_t)));
+}
+
+/* The buffers of recorder `stat` for its rows, all or none.  Running out of device memory is DCSIM_E_NOMEM with `need`
+ * bytes in the message, and clears the sticky error: the handle stays usable. */
+static int recorder_alloc(dcsim_t* h, int stat, long long need) {
+  const rec_desc& R = recorder_table[stat];
+  dcsim_slot& S = h->rec[stat];
+  cudaError_t e = cudaSuccess;
+  for (int k = 0; k < 2 && R.buf[k].bytes; ++k) {
+    const size_t bytes = rec_buf_bytes(h, stat, k);
+    e = cudaMalloc(&S.d[k], bytes ? bytes : sizeof(double)); /* a cluster ensemble of no tick is on all the same */
+    if (e != cudaSuccess) { S.d[k] = NULL; break; }
+  }
+  if (e == cudaSuccess) return DCSIM_OK;
+  recorder_free(h, stat);
+  if (e != cudaErrorMemoryAllocation) return set_err(h, DCSIM_E_CUDA, "CUDA error: %s%lld", cudaGetErrorString(e));
+  cudaGetLastError();
+  snprintf(h->err, sizeof(h->err), "enable %s: %lld bytes of device memory do not fit (%s)", R.name, need, R.nomem_hint);
+  return DCSIM_E_NOMEM;
+}
+
+/* Bytes of part `part` of recorder `stat`'s fetch, and where in its buffer it starts. */
+static size_t part_bytes(const dcsim_t* h, int stat, int part) {
+  const rec_part& p = recorder_table[stat].part[part];
+  return p.bytes ? p.bytes(h) : rec_buf_bytes(h, stat, p.buf);
+}
+static size_t part_offset(const dcsim_t* h, int stat, int part) {
+  size_t off = 0;
+  for (int q = 0; q < part; ++q)
+    if (recorder_table[stat].part[q].buf == recorder_table[stat].part[part].buf) off += part_bytes(h, stat, q);
+  return off;
+}
+} /* extern "C++" */
+
+int dcsim_recorder_enable(dcsim_t* h, int stat, double arg) {
   if (!h) return DCSIM_E_INVALID;
-  if (!(bin_s >= 0.0 && bin_s <= DBL_MAX)) return set_err(h, DCSIM_E_INVALID, "enable_job_ensemble: bin_s must be finite and >= 0%s%lld");
-  const double bin = bin_s > 0.0 ? bin_s : h->spec.log_interval;
-  if (h->d_jens && h->jens_bin == bin) return DCSIM_OK;
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_ensemble must precede the first advance%s%lld");
+  int rc = check_stat(h, stat);
+  if (rc != DCSIM_OK) return rc;
+  const rec_desc& R = recorder_table[stat];
+  dcsim_slot& S = h->rec[stat];
+  double val = 0.0; /* the resolved argument */
+  uint64_t rows = 1;
+  switch (R.arg) {
+    case ARG_TICKS:
+      if (!(arg >= 0.0 && arg <= 4294967295.0 && arg == floor(arg)))
+        return enable_err(h, DCSIM_E_INVALID, stat, R.arg_name, " must be a whole number in [0, 2^32)");
+      rows = arg > 0.0 ? (uint64_t)arg : dcsim_ens_ticks(&h->spec);
+      break;
+    case ARG_BIN:
+      if (!(arg >= 0.0 && arg <= DBL_MAX)) return enable_err(h, DCSIM_E_INVALID, stat, R.arg_name, " must be finite and >= 0");
+      val = arg > 0.0 ? arg : h->spec.log_interval;
+      rows = dcsim_jens_windows(h->spec.end_time, val) + 1;
+      break;
+    case ARG_LIMIT:
+      if (!(arg >= 0.0)) return enable_err(h, DCSIM_E_INVALID, stat, R.arg_name, " must be >= 0 (+inf: none)");
+      val = arg;
+      break;
+  }
+  if (R.needs_jens) {
+    if (!h->rec[DCSIM_STAT_JOB_ENSEMBLE].d[0]) return enable_err(h, DCSIM_E_STATE, stat, "needs the job ensemble (enable it first)");
+    rows = h->rec[DCSIM_STAT_JOB_ENSEMBLE].rows;
+  }
+  if (h->member && !R.member_ok) return enable_err(h, DCSIM_E_STATE, stat, "not on a member of a shared group");
+  if (R.retarget && S.d[0] && S.rows == rows && S.arg == val) return DCSIM_OK;
+  if (h->launches) return enable_err(h, DCSIM_E_STATE, stat, "must precede the first advance");
   CUDA_TRY(h, cudaSetDevice(h->device));
-  cudaFree(h->d_jens); cudaFree(h->d_jens_hist);
-  h->d_jens = NULL; h->d_jens_hist = NULL; h->jens_windows = 0; h->jens_bin = 0.0;
-  cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); /* sized by the windows: re-enabled after the job ensemble */
-  h->d_jwait = NULL; h->d_jwait_hist = NULL;
-  cudaFree(h->d_jres); cudaFree(h->d_jres_cnt); /* likewise */
-  h->d_jres = NULL; h->d_jres_cnt = NULL;
-  const uint64_t windows = dcsim_jens_windows(h->spec.end_time, bin);
-  const double need = ((double)windows + 1.0) * (double)jens_row_bytes(h) + (double)jens_hist_bytes(h);
-  const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
-  const char* nomem = "enable_job_ensemble: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)";
-  if (windows >= 0xffffffffull || need >= 9.0e18) return set_err(h, DCSIM_E_NOMEM, nomem, "", need_ll);
-  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  if (!h->d_jens_hist_out) CUDA_TRY(h, cudaMalloc(&h->d_jens_hist_out, (size_t)h->spec.n_dc * 2 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
-  const size_t rows_bytes = (windows + 1) * jens_row_bytes(h);
-  const int rc = recorder_alloc(h, (void**)&h->d_jens, rows_bytes, (void**)&h->d_jens_hist, jens_hist_bytes(h), nomem, need_ll);
-  if (rc != DCSIM_OK) return rc;
-  h->jens_bin = bin; h->jens_windows = windows;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens, 0, rows_bytes, h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jens_hist, 0, jens_hist_bytes(h), h->g->stream));
-  return DCSIM_OK;
+  if (R.retarget) { /* other rows: new buffers, and none for the recorders that live in the job ensemble's rows */
+    recorder_free(h, stat);
+    for (int s = 0; s < DCSIM_STATS; ++s)
+      if (stat == DCSIM_STAT_JOB_ENSEMBLE && recorder_table[s].needs_jens) recorder_free(h, s);
+  }
+  if (!S.d[0]) {
+    double need = 0.0; /* in double: a narrow bin_s asks for more than size_t holds */
+    for (int k = 0; k < 2 && R.buf[k].bytes; ++k) need += (R.buf[k].per_row ? (double)rows : 1.0) * (double)R.buf[k].bytes(h);
+    const long long need_ll = need < 9.0e18 ? (long long)need : 9000000000000000000ll;
+    if (rows > 0xffffffffull || need >= 9.0e18) { /* W capped by dcsim_jens_windows, or past any device */
+      snprintf(h->err, sizeof(h->err), "enable %s: %lld bytes of device memory do not fit (%s)", R.name, need_ll, R.nomem_hint);
+      return DCSIM_E_NOMEM;
+    }
+    uint32_t** words = stat == DCSIM_STAT_CLUSTER_ENSEMBLE ? &h->d_ens_nlog : &h->d_status;
+    if (!*words) CUDA_TRY(h, cudaMalloc(words, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
+    unsigned long long** hist = hist_scratch(h, stat);
+    if (hist && !*hist) CUDA_TRY(h, cudaMalloc(hist, (size_t)hist_row_len(h, stat) * sizeof(unsigned long long)));
+    S.rows = rows;
+    if ((rc = recorder_alloc(h, stat, need_ll)) != DCSIM_OK) return rc;
+  }
+  S.arg = val;
+  return recorder_fill(h, stat);
 }
 
-int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out) {
-  if (!h || !windows_out) return DCSIM_E_INVALID;
-  *windows_out = h->d_jens ? (uint32_t)h->jens_windows : 0u;
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes) {
-  if (!h) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
-  if (rc != DCSIM_OK) return rc;
-  const size_t need_rows = (h->jens_windows + 1) * jens_row_bytes(h), need_hist = jens_hist_bytes(h);
-  if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
-    return set_err(h, DCSIM_E_INVALID, "fetch_job_ensemble: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
-  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jens, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
-  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jens_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
+int dcsim_recorder_state(dcsim_t* h, int stat, dcsim_recorder_state_t* out) {
   if (!h || !out) return DCSIM_E_INVALID;
-  const uint32_t row_len = 2u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
-  const size_t need = (size_t)row_len * sizeof(uint64_t);
-  if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_latency_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
-  const int rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble");
+  const int rc = check_stat(h, stat);
   if (rc != DCSIM_OK) return rc;
-  CUDA_TRY(h, hist_reduce(h, h->d_jens_hist, row_len, h->d_status, h->d_jens_hist_out, out));
+  const dcsim_slot& S = h->rec[stat];
+  memset(out, 0, sizeof(*out));
+  out->on = S.d[0] != NULL;
+  out->parts = recorder_table[stat].parts;
+  out->arg = S.arg;
+  out->rows = S.rows;
+  for (int p = 0; out->on && p < out->parts; ++p) out->part_bytes[p] = part_bytes(h, stat, p);
   return DCSIM_OK;
 }
 
-int dcsim_enable_job_waits(dcsim_t* h) {
-  if (!h) return DCSIM_E_INVALID;
-  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "enable_job_waits needs the job ensemble (dcsim_enable_job_ensemble first)%s%lld");
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_job_waits on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_waits must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  const size_t rows_bytes = (h->jens_windows + 1) * jwait_row_bytes(h);
-  if (!h->d_jwait) {
-    if (!h->d_jwait_hist_out) CUDA_TRY(h, cudaMalloc(&h->d_jwait_hist_out, (size_t)h->spec.n_dc * 4 * DCSIM_LAT_BINS * sizeof(unsigned long long)));
-    const int rc = recorder_alloc(h, (void**)&h->d_jwait, rows_bytes, (void**)&h->d_jwait_hist, jwait_hist_bytes(h),
-                                  "enable_job_waits: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)",
-                                  (long long)(rows_bytes + jwait_hist_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
-  }
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jwait, 0, rows_bytes, h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jwait_hist, 0, jwait_hist_bytes(h), h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes) {
-  if (!h) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
-  if (rc != DCSIM_OK) return rc;
-  const size_t need_rows = (h->jens_windows + 1) * jwait_row_bytes(h), need_hist = jwait_hist_bytes(h);
-  if ((rows && rows_bytes < need_rows) || (hist && hist_bytes < need_hist))
-    return set_err(h, DCSIM_E_INVALID, "fetch_job_waits: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
-  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jwait, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
-  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jwait_hist, need_hist, cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes) {
+int dcsim_recorder_fetch(dcsim_t* h, int stat, int part, void* out, size_t out_bytes) {
   if (!h || !out) return DCSIM_E_INVALID;
-  const uint32_t row_len = 4u * (uint32_t)h->spec.n_dc * DCSIM_LAT_BINS;
-  const size_t need = (size_t)row_len * sizeof(uint64_t);
-  if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "fetch_dc_wait_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
-  const int rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits");
+  int rc = check_stat(h, stat);
   if (rc != DCSIM_OK) return rc;
-  CUDA_TRY(h, hist_reduce(h, h->d_jwait_hist, row_len, h->d_status, h->d_jwait_hist_out, out));
-  return DCSIM_OK;
-}
-
-int dcsim_enable_job_resources(dcsim_t* h) {
-  if (!h) return DCSIM_E_INVALID;
-  if (!h->d_jens) return set_err(h, DCSIM_E_STATE, "enable_job_resources needs the job ensemble (dcsim_enable_job_ensemble first)%s%lld");
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_job_resources on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_job_resources must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  const size_t rows_bytes = (h->jens_windows + 1) * jres_row_bytes(h);
-  if (!h->d_jres) {
-    const int rc = recorder_alloc(h, (void**)&h->d_jres, rows_bytes, (void**)&h->d_jres_cnt, jres_cnt_bytes(h),
-                                  "enable_job_resources: %s%lld bytes of device memory do not fit (a wider bin_s or fewer replicas)",
-                                  (long long)(rows_bytes + jres_cnt_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
+  if (part < 0 || part >= recorder_table[stat].parts)
+    return set_err(h, DCSIM_E_INVALID, "recorder_fetch: no part %s%lld of this recorder", "", (long long)part);
+  if ((rc = recorder_read(h, stat)) != DCSIM_OK) return rc;
+  size_t bytes = part_bytes(h, stat, part);
+  if (stat == DCSIM_STAT_CLUSTER_ENSEMBLE) { /* the whole ticks that fit, at most the capacity */
+    const uint64_t tick = ens_tick_bytes(h), ticks = out_bytes / tick;
+    bytes = (size_t)((ticks < h->rec[stat].rows ? ticks : h->rec[stat].rows) * tick);
+  } else if (out_bytes < bytes) {
+    return set_err(h, DCSIM_E_INVALID, "recorder_fetch: buffer too small (need %s%lld bytes)", "", (long long)bytes);
   }
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jres, 0, rows_bytes, h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_jres_cnt, 0, jres_cnt_bytes(h), h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* mix, size_t mix_bytes, uint32_t* hist,
-                              size_t hist_bytes) {
-  if (!h) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_jres, "job resources", "dcsim_enable_job_resources");
-  if (rc != DCSIM_OK) return rc;
-  const size_t need_rows = (h->jens_windows + 1) * jres_row_bytes(h);
-  const size_t need_mix = (size_t)jres_mix_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t);
-  const size_t need_hist = (size_t)jres_hist_cols(h) * (size_t)h->n_replicas * sizeof(uint32_t);
-  if ((rows && rows_bytes < need_rows) || (mix && mix_bytes < need_mix) || (hist && hist_bytes < need_hist))
-    return set_err(h, DCSIM_E_INVALID, "fetch_job_resources: buffer too small (rows need %s%lld bytes)", "", (long long)need_rows);
-  if (rows) CUDA_TRY(h, cudaMemcpyAsync(rows, h->d_jres, need_rows, cudaMemcpyDeviceToHost, h->g->stream));
-  if (mix) CUDA_TRY(h, cudaMemcpyAsync(mix, h->d_jres_cnt, need_mix, cudaMemcpyDeviceToHost, h->g->stream));
-  if (hist) CUDA_TRY(h, cudaMemcpyAsync(hist, h->d_jres_cnt + jres_mix_cols(h) * h->n_replicas, need_hist,
-                                        cudaMemcpyDeviceToHost, h->g->stream));
+  if (!bytes) return DCSIM_OK;
+  const char* src = (const char*)h->rec[stat].d[recorder_table[stat].part[part].buf] + part_offset(h, stat, part);
+  CUDA_TRY(h, cudaMemcpyAsync(out, src, bytes, cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
   return DCSIM_OK;
 }
 
-int dcsim_enable_power_profile(dcsim_t* h, double threshold_w) {
-  if (!h) return DCSIM_E_INVALID;
-  if (!(threshold_w >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_power_profile: the threshold must be >= 0 (+inf: none)%s%lld");
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_power_profile on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_power_profile must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  if (!h->d_pp) {
-    const int rc = recorder_alloc(h, (void**)&h->d_pp, pp_bytes(h), (void**)&h->d_pp_work, pp_work_bytes(h),
-                                  "enable_power_profile: %s%lld bytes of device memory do not fit (run fewer replicas)",
-                                  (long long)(pp_bytes(h) + pp_work_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
-  }
-  h->pp_threshold = threshold_w;
-  CUDA_TRY(h, cudaMemsetAsync(h->d_pp, 0, pp_bytes(h), h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_pp_work, 0, pp_work_bytes(h), h->g->stream));
+int dcsim_recorder_histogram(dcsim_t* h, int stat, uint64_t* out, size_t out_bytes) {
+  if (!h || !out) return DCSIM_E_INVALID;
+  int rc = check_stat(h, stat);
+  if (rc != DCSIM_OK) return rc;
+  unsigned long long** sum = hist_scratch(h, stat);
+  if (!sum) return set_err(h, DCSIM_E_INVALID, "recorder_histogram: statistic %s%lld has no histogram", "", (long long)stat);
+  const uint32_t row_len = hist_row_len(h, stat);
+  const size_t need = (size_t)row_len * sizeof(uint64_t);
+  if (out_bytes < need) return set_err(h, DCSIM_E_INVALID, "recorder_histogram: buffer too small (need %s%lld bytes)", "", (long long)need);
+  if ((rc = status_words(h, stat)) != DCSIM_OK) return rc;
+  CUDA_TRY(h, hist_reduce(h, (const uint32_t*)h->rec[stat].d[1], row_len, h->d_status, *sum, out));
   return DCSIM_OK;
 }
 
@@ -1664,120 +1693,18 @@ int dcsim_power_profile_range(dcsim_t* h, double* hi_out) {
   return DCSIM_OK;
 }
 
-int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes) {
-  if (!h || !out) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_pp, "power profile", "dcsim_enable_power_profile");
-  if (rc != DCSIM_OK) return rc;
-  if (out_bytes < pp_bytes(h))
-    return set_err(h, DCSIM_E_INVALID, "fetch_power_profile: buffer too small (need %s%lld bytes)", "", (long long)pp_bytes(h));
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_pp, pp_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_enable_energy_cost(dcsim_t* h) {
-  if (!h) return DCSIM_E_INVALID;
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_energy_cost on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_energy_cost must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  if (!h->d_cost) {
-    const int rc = recorder_alloc(h, (void**)&h->d_cost, cost_bytes(h), (void**)&h->d_cost_work, cost_work_bytes(h),
-                                  "enable_energy_cost: %s%lld bytes of device memory do not fit (run fewer replicas)",
-                                  (long long)(cost_bytes(h) + cost_work_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
-  }
-  CUDA_TRY(h, cudaMemsetAsync(h->d_cost, 0, cost_bytes(h), h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_cost_work, 0, cost_work_bytes(h), h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes) {
-  if (!h || !out) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost");
-  if (rc != DCSIM_OK) return rc;
-  if (out_bytes < cost_bytes(h))
-    return set_err(h, DCSIM_E_INVALID, "fetch_energy_cost: buffer too small (need %s%lld bytes)", "", (long long)cost_bytes(h));
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_cost, cost_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_enable_tail_latency(dcsim_t* h, double sla_s) {
-  if (!h) return DCSIM_E_INVALID;
-  if (!(sla_s >= 0.0)) return set_err(h, DCSIM_E_INVALID, "enable_tail_latency: sla_s must be >= 0 (+inf: none)%s%lld");
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_tail_latency on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_tail_latency must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  if (!h->d_tail) {
-    const int rc = recorder_alloc(h, (void**)&h->d_tail, tail_slot_bytes(h), (void**)&h->d_tail_cols, tail_cols_bytes(h),
-                                  "enable_tail_latency: %s%lld bytes of device memory do not fit (run fewer replicas)",
-                                  (long long)(tail_slot_bytes(h) + tail_cols_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
-  }
-  CUDA_TRY(h, cudaMemsetAsync(h->d_tail, 0xff, tail_slot_bytes(h), h->g->stream)); /* NaN: not finished */
-  h->tail_sla = sla_s;
-  h->tail_fresh = 0;
-  return DCSIM_OK;
-}
-
-/* The tail columns of the finished batch, selected once per batch on the stream (see dcsim_fetch_tail_latency). */
-static int tail_ready(dcsim_t* h) {
-  int rc = recorder_ready(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
-  if (rc != DCSIM_OK || h->tail_fresh) return rc;
-  int done = 0;
-  if ((rc = dcsim_all_done(h, &done)) != DCSIM_OK) return rc;
-  if (!done) return set_err(h, DCSIM_E_STATE, "tail latency read while replicas are still running (advance to the end first)%s%lld");
-  dcsim_kparams_t P;
-  fill_kparams(h, &P, 0);
-  const uint64_t per_sm = 8; /* 256 threads and 18 KB each: 8 CTAs fit an SM */
-  const uint64_t grid = h->n_replicas < per_sm * (uint64_t)h->sm_count ? h->n_replicas : per_sm * (uint64_t)h->sm_count;
-  dcsim_tail_select_kernel<<<(int)grid, DCSIM_TAIL_THREADS, 0, h->g->stream>>>(P);
-  CUDA_TRY(h, cudaGetLastError());
-  h->tail_fresh = 1;
-  return DCSIM_OK;
-}
-
-int dcsim_fetch_tail_latency(dcsim_t* h, double* out, size_t out_bytes) {
-  if (!h || !out) return DCSIM_E_INVALID;
-  if (out_bytes < tail_cols_bytes(h))
-    return set_err(h, DCSIM_E_INVALID, "fetch_tail_latency: buffer too small (need %s%lld bytes)", "", (long long)tail_cols_bytes(h));
-  const int rc = tail_ready(h);
-  if (rc != DCSIM_OK) return rc;
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_tail_cols, tail_cols_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
 int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* out, size_t out_bytes) {
   if (!h || !out) return DCSIM_E_INVALID;
   if (first > h->n_replicas || count > h->n_replicas - first)
     return set_err(h, DCSIM_E_INVALID, "fetch_tail_jobs: replicas [first, first + count) out of range%s%lld");
-  const int rc = recorder_ready(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency");
+  const int rc = recorder_ready(h, DCSIM_STAT_TAIL_LATENCY);
   if (rc != DCSIM_OK) return rc;
   const size_t per = (size_t)h->g->cap_arr * 2, need = (size_t)count * per * sizeof(double);
   if (out_bytes < need)
     return set_err(h, DCSIM_E_INVALID, "fetch_tail_jobs: buffer too small (need %s%lld bytes)", "", (long long)need);
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_tail + (size_t)first * per, need, cudaMemcpyDeviceToHost, h->g->stream));
+  CUDA_TRY(h, cudaMemcpyAsync(out, (const double*)h->rec[DCSIM_STAT_TAIL_LATENCY].d[0] + (size_t)first * per, need,
+                              cudaMemcpyDeviceToHost, h->g->stream));
   CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
-int dcsim_enable_occupancy(dcsim_t* h) {
-  if (!h) return DCSIM_E_INVALID;
-  if (h->member) return set_err(h, DCSIM_E_STATE, "enable_occupancy on a member of a shared group%s%lld");
-  if (h->launches) return set_err(h, DCSIM_E_STATE, "enable_occupancy must precede the first advance%s%lld");
-  CUDA_TRY(h, cudaSetDevice(h->device));
-  if (!h->d_status) CUDA_TRY(h, cudaMalloc(&h->d_status, ((size_t)h->n_replicas + 1) * sizeof(uint32_t)));
-  if (!h->d_occ) {
-    const int rc = recorder_alloc(h, (void**)&h->d_occ, occ_bytes(h), (void**)&h->d_occ_work, occ_work_bytes(h),
-                                  "enable_occupancy: %s%lld bytes of device memory do not fit (run fewer replicas)",
-                                  (long long)(occ_bytes(h) + occ_work_bytes(h)));
-    if (rc != DCSIM_OK) return rc;
-  }
-  CUDA_TRY(h, cudaMemsetAsync(h->d_occ, 0, occ_bytes(h), h->g->stream));
-  CUDA_TRY(h, cudaMemsetAsync(h->d_occ_work, 0, occ_work_bytes(h), h->g->stream));
   return DCSIM_OK;
 }
 
@@ -1787,70 +1714,52 @@ int dcsim_occupancy_bin_widths(dcsim_t* h, int32_t* w_out) {
   return DCSIM_OK;
 }
 
-int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes) {
-  if (!h || !out) return DCSIM_E_INVALID;
-  const int rc = recorder_ready(h, h->d_occ, "occupancy", "dcsim_enable_occupancy");
-  if (rc != DCSIM_OK) return rc;
-  if (out_bytes < occ_bytes(h))
-    return set_err(h, DCSIM_E_INVALID, "fetch_occupancy: buffer too small (need %s%lld bytes)", "", (long long)occ_bytes(h));
-  CUDA_TRY(h, cudaMemcpyAsync(out, h->d_occ, occ_bytes(h), cudaMemcpyDeviceToHost, h->g->stream));
-  CUDA_TRY(h, cudaStreamSynchronize(h->g->stream));
-  return DCSIM_OK;
-}
-
 extern "C++" {
 /* The batch recorder `stat` (DCSIM_STAT_*) as the two passes see it: f(src, columns, spread_columns) with its column
- * source and column counts for the handle's current state.  With `ready`, the recorder's precondition runs first: it
- * fails when the recorder is off or the batch has not advanced, and queues what the source reads (the tick counts, the
- * status words, the tail selection) on the stream ahead of the pass.  Without it this is host arithmetic only. */
+ * source and column counts for the handle's current state.  With `ready`, status_words runs first: it fails when the
+ * recorder is off or the batch has not advanced, and queues what the source reads (the tick counts, the status words,
+ * the tail selection) on the stream ahead of the pass.  Without it this is host arithmetic only. */
 template <class F>
 static int with_stat(dcsim_t* h, int stat, bool ready, F&& f) {
+  int rc = check_stat(h, stat);
+  if (rc != DCSIM_OK || (ready && (rc = status_words(h, stat)) != DCSIM_OK)) return rc;
   const int n_dc = h->spec.n_dc;
   const uint32_t cells = 2u * (uint32_t)n_dc;
-  const uint64_t rows = (h->d_jens ? h->jens_windows : 0) + 1; /* the job ensemble's windows, then the whole run */
-  int rc = DCSIM_OK;
+  const dcsim_slot* R = h->rec;
+  const double* jens = (const double*)R[DCSIM_STAT_JOB_ENSEMBLE].d[0];
+  const uint64_t rows = jens ? R[DCSIM_STAT_JOB_ENSEMBLE].rows : 1; /* the job ensemble's windows, then the whole run */
+  const dcsim_slot& S = R[stat];
   switch (stat) {
     case DCSIM_STAT_CLUSTER_ENSEMBLE: {
-      if (ready && (rc = ens_counts(h)) != DCSIM_OK) return rc;
       const uint32_t cols_per_tick = DCSIM_ENS_FIELDS * (uint32_t)n_dc;
-      const uint64_t cols = (uint64_t)(h->d_ens ? h->ens_cap : 0u) * cols_per_tick;
-      return f(dcsim_ens_cluster_src{h->d_ens, h->d_ens_nlog, h->n_replicas, cols_per_tick, n_dc}, cols, cols);
+      const uint64_t cols = S.rows * cols_per_tick;
+      return f(dcsim_ens_cluster_src{(const double*)S.d[0], h->d_ens_nlog, h->n_replicas, cols_per_tick, n_dc}, cols, cols);
     }
     case DCSIM_STAT_JOB_ENSEMBLE: {
-      if (ready && (rc = status_words(h, h->d_jens, "job ensemble", "dcsim_enable_job_ensemble")) != DCSIM_OK) return rc;
       const uint64_t cols = rows * DCSIM_JENS_FIELDS * cells;
-      return f(dcsim_ens_job_src{h->d_jens, h->d_status, h->n_replicas, cells}, cols, cols);
+      return f(dcsim_ens_job_src{jens, h->d_status, h->n_replicas, cells}, cols, cols);
     }
     case DCSIM_STAT_POWER_PROFILE:
-      if (ready && (rc = status_words(h, h->d_pp, "power profile", "dcsim_enable_power_profile")) != DCSIM_OK) return rc;
-      return f(dcsim_ens_pp_src{h->d_pp, h->d_status, h->n_replicas}, pp_cols(h), (uint64_t)(DCSIM_PP_FIELDS + n_dc));
+      return f(dcsim_ens_pp_src{(const double*)S.d[0], h->d_status, h->n_replicas}, pp_cols(h), (uint64_t)(DCSIM_PP_FIELDS + n_dc));
     case DCSIM_STAT_JOB_WAITS: {
-      if (ready && (rc = status_words(h, h->d_jwait, "job waits", "dcsim_enable_job_waits")) != DCSIM_OK) return rc;
       const uint64_t cols = rows * DCSIM_JWAIT_FIELDS * cells;
-      return f(dcsim_ens_wait_src{h->d_jwait, h->d_jens, h->d_status, h->n_replicas, cells}, cols, cols);
+      return f(dcsim_ens_wait_src{(const double*)S.d[0], jens, h->d_status, h->n_replicas, cells}, cols, cols);
     }
     case DCSIM_STAT_OCCUPANCY:
-      if (ready && (rc = status_words(h, h->d_occ, "occupancy", "dcsim_enable_occupancy")) != DCSIM_OK) return rc;
-      return f(dcsim_ens_occ_src{h->d_occ, h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)n_dc},
+      return f(dcsim_ens_occ_src{(const double*)S.d[0], h->d_status, h->n_replicas, (uint32_t)occ_stat_cols(h), (uint32_t)n_dc},
                occ_cols(h), occ_stat_cols(h));
     case DCSIM_STAT_TAIL_LATENCY: {
-      if (ready && ((rc = tail_ready(h)) != DCSIM_OK ||
-                    (rc = status_words(h, h->d_tail, "tail latency", "dcsim_enable_tail_latency")) != DCSIM_OK)) return rc;
       const uint32_t group_cols = 2u * (uint32_t)(n_dc + 1) * DCSIM_TAIL_GROUP_FIELDS;
       const uint64_t cols = DCSIM_TAIL_COLS(n_dc);
-      return f(dcsim_ens_tail_src{h->d_tail_cols, h->d_status, h->n_replicas, group_cols}, cols, cols);
+      return f(dcsim_ens_tail_src{(const double*)S.d[1], h->d_status, h->n_replicas, group_cols}, cols, cols);
     }
     case DCSIM_STAT_JOB_RESOURCES: {
-      if (ready && (rc = status_words(h, h->d_jres, "job resources", "dcsim_enable_job_resources")) != DCSIM_OK) return rc;
       const uint64_t win_cols = rows * DCSIM_JRES_FIELDS * cells; /* the counts after them need no spread */
-      return f(dcsim_ens_res_src{h->d_jres, h->d_jens, h->d_jres_cnt, h->d_status, h->n_replicas, cells, win_cols},
+      return f(dcsim_ens_res_src{(const double*)S.d[0], jens, (const uint32_t*)S.d[1], h->d_status, h->n_replicas, cells, win_cols},
                win_cols + jres_mix_cols(h) + jres_hist_cols(h), win_cols);
     }
-    case DCSIM_STAT_ENERGY_COST:
-      if (ready && (rc = status_words(h, h->d_cost, "energy cost", "dcsim_enable_energy_cost")) != DCSIM_OK) return rc;
-      return f(dcsim_ens_cost_src{h->d_cost, h->d_status, h->n_replicas}, cost_cols(h), cost_cols(h));
-    default:
-      return set_err(h, DCSIM_E_INVALID, "unknown statistic %s%lld (DCSIM_STAT_*)", "", (long long)stat);
+    default: /* DCSIM_STAT_ENERGY_COST */
+      return f(dcsim_ens_cost_src{(const double*)S.d[0], h->d_status, h->n_replicas}, cost_cols(h), cost_cols(h));
   }
 }
 } /* extern "C++" */
@@ -1946,14 +1855,8 @@ void dcsim_destroy(dcsim_t* h) {
   cudaFree(h->d_trace); cudaFree(h->d_jobs); cudaFree(h->d_cluster);
   cudaFree(h->d_hist); cudaFree(h->d_agg); cudaFree(h->d_hist_out);
   if (h->h_summary_pinned) cudaFreeHost(h->h_summary_pinned);
-  cudaFree(h->d_ens); cudaFree(h->d_ens_nlog);
-  cudaFree(h->d_jens); cudaFree(h->d_jens_hist); cudaFree(h->d_jens_hist_out);
-  cudaFree(h->d_pp); cudaFree(h->d_pp_work); cudaFree(h->d_status);
-  cudaFree(h->d_occ); cudaFree(h->d_occ_work);
-  cudaFree(h->d_cost); cudaFree(h->d_cost_work);
-  cudaFree(h->d_tail); cudaFree(h->d_tail_cols);
-  cudaFree(h->d_jwait); cudaFree(h->d_jwait_hist); cudaFree(h->d_jwait_hist_out);
-  cudaFree(h->d_jres); cudaFree(h->d_jres_cnt);
+  for (int s = 0; s < DCSIM_STATS; ++s) recorder_free(h, s);
+  cudaFree(h->d_ens_nlog); cudaFree(h->d_jens_hist_out); cudaFree(h->d_jwait_hist_out); cudaFree(h->d_status);
   group_release(h->g); /* the arrival lists and the stream go with the group's last handle */
   delete h;
 }

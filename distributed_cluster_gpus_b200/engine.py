@@ -1,5 +1,6 @@
 """BatchedEngine — thin owner of one ``dcsim_t`` handle (one CUDA device, one stream, R replicas)."""
 import ctypes as C
+import math
 import os
 
 import numpy as np
@@ -103,8 +104,6 @@ class BatchedEngine:
         if cuda_stream:
             self.set_stream(cuda_stream)
         self._trace_cap = self._jobs_cap = self._cluster_cap = 0
-        self._ens_cap, self._ens_on = 0, False
-        self._jens_windows, self._jens_bin = 0, None
 
     @classmethod
     def shared(cls, spec: S.Spec, owner: "BatchedEngine") -> "BatchedEngine":
@@ -201,106 +200,121 @@ class BatchedEngine:
         N.check(self._lib.dcsim_fetch_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
         return out
 
+    # -- the batch recorders (RECORDERS; ensemble.py turns each one into batch statistics) ---------------------------
+    # The library holds each recorder's state (include/dcsim_b200.h, dcsim_recorder_*): these helpers read it there.
+    def _enable(self, name: str, arg=0.0):
+        N.check(self._lib.dcsim_recorder_enable(self._h, RECORDERS.index(name), float(arg)), self._h)
+
+    def _state(self, name: str) -> S.RecorderState:
+        st = S.RecorderState()
+        N.check(self._lib.dcsim_recorder_state(self._h, RECORDERS.index(name), C.byref(st)), self._h)
+        return st
+
+    def _fetch(self, name: str, part: int, shape, dtype) -> np.ndarray:
+        """Part ``part`` of recorder ``name``'s raw data as an array of ``shape``, whose bytes must be the part's (the
+        cluster ensemble's rows: at most)."""
+        out = np.empty(shape, dtype=dtype)
+        st = self._state(name)
+        need = int(st.part_bytes[part])
+        if st.on and (out.nbytes > need or (out.nbytes < need and (name, part) != ("cluster_ensemble", 0))):
+            raise RuntimeError(f"{name} part {part}: {out.nbytes} bytes asked for, the library holds {need}")
+        self._ens_check(self._lib.dcsim_recorder_fetch(self._h, RECORDERS.index(name), part, C.c_void_p(out.ctypes.data),
+                                                       out.nbytes))
+        return out
+
+    def _histogram(self, name: str, shape) -> np.ndarray:
+        out = np.zeros(shape, dtype=np.uint64)
+        N.check(self._lib.dcsim_recorder_histogram(self._h, RECORDERS.index(name), C.c_void_p(out.ctypes.data),
+                                                   out.nbytes), self._h)
+        return out
+
+    def _arg(self, name: str):
+        """The resolved argument of recorder ``name``: window width, threshold or SLA (None: none, or it is off)."""
+        st = self._state(name)
+        return float(st.arg) if st.on and st.arg != math.inf else None
+
     # -- cluster-log ensemble (ensemble.py turns it into per-tick statistics) --------------------------------------
     def enable_cluster_ensemble(self, max_ticks=None):
         """Opt-in, before the first advance of a batch (stays on across reset): every replica records the values of its
         cluster_log.csv rows at every log tick (ensemble.FIELDS).  ``max_ticks=None``: the exact tick count of the spec."""
-        N.check(self._lib.dcsim_enable_cluster_ensemble(self._h, int(max_ticks or 0)), self._h)
-        cap = C.c_uint32(0)
-        N.check(self._lib.dcsim_cluster_ensemble_capacity(self._h, C.byref(cap)), self._h)
-        self._ens_cap, self._ens_on = int(cap.value), True
+        self._enable("cluster_ensemble", int(max_ticks or 0))
 
     @property
     def cluster_ensemble_capacity(self) -> int:
         """Log ticks the recorder holds (0: not enabled, or a spec without a log tick: log_interval > duration)."""
-        return self._ens_cap
+        return int(self._state("cluster_ensemble").rows)
 
     def _ens_check(self, rc):
         """A replica recorded more ticks than the capacity: RecorderOverflow (never a truncated ensemble)."""
-        if rc == N.E_STATE and self._ens_cap and b"overflow" in (self._lib.dcsim_last_error(self._h) or b""):
+        if rc == N.E_STATE and b"overflow" in (self._lib.dcsim_last_error(self._h) or b"") and self.cluster_ensemble_capacity:
             needed = int(self.summary()[:, S.S_EV_LOG].max())
-            raise RecorderOverflow(3, needed, self._ens_cap)
+            raise RecorderOverflow(3, needed, self.cluster_ensemble_capacity)
         N.check(rc, self._h)
 
     def cluster_ensemble_rows(self) -> np.ndarray:
         """[ticks, FIELDS, n_dc, n_replicas] float64, ticks = the most any replica recorded; NaN where a replica did not
         reach a tick.  Raises RecorderOverflow if a replica went past the capacity.  For tests and small batches."""
-        if not self._ens_on:
+        if not self._state("cluster_ensemble").on:
             raise RuntimeError("cluster ensemble not enabled (enable_cluster_ensemble)")
-        ticks = min(int(self.summary()[:, S.S_EV_LOG].max()), self._ens_cap)
-        out = np.empty((ticks, ENS_FIELDS, self.spec.n_dc, self.n_replicas), dtype=np.float64)
-        self._ens_check(self._lib.dcsim_fetch_cluster_ensemble(self._h, C.c_void_p(out.ctypes.data), out.nbytes))
-        return out
+        ticks = min(int(self.summary()[:, S.S_EV_LOG].max()), self.cluster_ensemble_capacity)
+        return self._fetch("cluster_ensemble", 0, (ticks, ENS_FIELDS, self.spec.n_dc, self.n_replicas), np.float64)
 
     # -- job-log ensemble (ensemble.job_ensemble turns it into per-window statistics) --------------------------------
     def enable_job_ensemble(self, bin_s=None):
         """Opt-in, before the first advance of a batch (stays on across reset): every replica sums its finished jobs and
         their latencies per finish window of ``bin_s`` seconds (None / 0: log_interval), DC and job type, plus a per-DC
-        job-latency histogram."""
-        if self._jens_bin != (float(bin_s) if bin_s else float(self.spec.log_interval)):
-            self._jwait_on = False     # the library drops the waits recorder with the old windows, even when this fails
-            self._jres_on = False      # and the job-resources recorder
-        N.check(self._lib.dcsim_enable_job_ensemble(self._h, float(bin_s or 0.0)), self._h)
-        w = C.c_uint32(0)
-        N.check(self._lib.dcsim_job_ensemble_windows(self._h, C.byref(w)), self._h)
-        self._jens_windows = int(w.value)
-        self._jens_bin = float(bin_s) if bin_s else float(self.spec.log_interval)
+        job-latency histogram.  Another window width drops the job-waits and job-resources recorders."""
+        self._enable("job_ensemble", float(bin_s or 0.0))
 
     @property
     def job_ensemble_windows(self) -> int:
         """W, the finish windows (0: not enabled); the recorder's rows are W + 1, the last one the whole run."""
-        return self._jens_windows
+        st = self._state("job_ensemble")
+        return int(st.rows) - 1 if st.on else 0
 
     @property
     def job_ensemble_bin(self):
         """The window width [s] (None: not enabled)."""
-        return self._jens_bin if self._jens_windows else None
+        return self._arg("job_ensemble")
 
     def job_ensemble_rows(self):
         """(rows [W + 1, JENS_STORED, n_dc, 2, n_replicas] float64 {jobs, lat_sum}, hist [n_dc, 2, LAT_BINS, n_replicas]
         uint32): every replica's raw recorder.  For tests and small batches."""
-        if not self._jens_windows:
+        W = self.job_ensemble_windows
+        if not W:
             raise RuntimeError("job ensemble not enabled (enable_job_ensemble)")
-        rows = np.empty((self._jens_windows + 1, JENS_STORED, self.spec.n_dc, 2, self.n_replicas), dtype=np.float64)
-        hist = np.empty((self.n_replicas, self.spec.n_dc, 2, LAT_BINS), dtype=np.uint32)
-        N.check(self._lib.dcsim_fetch_job_ensemble(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
-                                                   C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        rows = self._fetch("job_ensemble", 0, (W + 1, JENS_STORED, self.spec.n_dc, 2, self.n_replicas), np.float64)
+        hist = self._fetch("job_ensemble", 1, (self.n_replicas, self.spec.n_dc, 2, LAT_BINS), np.uint32)
         return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
 
     def dc_latency_histogram(self) -> np.ndarray:
         """[n_dc, 2, LAT_BINS] uint64: job-latency counts per DC and job type over the replicas with status 0."""
-        out = np.zeros((self.spec.n_dc, 2, LAT_BINS), dtype=np.uint64)
-        N.check(self._lib.dcsim_fetch_dc_latency_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
-        return out
+        return self._histogram("job_ensemble", (self.spec.n_dc, 2, LAT_BINS))
 
     # -- waiting and response times (ensemble.job_waits), in the job ensemble's cells ---------------------------------
     def enable_job_waits(self):
         """Opt-in, after enable_job_ensemble and before the first advance of a batch (stays on across reset, zeroed by
         it): every finished job adds its wait (start - xfer_done) and response time (finish - arrival) to its cells of the
         job ensemble, and to per-DC wait and response histograms.  The running records then carry the job id."""
-        N.check(self._lib.dcsim_enable_job_waits(self._h), self._h)
-        self._jwait_on = True
+        self._enable("job_waits")
 
     @property
     def job_waits_enabled(self) -> bool:
-        return getattr(self, "_jwait_on", False) and bool(self._jens_windows)
+        return bool(self._state("job_waits").on)
 
     def job_waits_rows(self):
         """(rows [W + 1, JWAIT_STORED, n_dc, 2, n_replicas] float64 {waited, wait_sum, resp_sum}, hist [n_dc, 2 kinds,
         2, LAT_BINS, n_replicas] uint32): every replica's raw recorder.  For tests and small batches."""
         if not self.job_waits_enabled:
             raise RuntimeError("job waits not enabled (enable_job_waits)")
-        rows = np.empty((self._jens_windows + 1, JWAIT_STORED, self.spec.n_dc, 2, self.n_replicas), dtype=np.float64)
-        hist = np.empty((self.n_replicas, self.spec.n_dc, 2, 2, LAT_BINS), dtype=np.uint32)
-        N.check(self._lib.dcsim_fetch_job_waits(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
-                                                C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        W = self.job_ensemble_windows
+        rows = self._fetch("job_waits", 0, (W + 1, JWAIT_STORED, self.spec.n_dc, 2, self.n_replicas), np.float64)
+        hist = self._fetch("job_waits", 1, (self.n_replicas, self.spec.n_dc, 2, 2, LAT_BINS), np.uint32)
         return rows, np.ascontiguousarray(np.moveaxis(hist, 0, -1))
 
     def dc_wait_histogram(self) -> np.ndarray:
         """[n_dc, 2 kinds (wait, response), 2, LAT_BINS] uint64 over the replicas with status 0."""
-        out = np.zeros((self.spec.n_dc, 2, 2, LAT_BINS), dtype=np.uint64)
-        N.check(self._lib.dcsim_fetch_dc_wait_histogram(self._h, C.c_void_p(out.ctypes.data), out.nbytes), self._h)
-        return out
+        return self._histogram("job_waits", (self.spec.n_dc, 2, 2, LAT_BINS))
 
     # -- job resources (ensemble.job_resources), in the job ensemble's cells ------------------------------------------
     def enable_job_resources(self):
@@ -308,12 +322,11 @@ class BatchedEngine:
         it): every finished job adds its GPU count, frequency and predicted energy E_pred * size to its cells of the job
         ensemble, and one count each to its DC's (n, f) mix and energy-per-job histogram.  The running records then
         carry the size and frequency."""
-        N.check(self._lib.dcsim_enable_job_resources(self._h), self._h)
-        self._jres_on = True
+        self._enable("job_resources")
 
     @property
     def job_resources_enabled(self) -> bool:
-        return getattr(self, "_jres_on", False) and bool(self._jens_windows)
+        return bool(self._state("job_resources").on)
 
     def job_resources_rows(self):
         """(rows [W + 1, JRES_STORED, n_dc, 2, n_replicas] float64 {gpu_sum, freq_sum, energy_sum}, mix [n_dc, 2, G,
@@ -322,12 +335,9 @@ class BatchedEngine:
         if not self.job_resources_enabled:
             raise RuntimeError("job resources not enabled (enable_job_resources)")
         n_dc, n, G = self.spec.n_dc, self.n_replicas, jres_mix_g(self.spec.max_gpus_per_job)
-        rows = np.empty((self._jens_windows + 1, JRES_STORED, n_dc, 2, n), dtype=np.float64)
-        mix = np.empty((n_dc, 2, G * MAX_FREQ + 1, n), dtype=np.uint32)
-        hist = np.empty((n_dc, 2, JRES_EBINS, n), dtype=np.uint32)
-        N.check(self._lib.dcsim_fetch_job_resources(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes,
-                                                    C.c_void_p(mix.ctypes.data), mix.nbytes,
-                                                    C.c_void_p(hist.ctypes.data), hist.nbytes), self._h)
+        rows = self._fetch("job_resources", 0, (self.job_ensemble_windows + 1, JRES_STORED, n_dc, 2, n), np.float64)
+        mix = self._fetch("job_resources", 1, (n_dc, 2, G * MAX_FREQ + 1, n), np.uint32)
+        hist = self._fetch("job_resources", 2, (n_dc, 2, JRES_EBINS, n), np.uint32)
         return rows, mix[:, :, :-1].reshape(n_dc, 2, G, MAX_FREQ, n), np.ascontiguousarray(mix[:, :, -1]), hist
 
     # -- power profile (ensemble.power_profile turns it into batch statistics) ----------------------------------------
@@ -336,19 +346,16 @@ class BatchedEngine:
         cluster power step function — peak, time and energy over ``threshold`` watts (None: no threshold), per-DC peaks
         and a time-weighted power histogram (include/dcsim_b200.h DCSIM_PP_*).  Runs the event-loop instantiation with
         the recorder compiled in."""
-        N.check(self._lib.dcsim_enable_power_profile(self._h, float("inf") if threshold is None else float(threshold)),
-                self._h)
-        self._pp_threshold = None if threshold is None else float(threshold)
-        self._pp_on = True
+        self._enable("power_profile", math.inf if threshold is None else threshold)
 
     @property
     def power_profile_enabled(self) -> bool:
-        return getattr(self, "_pp_on", False)
+        return bool(self._state("power_profile").on)
 
     @property
     def power_threshold(self):
         """The threshold [W] of the enabled profile (None: none)."""
-        return getattr(self, "_pp_threshold", None)
+        return self._arg("power_profile")
 
     def power_profile_range(self) -> float:
         """hi [W]: the power histogram covers [0, hi] in PP_BINS bins (the library's bound, dcsim_power_profile_range)."""
@@ -358,9 +365,7 @@ class BatchedEngine:
 
     def power_profile_rows(self) -> np.ndarray:
         """[PP_FIELDS + n_dc + PP_BINS, n_replicas] float64: every replica's raw profile.  For tests and small batches."""
-        rows = np.empty((S.PP_FIELDS + self.spec.n_dc + S.PP_BINS, self.n_replicas), dtype=np.float64)
-        N.check(self._lib.dcsim_fetch_power_profile(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
-        return rows
+        return self._fetch("power_profile", 0, (S.PP_FIELDS + self.spec.n_dc + S.PP_BINS, self.n_replicas), np.float64)
 
     # -- occupancy (ensemble.occupancy turns it into batch statistics) ------------------------------------------------
     def enable_occupancy(self):
@@ -368,12 +373,11 @@ class BatchedEngine:
         DC, the time-weighted queue lengths, running jobs and busy GPUs between every two events — areas, maxima, time
         queued / saturated / idle, and queue-length and busy-GPU histograms (include/dcsim_b200.h DCSIM_OCC_*).  Runs the
         event-loop instantiation with the profile recorders compiled in."""
-        N.check(self._lib.dcsim_enable_occupancy(self._h), self._h)
-        self._occ_on = True
+        self._enable("occupancy")
 
     @property
     def occupancy_enabled(self) -> bool:
-        return getattr(self, "_occ_on", False)
+        return bool(self._state("occupancy").on)
 
     def occupancy_bin_widths(self) -> np.ndarray:
         """[n_dc] int32: GPUs per busy-GPU bin of each DC (1 for DCs of up to 127 GPUs)."""
@@ -385,27 +389,22 @@ class BatchedEngine:
         """[1 + OCC_FIELDS * n_dc + 2 * OCC_BINS * n_dc, n_replicas] float64: every replica's raw columns.  For tests
         and small batches."""
         n_dc = self.spec.n_dc
-        rows = np.empty((1 + S.OCC_FIELDS * n_dc + 2 * S.OCC_BINS * n_dc, self.n_replicas), dtype=np.float64)
-        N.check(self._lib.dcsim_fetch_occupancy(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
-        return rows
+        return self._fetch("occupancy", 0, (1 + S.OCC_FIELDS * n_dc + 2 * S.OCC_BINS * n_dc, self.n_replicas), np.float64)
 
     # -- energy cost and carbon (ensemble.energy_cost turns it into batch statistics) --------------------------------
     def enable_energy_cost(self):
         """Opt-in, before the first advance of a batch (stays on across reset, zeroed by it): every replica records each
         DC's energy by hour of day, its cost under the DC's hourly tariff and its carbon (include/dcsim_b200.h
         DCSIM_COST_*).  Runs the event-loop instantiation with the profile recorders compiled in."""
-        N.check(self._lib.dcsim_enable_energy_cost(self._h), self._h)
-        self._cost_on = True
+        self._enable("energy_cost")
 
     @property
     def energy_cost_enabled(self) -> bool:
-        return getattr(self, "_cost_on", False)
+        return bool(self._state("energy_cost").on)
 
     def energy_cost_rows(self) -> np.ndarray:
         """[cost_cols(n_dc), n_replicas] float64: every replica's raw columns.  For tests and small batches."""
-        rows = np.empty((S.cost_cols(self.spec.n_dc), self.n_replicas), dtype=np.float64)
-        N.check(self._lib.dcsim_fetch_energy_cost(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
-        return rows
+        return self._fetch("energy_cost", 0, (S.cost_cols(self.spec.n_dc), self.n_replicas), np.float64)
 
     # -- per-run tail latency (ensemble.tail_latency turns it into batch statistics) ----------------------------------
     def enable_tail_latency(self, sla_s=None):
@@ -414,25 +413,21 @@ class BatchedEngine:
         replica's exact p50 / p95 / p99 / p99.9 / max of service, wait and response time per (job type, scope), and
         whether its p99 met ``sla_s`` seconds (None: no SLA) — include/dcsim_b200.h DCSIM_TAIL_*.  The running records
         then carry the job id."""
-        N.check(self._lib.dcsim_enable_tail_latency(self._h, float("inf") if sla_s is None else float(sla_s)), self._h)
-        self._tail_sla = None if sla_s is None else float(sla_s)
-        self._tail_on = True
+        self._enable("tail_latency", math.inf if sla_s is None else sla_s)
 
     @property
     def tail_latency_enabled(self) -> bool:
-        return getattr(self, "_tail_on", False)
+        return bool(self._state("tail_latency").on)
 
     @property
     def tail_latency_sla(self):
         """The SLA [s] of the enabled recorder (None: none)."""
-        return getattr(self, "_tail_sla", None)
+        return self._arg("tail_latency")
 
     def tail_latency_rows(self) -> np.ndarray:
         """[S.tail_cols(n_dc), n_replicas] float64: every replica's columns (NaN: does not count).  Runs the selection
         pass first if the batch has not had it yet.  For tests and small batches."""
-        rows = np.empty((S.tail_cols(self.spec.n_dc), self.n_replicas), dtype=np.float64)
-        N.check(self._lib.dcsim_fetch_tail_latency(self._h, C.c_void_p(rows.ctypes.data), rows.nbytes), self._h)
-        return rows
+        return self._fetch("tail_latency", 0, (S.tail_cols(self.spec.n_dc), self.n_replicas), np.float64)
 
     def tail_latency_jobs(self, first: int = 0, count=None) -> np.ndarray:
         """[count, cap_arrivals, 2] float64: the raw slot buffer of local replicas [first, first + count) (None: to the
@@ -486,7 +481,7 @@ class BatchedEngine:
         N.check(self._lib.dcsim_recorder_counts(self._h, C.byref(out)), self._h)
         return int(out[0]), int(out[1]), int(out[2])
 
-    def _fetch(self, fn, dtype, cap, which):
+    def _fetch_log(self, fn, dtype, cap, which):
         arr = np.zeros(max(cap, 1), dtype=dtype)
         n = C.c_uint32(0)
         N.check(fn(self._h, C.c_void_p(arr.ctypes.data), cap, C.byref(n)), self._h)
@@ -496,13 +491,13 @@ class BatchedEngine:
 
     def trace(self):
         """The first `capacity` processed events of the traced replica (a debug aid: a prefix by design)."""
-        return self._fetch(self._lib.dcsim_fetch_trace, TRACE_DTYPE, self._trace_cap, None)
+        return self._fetch_log(self._lib.dcsim_fetch_trace, TRACE_DTYPE, self._trace_cap, None)
 
     def job_log(self):
-        return self._fetch(self._lib.dcsim_fetch_job_log, JOB_DTYPE, self._jobs_cap, 1)
+        return self._fetch_log(self._lib.dcsim_fetch_job_log, JOB_DTYPE, self._jobs_cap, 1)
 
     def cluster_log(self):
-        return self._fetch(self._lib.dcsim_fetch_cluster_log, CLUSTER_DTYPE, self._cluster_cap, 2)
+        return self._fetch_log(self._lib.dcsim_fetch_cluster_log, CLUSTER_DTYPE, self._cluster_cap, 2)
 
     def launch_info(self) -> dict:
         li = S.LaunchInfo()
@@ -592,13 +587,15 @@ def _recorders(sp, cluster_ensemble=False, job_ensemble=False, job_ensemble_bin=
     return tuple((name, args) for name, on, args in calls if on)
 
 
+# the keyword of acquire_engine that carries each recorder's argument
+_RECORDER_ARGS = {"job_ensemble": "job_ensemble_bin", "power_profile": "power_threshold", "tail_latency": "tail_sla_s"}
+
+
 def _engine_recorders(eng):
-    """The recorder keywords of acquire_engine that ``eng`` runs with."""
-    return dict(cluster_ensemble=eng.cluster_ensemble_capacity > 0, job_ensemble=eng.job_ensemble_bin is not None,
-                job_ensemble_bin=eng.job_ensemble_bin, power_profile=eng.power_profile_enabled,
-                power_threshold=eng.power_threshold, job_waits=eng.job_waits_enabled, occupancy=eng.occupancy_enabled,
-                tail_latency=eng.tail_latency_enabled, tail_sla_s=eng.tail_latency_sla,
-                job_resources=eng.job_resources_enabled, energy_cost=eng.energy_cost_enabled)
+    """The recorder keywords of acquire_engine that ``eng`` runs with, as the library holds its recorders."""
+    kw = {name: bool(eng._state(name).on) for name in RECORDERS}
+    kw.update((key, eng._arg(name)) for name, key in _RECORDER_ARGS.items())
+    return kw
 
 
 def _cache_key(sp, n_replicas, device, cuda_stream, recorders):

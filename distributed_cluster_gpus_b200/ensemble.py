@@ -286,8 +286,11 @@ def device_passes(dev, cols: int, moments_into, spread_into, stat_cols: int = No
 
 
 def _recorder_passes(engine, name: str):
-    """device_passes over recorder ``name`` (engine.RECORDERS) of ``engine``, on the columns the library reduces."""
+    """device_passes over recorder ``name`` (engine.RECORDERS) of ``engine``, on the columns the library reduces.  A
+    recorder that is off is a RuntimeError here, but for the two ensembles: the library refuses those."""
     import torch
+    if name not in ("cluster_ensemble", "job_ensemble") and not getattr(engine, f"{name}_enabled"):
+        raise RuntimeError(f"{name.replace('_', ' ')} not enabled (enable_{name})")
     cols, spread_cols = engine.stat_columns(name)
     return device_passes(torch.device("cuda", engine.device), cols, functools.partial(engine.stat_moments_into, name),
                          functools.partial(engine.stat_spread_into, name), spread_cols)
@@ -618,8 +621,6 @@ def job_waits(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> JobWait
     """Statistics of the waiting / response-time recorder of ``engine`` (a finished BatchedEngine with enable_job_waits()),
     over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
     import torch
-    if not engine.job_waits_enabled:
-        raise RuntimeError("job waits not enabled (enable_job_waits)")
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
     passes = _recorder_passes(engine, "job_waits")
@@ -840,8 +841,6 @@ def job_resources(engine, quantiles: Sequence[float] = DEFAULT_QUANTILES) -> Job
     """Statistics of the job-resources recorder of ``engine`` (a finished BatchedEngine with enable_job_resources()),
     over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
     from .engine import jres_mix_g
-    if not engine.job_resources_enabled:
-        raise RuntimeError("job resources not enabled (enable_job_resources)")
     sp = engine.spec
     passes = _recorder_passes(engine, "job_resources")
     return res_finalize(*passes, sp.n_dc, jres_mix_g(sp.max_gpus_per_job), _res_levels(sp), engine.job_ensemble_bin,
@@ -997,8 +996,6 @@ def power_profile(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES, summary
     ranks when torch.distributed runs with world > 1 (every rank calls this).  ``summary``: the engine's summary rows if
     the caller has them already (they give the pooled energy)."""
     import torch
-    if not engine.power_profile_enabled:
-        raise RuntimeError("power profile not enabled (enable_power_profile)")
     dev = torch.device("cuda", engine.device)
     n_dc = engine.spec.n_dc
     passes = _recorder_passes(engine, "power_profile")
@@ -1153,8 +1150,6 @@ def occ_finalize(mom, m2, hist, n_dc: int, widths, quantiles: Sequence[float] = 
 def occupancy(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> OccupancyResult:
     """Statistics of the occupancy recorder of ``engine`` (a finished BatchedEngine with enable_occupancy()), over all
     ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    if not engine.occupancy_enabled:
-        raise RuntimeError("occupancy not enabled (enable_occupancy)")
     passes = _recorder_passes(engine, "occupancy")
     return occ_finalize(*passes, engine.spec.n_dc, engine.occupancy_bin_widths(), quantiles)
 
@@ -1332,8 +1327,6 @@ def tail_finalize(mom, m2, hist, n_dc: int, sla_s: float, quantiles: Sequence[fl
 def tail_latency(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> TailLatencyResult:
     """Statistics of the per-run tail-latency columns of ``engine`` (a finished BatchedEngine with
     enable_tail_latency()), over all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    if not engine.tail_latency_enabled:
-        raise RuntimeError("tail latency not enabled (enable_tail_latency)")
     passes = _recorder_passes(engine, "tail_latency")
     sla = engine.tail_latency_sla
     return tail_finalize(*passes, engine.spec.n_dc, math.inf if sla is None else sla, quantiles)
@@ -1456,8 +1449,6 @@ def _cost_tables(sp):
 def energy_cost(engine, quantiles: Sequence[float] = PP_CSV_QUANTILES) -> EnergyCostResult:
     """Statistics of the energy-cost recorder of ``engine`` (a finished BatchedEngine with enable_energy_cost()), over
     all ranks when torch.distributed runs with world > 1 (every rank calls this)."""
-    if not engine.energy_cost_enabled:
-        raise RuntimeError("energy cost not enabled (enable_energy_cost)")
     passes = _recorder_passes(engine, "energy_cost")
     return cost_finalize(*passes, engine.spec.n_dc, *_cost_tables(engine.spec), quantiles)
 

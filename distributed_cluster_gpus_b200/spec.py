@@ -179,6 +179,12 @@ class LaunchInfo(C.Structure):
                 ("lanes_per_replica", C.c_int32)]
 
 
+class RecorderState(C.Structure):
+    """dcsim_recorder_state_t: a batch recorder as the library holds it (all 0 but ``parts`` while it is off)."""
+    _fields_ = [("on", C.c_int32), ("parts", C.c_int32), ("arg", C.c_double), ("rows", C.c_uint64),
+                ("part_bytes", C.c_uint64 * 3)]
+
+
 def _price_for(energy_price, dc_name: str, hour: int) -> float:
     """SIM:986-1005 for a given hour."""
     ep = energy_price or {}

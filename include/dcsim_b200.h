@@ -356,6 +356,36 @@ int dcsim_stat_moments(dcsim_t* h, int stat, double* dev_out);
 int dcsim_stat_spread(dcsim_t* h, int stat, const double* dev_mean, const double* dev_lo, const double* dev_hi,
                       double* dev_m2_out, uint64_t* dev_hist_out);
 
+/* ---- the batch recorders' lifecycle, by the same ids ------------------------------------------------------------------
+ * dcsim_recorder_enable switches recorder `stat` on with argument `arg` (each recorder's block names it; 0 for those
+ * without one).  Opt-in, before the first advance of a batch; a recorder stays on across dcsim_reset, which refills its
+ * buffers as enabling does (zeroed; the cluster ensemble's rows and the tail slots NaN, the tail columns stale).  Enabling
+ * an enabled recorder again:
+ *   cluster_ensemble, job_ensemble   another capacity / window width reallocates (a job ensemble of other windows drops
+ *                                    job_waits and job_resources); the same one is DCSIM_OK, even after an advance;
+ *   the others                       keep their buffers, refilled, and take the new argument.
+ * Checked in this order: DCSIM_E_INVALID for a bad argument; DCSIM_E_STATE when job_waits or job_resources come without
+ * the job ensemble, when any but the two ensembles is enabled on a member of a shared group, and after the first advance;
+ * DCSIM_E_NOMEM, with the byte count in dcsim_last_error, when the buffers do not fit (the handle stays usable).
+ * dcsim_recorder_state is host only (like dcsim_stat_columns) and all 0 but `parts` while the recorder is off.
+ * dcsim_recorder_fetch copies part `part` of the raw per-replica data to host memory (synchronises), after the same
+ * checks and precondition as the reductions (DCSIM_E_STATE when off or before the first advance; the cluster ensemble's
+ * capacity check, the tail selection).  A part must fit in out_bytes (DCSIM_E_INVALID), except the cluster ensemble's
+ * rows: the whole ticks that fit, at most the capacity.  For tests and small batches.
+ * dcsim_recorder_histogram sums the per-replica histograms of the job ensemble or job waits over the replicas with
+ * status 0 (synchronises); any other id is DCSIM_E_INVALID. */
+typedef struct {
+  int32_t on;             /* 1: enabled on this handle */
+  int32_t parts;          /* parts dcsim_recorder_fetch copies (1..3) */
+  double arg;             /* resolved argument: bin_s, threshold_w, sla_s (+inf: none); 0 for the others */
+  uint64_t rows;          /* cluster ensemble: tick capacity; job ensemble, job waits, job resources: W + 1; else 1 */
+  uint64_t part_bytes[3]; /* full size of each part */
+} dcsim_recorder_state_t;
+int dcsim_recorder_enable(dcsim_t* h, int stat, double arg);
+int dcsim_recorder_state(dcsim_t* h, int stat, dcsim_recorder_state_t* out);
+int dcsim_recorder_fetch(dcsim_t* h, int stat, int part, void* out, size_t out_bytes);
+int dcsim_recorder_histogram(dcsim_t* h, int stat, uint64_t* out, size_t out_bytes);
+
 /* Cluster-log ensemble: at every log tick, for EVERY replica, the values the replica's cluster_log.csv row of each DC
  * would hold (simulator_paper_multi.py write_csv_logs), unrounded.  Device layout [tick][field][dc][replica] doubles,
  * replica fastest (the reductions read it coalesced).  Tick k is the k-th processed log event (instant: the chain
@@ -376,16 +406,10 @@ enum {
   DCSIM_ENS_ENERGY_J = 10,   /* unrounded (the CSV shows energy_kJ) */
   DCSIM_ENS_FIELDS = 11
 };
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, like the latency histogram).  max_ticks = 0:
- * the exact number of log ticks of the spec (the t += log_interval chain replayed against the loop's t > end_time
- * cut-off).  DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the buffer does not fit. */
-int dcsim_enable_cluster_ensemble(dcsim_t* h, uint32_t max_ticks);
-/* Tick capacity of the recorder (0 = not enabled). */
-int dcsim_cluster_ensemble_capacity(dcsim_t* h, uint32_t* ticks_out);
-/* Copies the first min(capacity, out_bytes / row bytes) ticks of the raw values, [tick][field][dc][replica] doubles,
- * to host memory (synchronises).  Ticks a replica did not reach read as NaN.  For tests and small batches. */
-int dcsim_fetch_cluster_ensemble(dcsim_t* h, double* out, size_t out_bytes);
-/* DCSIM_STAT_CLUSTER_ENSEMBLE: columns (tick, field, dc), capacity * FIELDS * n_dc of them (0 when not enabled), each
+/* DCSIM_STAT_CLUSTER_ENSEMBLE, arg max_ticks, a whole number: the tick capacity (rows); 0: the exact number of log
+ * ticks of the spec (the t += log_interval chain replayed against the loop's t > end_time cut-off).  Part 0: the
+ * values, [tick][field][dc][replica] doubles; ticks a replica did not reach read as NaN. */
+/* Statistic: columns (tick, field, dc), capacity * FIELDS * n_dc of them (0 when not enabled), each
  * over the replicas that recorded the tick; the spread covers every column.  Integer fields: busy, run_*, q_*.  Both
  * passes synchronise once to check the capacity. */
 
@@ -406,20 +430,11 @@ enum {
   DCSIM_JENS_MEAN_LATENCY = 2, /* LAT_SUM / JOBS (reductions only) */
   DCSIM_JENS_FIELDS = 3        /* fields of the reductions' columns */
 };
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  bin_s = 0: log_interval.
- * DCSIM_E_INVALID when bin_s is negative or not finite, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when
- * the buffers do not fit, DCSIM_E_STATE after the first advance. */
-int dcsim_enable_job_ensemble(dcsim_t* h, double bin_s);
-/* W, the number of finish windows (0 = not enabled); the rows are W + 1. */
-int dcsim_job_ensemble_windows(dcsim_t* h, uint32_t* windows_out);
-/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][STORED][n_dc][2][n_replicas] doubles,
- * `hist` [n_replicas][n_dc][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than its array is
- * DCSIM_E_INVALID.  For tests and small batches. */
-int dcsim_fetch_job_ensemble(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
-/* DCSIM_STAT_JOB_ENSEMBLE: columns (row, field, dc, jtype), (W + 1) * JENS_FIELDS * n_dc * 2 of them (W = 0 when not
- * enabled), over the valid replicas; the spread covers every column.  JOBS is the integer field. */
-/* The per-DC job-latency histograms summed over the valid replicas: `out` [n_dc][2][DCSIM_LAT_BINS] u64 (synchronises). */
-int dcsim_fetch_dc_latency_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
+/* DCSIM_STAT_JOB_ENSEMBLE, arg bin_s, finite and >= 0 (0: log_interval); rows W + 1.  Part 0: `rows`
+ * [W + 1][STORED][n_dc][2][n_replicas] doubles, part 1: `hist` [n_replicas][n_dc][2][DCSIM_LAT_BINS] u32.
+ * dcsim_recorder_histogram: the per-DC job-latency histograms summed over the valid replicas, [n_dc][2][DCSIM_LAT_BINS]
+ * u64.  Statistic: columns (row, field, dc, jtype), (W + 1) * JENS_FIELDS * n_dc * 2 of them (W = 0 when not enabled),
+ * over the valid replicas; the spread covers every column.  JOBS is the integer field. */
 
 /* Waiting and response times (beside the job-log ensemble, in its cells): a finished job's arrival instant `arr`
  * (simulator_paper_multi.py:539-540), its xfer_done instant `tx` (SIM:580-588) and its start and finish give
@@ -441,22 +456,12 @@ enum {
   DCSIM_JWAIT_MEAN_RESPONSE = 4, /* RESP_SUM / JOBS (reductions only) */
   DCSIM_JWAIT_FIELDS = 5         /* fields of the reductions' columns */
 };
-/* Opt-in, after dcsim_enable_job_ensemble and before the first advance of a batch (stays on across dcsim_reset, zeroed
- * by it; a later dcsim_enable_job_ensemble with another bin_s switches it off).  The running-job records then carry the
- * job id (the layout job_log.csv uses).  DCSIM_E_STATE without the job
- * ensemble, after the first advance or on a member of a shared group; DCSIM_E_NOMEM (with the byte count in
- * dcsim_last_error) when the buffers do not fit. */
-int dcsim_enable_job_waits(dcsim_t* h);
-/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][DCSIM_JWAIT_STORED][n_dc][2]
- * [n_replicas] doubles, `hist` [n_replicas][n_dc][2][2][DCSIM_LAT_BINS] u32.  Either may be NULL; a buffer smaller than
- * its array is DCSIM_E_INVALID. */
-int dcsim_fetch_job_waits(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* hist, size_t hist_bytes);
-/* DCSIM_STAT_JOB_WAITS: columns (row, field, dc, jtype), (W + 1) * DCSIM_JWAIT_FIELDS * n_dc * 2 of them (W = 0 when
- * the job ensemble is off), over the valid replicas as described above; the spread covers every column.  WAITED is the
- * integer field. */
-/* The per-DC wait and response histograms summed over the valid replicas: `out` [n_dc][2 kinds][2][DCSIM_LAT_BINS] u64
- * (synchronises). */
-int dcsim_fetch_dc_wait_histogram(dcsim_t* h, uint64_t* out, size_t out_bytes);
+/* DCSIM_STAT_JOB_WAITS, no arg, needs the job ensemble (its rows W + 1).  The running-job records then carry the job id
+ * (the layout job_log.csv uses).  Part 0: `rows` [W + 1][DCSIM_JWAIT_STORED][n_dc][2][n_replicas] doubles, part 1:
+ * `hist` [n_replicas][n_dc][2][2][DCSIM_LAT_BINS] u32.  dcsim_recorder_histogram: the per-DC wait and response
+ * histograms summed over the valid replicas, [n_dc][2 kinds][2][DCSIM_LAT_BINS] u64.  Statistic: columns (row, field,
+ * dc, jtype), (W + 1) * DCSIM_JWAIT_FIELDS * n_dc * 2 of them (W = 0 when the job ensemble is off), over the valid
+ * replicas as described above; the spread covers every column.  WAITED is the integer field. */
 
 /* Job resources (beside the job-log ensemble, in its cells): what every finished job (the set the job ensemble counts)
  * ran on and what the model predicted it would cost.  For a job of DC d with GPU count g (job_log.csv n_gpus), frequency
@@ -495,17 +500,10 @@ enum {
 #define DCSIM_JRES_OCT1 0x1.306fe0a31b716p+0
 #define DCSIM_JRES_OCT2 0x1.6a09e667f3bcdp+0
 #define DCSIM_JRES_OCT3 0x1.ae89f995ad3aep+0
-/* Opt-in, after dcsim_enable_job_ensemble and before the first advance of a batch (stays on across dcsim_reset, zeroed
- * by it; a later dcsim_enable_job_ensemble with another bin_s switches it off).  The running-job records then carry the
- * size and frequency (the layout job_log.csv uses).  DCSIM_E_STATE without the job ensemble, after the first advance or
- * on a member of a shared group; DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the buffers do not fit. */
-int dcsim_enable_job_resources(dcsim_t* h);
-/* Copies the raw per-replica data to host memory (synchronises): `rows` [W + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas]
- * doubles, `mix` [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] u32, `hist` [n_dc][2][DCSIM_JRES_EBINS][n_replicas] u32.
- * Any may be NULL; a buffer smaller than its array is DCSIM_E_INVALID. */
-int dcsim_fetch_job_resources(dcsim_t* h, double* rows, size_t rows_bytes, uint32_t* mix, size_t mix_bytes, uint32_t* hist,
-                              size_t hist_bytes);
-/* DCSIM_STAT_JOB_RESOURCES: (W + 1) * DCSIM_JRES_FIELDS * n_dc * 2 windowed columns (W = 0 when the job ensemble is
+/* DCSIM_STAT_JOB_RESOURCES, no arg, needs the job ensemble (its rows W + 1).  The running-job records then carry the
+ * size and frequency (the layout job_log.csv uses).  Part 0: `rows` [W + 1][DCSIM_JRES_STORED][n_dc][2][n_replicas]
+ * doubles, part 1: `mix` [n_dc][2][DCSIM_JRES_MIX_COLS(G)][n_replicas] u32, part 2: `hist`
+ * [n_dc][2][DCSIM_JRES_EBINS][n_replicas] u32.  Statistic: (W + 1) * DCSIM_JRES_FIELDS * n_dc * 2 windowed columns (W = 0 when the job ensemble is
  * off), then n_dc * 2 * (MIX_COLS(G) + EBINS) count columns, over the replicas with status 0; the count columns' sums
  * are the pooled mix and energy histogram.  The spread covers the windowed columns only, GPU_SUM the integer field. */
 
@@ -533,19 +531,14 @@ enum {
   DCSIM_PP_FIELDS = 8 /* then n_dc DC_PEAK_W columns, then DCSIM_PP_BINS histogram columns */
 };
 #define DCSIM_PP_BINS 1024
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  threshold_w = +inf: no
- * threshold (the OVER_* / EXCURSIONS fields stay 0).  DCSIM_E_INVALID for a NaN or negative threshold, DCSIM_E_STATE
- * after the first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error)
- * when the rows do not fit. */
-int dcsim_enable_power_profile(dcsim_t* h, double threshold_w);
+/* DCSIM_STAT_POWER_PROFILE, arg threshold_w >= 0; +inf: no threshold (the OVER_* / EXCURSIONS fields stay 0).  Part
+ * 0: the columns above. */
 /* hi: the histogram's upper end, an upper bound on the cluster power of any state the spec allows — sum over DCs of
  * total_gpus * max(idle or sleep power, per-GPU busy power at every (job type, frequency) a job can run at, the tail
  * formula's per-GPU active power at those frequencies), times (1 + 2^-20) for the rounding of the sums.  Host only;
  * works whether or not the profile is enabled. */
 int dcsim_power_profile_range(dcsim_t* h, double* hi_out);
-/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
-int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes);
-/* DCSIM_STAT_POWER_PROFILE: every stored column (the fields, DC_PEAK_W, the bins), DCSIM_PP_FIELDS + n_dc +
+/* Statistic: every stored column (the fields, DC_PEAK_W, the bins), DCSIM_PP_FIELDS + n_dc +
  * DCSIM_PP_BINS of them, over the replicas with status 0; the bins' sums are the pooled power-duration curve.  The
  * spread covers the first DCSIM_PP_FIELDS + n_dc columns only (the bins need none); EXCURSIONS and OUT_OF_RANGE are the
  * integer columns. */
@@ -580,13 +573,7 @@ int dcsim_fetch_power_profile(dcsim_t* h, double* out, size_t out_bytes);
 #define DCSIM_COST_TOTAL_USD(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 1)
 #define DCSIM_COST_TOTAL_G(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 2)
 #define DCSIM_COST_COLS(n_dc) ((DCSIM_HOURS + 3) * (n_dc) + 3)
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  DCSIM_E_STATE after the
- * first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the rows
- * and their working state do not fit. */
-int dcsim_enable_energy_cost(dcsim_t* h);
-/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
-int dcsim_fetch_energy_cost(dcsim_t* h, double* out, size_t out_bytes);
-/* DCSIM_STAT_ENERGY_COST: the DCSIM_COST_COLS(n_dc) stored columns, over the replicas with status 0; the spread covers
+/* DCSIM_STAT_ENERGY_COST, no arg.  Part 0: the columns above.  Statistic: the DCSIM_COST_COLS(n_dc) stored columns, over the replicas with status 0; the spread covers
  * every column.  No integer columns. */
 
 /* Occupancy: for EVERY replica and DC d, how long the queues were and how full the DC was over time.  Step functions over
@@ -613,15 +600,10 @@ enum {
 #define DCSIM_OCC_BINS 128
 /* Busy-GPU bin width of a DC with `total` GPUs: ceil((total + 1) / DCSIM_OCC_BINS), 1 for up to 127 GPUs. */
 #define DCSIM_OCC_BUSY_WIDTH(total) (((total) + DCSIM_OCC_BINS) / DCSIM_OCC_BINS)
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, zeroed by it).  DCSIM_E_STATE after the
- * first advance or on a member of a shared group, DCSIM_E_NOMEM (with the byte count in dcsim_last_error) when the rows
- * and their working state do not fit. */
-int dcsim_enable_occupancy(dcsim_t* h);
+/* DCSIM_STAT_OCCUPANCY, no arg.  Part 0: the columns above. */
 /* w_out[n_dc]: each DC's busy-GPU bin width (DCSIM_OCC_BUSY_WIDTH). */
 int dcsim_occupancy_bin_widths(dcsim_t* h, int32_t* w_out);
-/* Copies the raw per-replica columns to host memory (synchronises); a smaller buffer is DCSIM_E_INVALID. */
-int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes);
-/* DCSIM_STAT_OCCUPANCY: first DCSIM_OCC_FIELDS * n_dc statistics (field, dc), field-major, per replica Q_INF_AREA /
+/* Statistic: first DCSIM_OCC_FIELDS * n_dc statistics (field, dc), field-major, per replica Q_INF_AREA /
  * PROFILE_S, Q_TRN_AREA / PROFILE_S, RUN_AREA / PROFILE_S, Q_INF_MAX, Q_TRN_MAX, QUEUED_S / PROFILE_S, SATURATED_S /
  * PROFILE_S, IDLE_S / PROFILE_S; then the 2 * DCSIM_OCC_BINS * n_dc bins as stored.  A replica counts when its status
  * is 0 and PROFILE_S > 0.  The bins' sums are the pooled time-weighted distributions of queue length and busy GPUs.
@@ -631,8 +613,8 @@ int dcsim_fetch_occupancy(dcsim_t* h, double* out, size_t out_bytes);
  * (status 0 replica) with arrival instant arr (the ingress arrival, simulator_paper_multi.py:539-540), xfer_done instant
  * tx (SIM:580-588), start and finish, each one f64 subtraction:
  *   latency  = finish - start   (SIM:820: the latency_s column, the reference's p99 monitor sample)
- *   wait     = start - tx       (as dcsim_enable_job_waits)
- *   response = finish - arr     (as dcsim_enable_job_waits)
+ *   wait     = start - tx       (as DCSIM_STAT_JOB_WAITS)
+ *   response = finish - arr     (as DCSIM_STAT_JOB_WAITS)
  * A group is (job type, scope): scope 0 all DCs, scope 1 + d DC d (the DC the job ran in).  Per replica and group:
  *   JOBS        jobs of the group that finished;
  *   UNFINISHED  jobs the run created (a jid, SIM:541) of that type, routed to that DC, not finished at end_time
@@ -655,21 +637,16 @@ enum {
 };
 #define DCSIM_TAIL_STAT(kind, stat) (2 + (kind) * DCSIM_TAIL_STATS + (stat))
 #define DCSIM_TAIL_COLS(n_dc) (2 * ((n_dc) + 1) * DCSIM_TAIL_GROUP_FIELDS + 2 * DCSIM_TAIL_KINDS)
-/* Opt-in (before the first advance of a batch; stays on across dcsim_reset, cleared by it).  Each finished job stores its
- * start and finish into a per-arrival slot buffer [n_replicas][cap_arrivals][2] doubles (16 bytes per slot, NaN until
- * it finishes); the running records carry the job id (the layout job_log.csv uses).  DCSIM_E_INVALID for a NaN or
- * negative sla_s (+inf: no SLA), DCSIM_E_STATE after the first advance or on a member of a shared group, DCSIM_E_NOMEM
- * (with the byte count in dcsim_last_error) when the buffers do not fit. */
-int dcsim_enable_tail_latency(dcsim_t* h, double sla_s);
-/* The columns to host memory, [DCSIM_TAIL_COLS(n_dc)][n_replicas] doubles (synchronises).  The columns are made from
- * the slot buffer by one selection pass on the handle's stream, run by the first of this call, dcsim_stat_moments or
- * dcsim_stat_spread after the batch is done (every later advance or reset makes them stale); DCSIM_E_STATE while a
- * replica is still running.  A smaller buffer is DCSIM_E_INVALID. */
-int dcsim_fetch_tail_latency(dcsim_t* h, double* out, size_t out_bytes);
+/* DCSIM_STAT_TAIL_LATENCY, arg sla_s >= 0 (+inf: no SLA).  Each finished job stores its start and finish into a
+ * per-arrival slot buffer [n_replicas][cap_arrivals][2] doubles (16 bytes per slot, NaN until it finishes); the running
+ * records carry the job id (the layout job_log.csv uses).  Part 0: the columns, [DCSIM_TAIL_COLS(n_dc)][n_replicas]
+ * doubles.  The columns are made from the slot buffer by one selection pass on the handle's stream, run by the first
+ * dcsim_recorder_fetch, dcsim_stat_moments or dcsim_stat_spread after the batch is done (every later advance or reset
+ * makes them stale); DCSIM_E_STATE while a replica is still running. */
 /* The raw slot buffer of local replicas [first, first + count): [count][cap_arrivals][2] doubles, (start, finish) of
  * arrival slot jid - 1 (synchronises).  A range, because a large batch's buffer takes tens of GB. */
 int dcsim_fetch_tail_jobs(dcsim_t* h, uint64_t first, uint64_t count, double* out, size_t out_bytes);
-/* DCSIM_STAT_TAIL_LATENCY: the DCSIM_TAIL_COLS(n_dc) columns; the spread covers every column.  A replica counts in a
+/* Statistic: the DCSIM_TAIL_COLS(n_dc) columns; the spread covers every column.  A replica counts in a
  * column when its status is 0 and the value is not NaN.  JOBS, UNFINISHED and SLA_MET are integer columns. */
 
 /* Paired reductions: columns (metric, field), metric-major, over replica r's summary rows of `base` and of a variant

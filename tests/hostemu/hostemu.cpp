@@ -96,9 +96,9 @@ size_t hostemu_sizeof_out(void) { return sizeof(hostemu_out_t); }
 uint32_t hostemu_merge_ring(void) { return DCSIM_MERGE_RING; }
 void hostemu_set_test_time_quantum(double q) { dcsim_test_time_quantum = q; } /* see dcsim_core.cuh dcsim_test_quantize */
 uint32_t hostemu_cap_arr(const void* spec_blob) { return dcsim_cap_arr((const dcsim_spec_t*)spec_blob); }
-/* the library's default tick capacity (dcsim_enable_cluster_ensemble with max_ticks = 0) */
+/* the library's default tick capacity (dcsim_recorder_enable of DCSIM_STAT_CLUSTER_ENSEMBLE with max_ticks = 0) */
 uint32_t hostemu_ens_ticks(const void* spec_blob) { return dcsim_ens_ticks((const dcsim_spec_t*)spec_blob); }
-/* the library's window count of the job-log ensemble for a resolved bin width (dcsim_enable_job_ensemble) */
+/* the library's window count of the job-log ensemble for a resolved bin width (dcsim_recorder_enable of DCSIM_STAT_JOB_ENSEMBLE) */
 uint64_t hostemu_jens_windows(const void* spec_blob, double bin_s) {
   return dcsim_jens_windows(((const dcsim_spec_t*)spec_blob)->end_time, bin_s);
 }
@@ -211,7 +211,7 @@ long long hostemu_run_batch(const void* spec_lists, const void* spec_run, size_t
     dcsim_make_layout(&P->spec, &P->L, dcsim_job_fields(o->jobs != NULL, P->jwait, P->tail, P->jres));
     if (o->layout) { o->layout[0] = P->L.total_bytes; o->layout[1] = (P->L.xring_mask + 1) / 2; o->layout[2] = P->L.cap_run;
                      o->layout[3] = P->L.cap_q[0]; o->layout[4] = P->L.cap_q[1]; o->layout[5] = P->L.rec_off; }
-    if (P->tail) memset(P->tail, 0xff, 2 * ne * sizeof(double)); /* NaN: not finished (dcsim_enable_tail_latency) */
+    if (P->tail) memset(P->tail, 0xff, 2 * ne * sizeof(double)); /* NaN: not finished (as dcsim_recorder_enable fills it) */
     P->state = (char*)calloc(n_replicas, (size_t)P->L.total_bytes);
     P->queues = (char*)calloc(n_replicas, (size_t)P->L.queue_bytes + 16);
     char* work = (char*)malloc((size_t)P->L.total_bytes);

@@ -1,7 +1,7 @@
 /*
  * TEST-ONLY.  The energy cost on the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c), for
  * tests/test_energy_cost*.py: oraclecost_run steps the oracle one event at a time, records the power every energy accrual
- * of every DC is about to integrate, and applies the definition of include/dcsim_b200.h (dcsim_enable_energy_cost) to
+ * of every DC is about to integrate, and applies the definition of include/dcsim_b200.h (DCSIM_STAT_ENERGY_COST) to
  * those intervals.  tests/golden/make_golden_cost.py does the same from the reference; this is its C twin, so a random
  * scenario has a bit-exact reference too.  Nothing here is part of, linked into, or reachable from the product library.
  */

@@ -2,12 +2,12 @@
  * TEST-ONLY.  Occupancy checkers on the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c),
  * for tests/test_occupancy.py:
  *   - oracleocc_occupancy steps the oracle one event at a time and applies the definition of include/dcsim_b200.h
- *     (dcsim_enable_occupancy) to each DC's queue lengths, running count and busy GPUs as they stand before each step;
+ *     (DCSIM_STAT_OCCUPANCY) to each DC's queue lengths, running count and busy GPUs as they stand before each step;
  *   - oracleocc_reached lists every job that reached its DC, with its xfer_done, start and finish instants (Little's law).
  * Nothing here is part of, linked into, or reachable from the product library.
  */
 
-/* One function's open level (include/dcsim_b200.h, dcsim_enable_occupancy): start (-1: none yet) and value. */
+/* One function's open level (include/dcsim_b200.h, DCSIM_STAT_OCCUPANCY): start (-1: none yet) and value. */
 typedef struct { double s, v; } occ_level_t;
 
 /* DC d's function `fn` (0 Qi, 1 Qt, 2 N, 3 Q, 4 B) closes level [s, e] at value v into `row`, laid out as the library's

@@ -1,7 +1,7 @@
 /*
  * TEST-ONLY.  The power profile on the C oracle (oracle/dcsim_oracle.c, compiled unchanged into oracle_probes.c), for
  * tests/test_recorder_corpus*.py: oraclepower_profile steps the oracle one event at a time, records the power every
- * energy accrual is about to integrate, and applies the definition of include/dcsim_b200.h (dcsim_enable_power_profile)
+ * energy accrual is about to integrate, and applies the definition of include/dcsim_b200.h (DCSIM_STAT_POWER_PROFILE)
  * to those intervals.  tests/golden/make_golden_power.py does the same from the reference; this is its C twin, so a
  * random scenario has a bit-exact reference too.  Nothing here is part of, linked into, or reachable from the product
  * library.

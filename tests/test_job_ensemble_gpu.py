@@ -135,6 +135,28 @@ def test_enable_errors_and_windows():
         assert e.value.code == N.E_NOMEM and "bytes" in str(e.value)
 
 
+def test_failed_retarget_leaves_the_ensemble_off():
+    """A re-target that does not fit frees the old ensemble (and the waits recorder in its windows) before it fails: the
+    engine then reports the ensemble off, and the engine cache keys it so, instead of the old windows."""
+    from distributed_cluster_gpus_b200 import _native as N
+    from distributed_cluster_gpus_b200.engine import _engine_recorders
+    sp = SC.to_spec(dict(SC.CFG3, duration=60.0))
+    with _engine(sp, 8, 5) as eng:
+        eng.enable_job_ensemble()
+        eng.enable_job_waits()
+        assert eng.job_ensemble_windows == 12 and eng.job_waits_enabled
+        with pytest.raises(N.DcsimError) as e:
+            eng.enable_job_ensemble(1e-12)                # 2^32 - 1 windows: refused before any allocation
+        assert e.value.code == N.E_NOMEM
+        assert eng.job_ensemble_windows == 0 and eng.job_ensemble_bin is None and not eng.job_waits_enabled
+        kw = _engine_recorders(eng)
+        assert not kw["job_ensemble"] and kw["job_ensemble_bin"] is None and not kw["job_waits"]
+        with pytest.raises(RuntimeError, match="job ensemble not enabled"):
+            eng.job_ensemble_rows()
+        eng.enable_job_ensemble()                         # the handle stays usable
+        assert eng.job_ensemble_windows == 12 and eng.job_ensemble_bin == sp.log_interval
+
+
 def test_bench_size_sample_matches_oracle():
     sp = SC.to_spec(SC.BY_NAME["cfg3_4x64_sinusoid_120s"])
     n = 65536

@@ -90,14 +90,15 @@ def test_columns_match_the_recorder_layouts(case, name, duration, log_interval, 
         sp.n_dc * 2 * (min(max_gpus, 32) * EN.RES_MAX_FREQ + 1 + EN.RES_EBINS)
 
 
-def test_a_recorder_that_is_off():
+def test_a_recorder_that_is_off_names_the_enable_call():
     """A cluster ensemble that is off has no columns: an empty result without a library call.  A job ensemble that is
-    off has its W = 0 columns, and its moments pass fails with the library's message."""
+    off has its W = 0 columns, and its moments pass fails with the library's message, which names the call that
+    enables it (dcsim_recorder_enable)."""
     from distributed_cluster_gpus_b200.engine import BatchedEngine
     with BatchedEngine(_spec("underloaded_1x64", 10.0, 8), 4, base_seed=3) as eng:
         eng.advance(0)
         assert EN.cluster_ensemble(eng).n.size == 0
-        with pytest.raises(N.DcsimError, match=r"job ensemble not enabled \(dcsim_enable_job_ensemble\)") as ei:
+        with pytest.raises(N.DcsimError, match=r"job ensemble not enabled \(dcsim_recorder_enable\)") as ei:
             EN.job_ensemble(eng)
         assert ei.value.code == N.E_STATE
 
